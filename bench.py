@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""bench.py — Mray/s of the B200 path-tracing hot path on BASELINE.json's configs[1]
+"""bench.py — Mray/s of the H100 path-tracing hot path on BASELINE.json's configs[1]
 (hexagon_room.json, 1920x1080, 256 spp, quaternary_sah BVH), at 1/2/4/8 GPUs.
 
 A "step" is one complete render of the frame: ray generation, wavefront loop (extend / shade /
@@ -16,6 +16,9 @@ shadow / regenerate) until every path has terminated, film resolve. Rays = close
              this run measured in a non-timed ncu epilogue over the same kernels: DRAM bytes (traffic,
              dram_gbs) and FP64 thread-instructions against the FP64 issue rate measured in the run.
   secondary  the same measurements on BASELINE config 3's scene (spaceship, 457 k triangles) at 64 spp.
+  --dump-outputs DIR
+             after the timed steps, DIR/frame.npy: the float32 frame (H x W x 3) the last timed step rendered.
+             Scene, camera and sampler seed are fixed, so two builds can be compared output for output.
   cpu_baseline / --impl reference
              the UNMODIFIED reference (oracle/_ref, best of {hw, hw/2, ...} host threads) on a bounded
              sample of the same workload: the SAME full frame at a REDUCED sample count (1 spp on the
@@ -71,7 +74,7 @@ def measured_peaks():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 class ClockSampler:
@@ -347,6 +350,9 @@ def measure(env, args, workload, steps, warmup, sqrtspp_override=0, profile=True
     sync_all()
     wall = time.perf_counter() - wall0
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "frame.npy"), frames.tensor().cpu().numpy().astype(np.float32))
 
     # ---- e2e: host buffers in, host buffers out. N=1: the plain C-ABI call mcrt_scene_upload + mcrt_render_rows
     # (float64 frame to the host). N>1: scene upload + sharded render + rank 0 reads the assembled float3 frame.
@@ -435,7 +441,7 @@ def measure(env, args, workload, steps, warmup, sqrtspp_override=0, profile=True
         "scene_bytes": scene_bytes,
         "note": ("the scene (%d bytes) is served from L1/L2, so `frac` counts cache hits as HBM bytes: it measures box/primitive-test throughput, "
                  "may exceed 1 and is not the binding roofline; dram_gbs is what crosses HBM, fp64 is the issue-rate bound" % scene_bytes)
-                if scene_bytes < 126e6 else "scene larger than L2",
+                if scene_bytes < 50e6 else "scene larger than L2",
     }
     if pe and ext_ms > 0:
         roofline["dram_frac"] = roofline["dram_gbs"] / peak
@@ -456,7 +462,7 @@ def measure(env, args, workload, steps, warmup, sqrtspp_override=0, profile=True
                    "paths_per_step": W * H * cam.sqrtspp ** 2, "rays_per_step": rays_total / steps,
                    "parallelism": (f"rows interleaved over {world} GPUs, scene replicated; each rank's film resolve stores its rows into every rank's "
                                    f"float3 frame over NVLink (CUDA IPC peer memory), one barrier per step") if world > 1 else "1 GPU",
-                   "l2": "per-step working set (32 Mi-path pool, 19 GB of queues) exceeds the 126 MB L2; see roofline.note for the scene arrays",
+                   "l2": "per-step working set (32 Mi-path pool, 19 GB of queues) exceeds the 50 MB L2; see roofline.note for the scene arrays",
                    "mode": "parity (float64 primitive tests and shading in the reference's operation order, --fmad=false)" if args.precision == "f64" else "fast (float32)"},
         "wall_ms_per_step": 1e3 * wall_max / steps,
         "rank_imbalance": {"max_over_mean_gpu_ms": dev_ms_max / max(1e-9, dev_ms_mean)},
@@ -542,6 +548,7 @@ def main():
     ap.add_argument("--no-profile", action="store_true", help="skip the ncu epilogue (measured DRAM traffic / FP64 counts)")
     ap.add_argument("--no-secondary", action="store_true", help="skip the spaceship block")
     ap.add_argument("--no-e2e", action="store_true", help="skip the host-buffer end-to-end leg (long single-purpose runs only)")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR", help="write the frame of the last timed step to DIR/frame.npy")
     ap.add_argument("--child-render", action="store_true", help=argparse.SUPPRESS)
     ap.add_argument("--baseline-seconds", type=float, default=0.0, help="reference arm: target seconds per step")
     args = ap.parse_args()

@@ -1,5 +1,5 @@
 /*
- * mcrt_abi.h — C ABI of the B200-native path-tracing integrator.
+ * mcrt_abi.h — C ABI of the H100-native path-tracing integrator.
  *
  * Drop-in boundary for the ray/BVH/BSDF hot path of linusmossberg/monte-carlo-ray-tracer.
  * The reference has no FFI; the interface this replaces is the C++ virtual

@@ -1,4 +1,4 @@
-"""B200-native path-tracing integrator for the ray/BVH/BSDF hot path of
+"""H100-native path-tracing integrator for the ray/BVH/BSDF hot path of
 linusmossberg/monte-carlo-ray-tracer — Python host mirror over the C ABI (include/mcrt_abi.h).
 
 The names follow the reference's classes for this path:

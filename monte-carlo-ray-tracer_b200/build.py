@@ -1,4 +1,4 @@
-"""Builds libmcrt_b200.so (the C-ABI product library) in-tree with nvcc for sm_100a.
+"""Builds libmcrt_b200.so (the C-ABI product library) in-tree with nvcc for sm_90a (H100).
 
 kernels_f64.cu is compiled with --fmad=false (parity with the reference's non-contracting CPU build);
 everything else with default FMA contraction. -lineinfo keeps ncu's source page usable."""
@@ -12,7 +12,7 @@ CSRC = os.path.join(HERE, "csrc")
 ROOT = os.path.dirname(HERE)
 LIB = os.path.join(HERE, "libmcrt_b200.so")
 
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-I", os.path.join(ROOT, "include"), "-I", CSRC]
 
 UNITS = [

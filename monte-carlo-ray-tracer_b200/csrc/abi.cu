@@ -1,4 +1,4 @@
-// C ABI of the B200 path-tracing integrator (include/mcrt_abi.h): context, scene upload (derives
+// C ABI of the H100 path-tracing integrator (include/mcrt_abi.h): context, scene upload (derives
 // the float64 parity layout and the float32 wide-node layout from the flattened reference scene),
 // the wavefront render loop and the batched sampleRay / Scene::intersect / sampler entry points.
 // There is deliberately no CPU fallback: without a CUDA device every entry point fails.
@@ -55,7 +55,7 @@ namespace
 struct mcrt_ctx
 {
     int device = 0;
-    int sm_count = 148;
+    int sm_count = 132;   // H100 SXM; mcrt_init reads the device's own count
     cudaStream_t stream = nullptr;
     std::string error;
 
@@ -136,7 +136,7 @@ struct mcrt_ctx
     int sort_shade_class = 1;   // k_shade walks paths grouped by the material class of their hit
     int sort_prim_key = -1;   // -1 auto (>= 4096 primitives), 0 origin-cell keys, 1 source-primitive keys
     uint32_t pool_paths = 1u << 23;   // measured on C2: 2 Mi 2269, 4 Mi 2378, 8 Mi 2463, 16 Mi 2503 Mray/s (coarser bins fill better)
-    int blocks_per_sm = 16;   // grid = SMs x this for the grid-stride stage kernels; measured r2 (profiles/r2_knob_sweep.txt): 4 -> 8 -> 16 = 3388 -> 3758 -> 3819 Mray/s on C2
+    int blocks_per_sm = 16;   // grid = SMs x this for the grid-stride stage kernels (more CTAs than fit at once keep every SM busy to the end of a stage)
     double ray_eps_scale = 1e-5;
     int poll_interval = 4;
     int stage_timing = 0;
@@ -368,8 +368,8 @@ namespace
         struct Item { int64_t node; std::vector<Item> group; double box[6]; uint32_t first, count; };   // node >= 0: reference node; -1: run of items; -2: part of a reference leaf
         // leaves larger than max_leaf are cut into runs of consecutive primitives with their own boxes (lanes of a
         // warp then spend similar time per leaf, and the tighter boxes cull more)
-        // measured on the B200 (profiles/r2_leaf_split.txt): cutting leaves to 2 primitives gains 5 % on the 44-primitive
-        // hexagon room (the reference's leaves hold up to 8 there), costs 2-10 % on the 457 k-triangle spaceship
+        // auto: cut leaves to 2 primitives on tiny scenes (the reference's leaves hold up to 8 in the 44-primitive hexagon
+        // room), keep the reference's leaves on big ones, where the extra nodes cost more than the tighter boxes save
         const uint32_t max_leaf = max_leaf_option == 0xFFFFFFFFu ? (s.n_prims < 4096u ? 2u : 0u) : max_leaf_option;
         auto primBox = [&](uint32_t prim, double* b)
         {

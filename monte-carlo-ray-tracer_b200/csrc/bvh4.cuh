@@ -36,9 +36,8 @@
 #define MCRT_SPECULATIVE 0
 #endif
 #ifndef MCRT_FAST_SMEM_STACK          // entries of the search stack kept in shared memory (per thread); the rest is local memory.
-#define MCRT_FAST_SMEM_STACK 0       // Measured on the B200 (profiles/r2_stream_stack_ab.txt): 12 entries in shared memory are 4-5 % SLOWER than
-#endif                               // the all-local stack on the hexagon room, the spaceship and the bulldozer alike (the L1 keeps the hot top of the
-                                     // local stacks, and the shared-memory form adds address arithmetic and a branch per push / pop). Kept as a knob.
+#define MCRT_FAST_SMEM_STACK 0       // 0: the all-local stack (the L1 keeps the hot top of the local stacks, and the shared-memory form adds
+#endif                               // address arithmetic and a branch per push / pop). Kept as a knob.
 
 namespace mcrt
 {
@@ -367,7 +366,7 @@ namespace mcrt
     }
 
     // Many rays per warp with dynamic fetch. Rays of one warp need very different numbers of steps (on
-    // the spaceship the plain one-ray-per-lane loop runs at 9 of 32 lanes: profiles/r2_ncu_v3_first.md),
+    // big scenes the plain one-ray-per-lane loop leaves most lanes of a warp idle),
     // so a lane whose ray is finished does not wait for the warp's longest ray: when fewer than
     // MCRT_FETCH_THRESHOLD lanes are still searching, the warp takes the next rays of the (sorted) queue
     // for its idle lanes from a global counter. load(ii, ray) -> item id, done(item, ray, hit).

@@ -26,8 +26,8 @@
 #include "film.cuh"
 
 // launch-bound knobs (overridable at build time for tuning experiments)
-// (measured on B200, r1: float traversal gains 25-30 % from 64 registers / 32 warps per SM, double
-// traversal loses to the spills; shade gains a little from 3 CTAs of 128 threads)
+// (float traversal runs at 64 registers / 32 warps per SM; double traversal keeps 128 registers, since it
+// would spill at 64; shade runs 3 CTAs of 128 threads)
 #ifndef MCRT_TRACE_MINBLOCKS_F64
 #define MCRT_TRACE_MINBLOCKS_F64 2
 #endif
@@ -44,7 +44,7 @@
 #define MCRT_TRACE_MINBLOCKS_DYN 4
 #endif
 #ifndef MCRT_KNN_MINBLOCKS                 // CTAs of 4 query warps per SM for k_knn
-#define MCRT_KNN_MINBLOCKS 8   // measured on water_caustics (B200): 4 -> 71, 6 -> 85, 8 -> 90 Mquery/s in-kernel (64 registers, spills and all)
+#define MCRT_KNN_MINBLOCKS 8   // 64 registers: the dependent warp collectives of a query need many warps to hide behind
 #endif
 #ifndef MCRT_SHADE_MINBLOCKS
 #define MCRT_SHADE_MINBLOCKS 3

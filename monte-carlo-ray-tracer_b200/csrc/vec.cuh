@@ -25,8 +25,8 @@ namespace mcrt
         MCRT_HD R operator[](int i) const { return i == 0 ? x : (i == 1 ? y : z); }
     };
 
-    // 4 * sizeof(R) alignment: a float64 record is one 256-bit global access on sm_100 (LDG.E.256 / STG.E.256)
-    // instead of two 128-bit ones - the path state, hit and shadow records are all V4<double>
+    // 4 * sizeof(R) alignment: a record never straddles a 32-byte sector, so a float64 record is two 128-bit
+    // accesses to one sector - the path state, hit and shadow records are all V4<double>
     template <class R> struct alignas(4 * sizeof(R)) V4
     {
         R x, y, z, w;
@@ -37,24 +37,25 @@ namespace mcrt
     };
 
     // Streaming access to the wavefront queues (path state, hits, shadow records: written once, read once per
-    // bounce, 6.5 GB per pool): L2 evict-first, so that the 126 MB L2 keeps the scene arrays every ray reads
-    // (BVH nodes, float64 triangle records) instead of queue records nobody will touch again.
+    // bounce, 6.5 GB per pool): the cache-streaming forms (ld.global.cs / st.global.cs = evict-first), so that
+    // the 50 MB L2 keeps the scene arrays every ray reads (BVH nodes, float64 triangle records) instead of
+    // queue records nobody will touch again. sm_90 has no 256-bit global access: a float64 record is two
+    // 128-bit ones.
 #if defined(__CUDACC__) && defined(MCRT_NO_STREAM)   // A/B switch: plain accesses
     template <class T> MCRT_D T ldStream(const T* p) { return *p; }
     template <class T> MCRT_D void stStream(T* p, const T& v) { *p = v; }
 #elif defined(__CUDACC__)
     MCRT_D V4<double> ldStream(const V4<double>* p)
     {
-        V4<double> v;
-        asm volatile("ld.global.L2::evict_first.v4.f64 {%0,%1,%2,%3}, [%4];" : "=d"(v.x), "=d"(v.y), "=d"(v.z), "=d"(v.w) : "l"(p));
-        return v;
+        const double2 a = __ldcs(reinterpret_cast<const double2*>(p));
+        const double2 b = __ldcs(reinterpret_cast<const double2*>(p) + 1);
+        return V4<double>(a.x, a.y, b.x, b.y);
     }
     MCRT_D void stStream(V4<double>* p, const V4<double>& v)
     {
-        asm volatile("st.global.L2::evict_first.v4.f64 [%0], {%1,%2,%3,%4};" :: "l"(p), "d"(v.x), "d"(v.y), "d"(v.z), "d"(v.w) : "memory");
+        __stcs(reinterpret_cast<double2*>(p), make_double2(v.x, v.y));
+        __stcs(reinterpret_cast<double2*>(p) + 1, make_double2(v.z, v.w));
     }
-    // 128-bit records: the cache-streaming forms (ld.global.cs / st.global.cs = evict-first); the L2::evict_first
-    // qualifier exists for the 256-bit instructions only
     MCRT_D V4<float> ldStream(const V4<float>* p)
     {
         const float4 f = __ldcs(reinterpret_cast<const float4*>(p));

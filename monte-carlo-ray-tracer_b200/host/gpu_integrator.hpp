@@ -1,4 +1,4 @@
-// GpuPathTracer / GpuPhotonMapper: the reference-side adapters that put the B200 path behind the
+// GpuPathTracer / GpuPhotonMapper: the reference-side adapters that put the GPU path behind the
 // reference's own Integrator interface (source/integrator/integrator.hpp:7-30).
 //
 //   Camera camera(j, option);                       // unchanged reference code: loads the Scene,

@@ -1,4 +1,4 @@
-// GpuPathTracer / GpuPhotonMapper: the B200 path behind the reference's own Integrator interface
+// GpuPathTracer / GpuPhotonMapper: the GPU path behind the reference's own Integrator interface
 // (source/integrator/integrator.hpp:7-30). They are drop-in replacements for the objects Camera::Camera
 // creates at source/camera/camera.cpp:22-29:
 //

@@ -91,7 +91,7 @@ def test_coincident_geometry_is_flagged(mcrt):
 @pytest.mark.parametrize("cid", ["v3_spaceship", "v5_lego_bulldozer"])
 def test_big_scene_unflagged_answers_equal_reference_order(cid, mcrt):
     """The same claim on the 457 k-triangle spaceship and the 2 M-triangle bulldozer (coincident faces in the model: ~1 % of rays that
-    start on its surfaces are flagged); profiles/r2_fast_search_cpu_check.txt is this check with 2 M rays per scene."""
+    start on its surfaces are flagged)."""
     from conftest import ROOT
     pack = os.path.join(ROOT, "bench_data", cid + ".mcrtpack.xz")
     if not os.path.exists(pack):
@@ -277,7 +277,7 @@ def test_curved_primitives_and_near_degenerate_directions(cid, mcrt):
 def test_every_intersect_call_of_a_render_agrees(cid, mcrt):
     """A whole render by the restated path tracer with EVERY Scene::intersect call - camera, bounce and shadow rays, the rays a renderer
     actually generates - also answered by the restated search: no unflagged answer differs, flags are a handful, and the image is the
-    reference's. profiles/r2_fast_search_render_check.txt: the same on the C2 benchmark rows (18.8 M calls, 5 flagged, 0 mismatches)."""
+    reference's."""
     scene = mcrt.Scene.from_pack(os.path.join(GOLDEN, cid + ".mcrtpack"))
     g = np.load(os.path.join(GOLDEN, cid + ".npz"))
     cam = scene.cameras()[0]

@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Summarise .ncu-rep captures into a small committed text file under profiles/.
+"""Summarise .ncu-rep captures into a small text file.
 usage: ncu_summary.py out.md report1.ncu-rep [report2 ...]"""
 import csv, io, subprocess, sys
 KEYS = ["gpu__time_duration.sum", "launch__grid_size", "launch__block_size", "launch__registers_per_thread",

@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
 """Parallel OBJ loader + vertex normals (mcrt_obj_load, mcrt_obj_vertex_normals) against the reference's
 Scene::parseOBJ / generateVertexNormals on the reference's own OBJ assets: equality and load time.
-Build container only (needs /root/reference). Output: profiles/r2_obj_loader.txt"""
+Needs the reference checkout. Prints one line per asset."""
 import glob
 import importlib
 import os
@@ -18,7 +18,6 @@ mcrt = importlib.import_module("monte-carlo-ray-tracer_b200")
 if __name__ == "__main__":
     s = ref.RefScene("ior_test.json", dict(width=8, height=8, sqrtspp=1))
     files = sorted(glob.glob("/root/reference/scenes/data/**/*.obj", recursive=True), key=os.path.getsize)
-    lines = []
     for f in files[-8:]:
         r = s.parse_obj(f)
         best = None
@@ -39,6 +38,4 @@ if __name__ == "__main__":
                     f"reference {sec * 1e3:.0f} ms, parallel {dt * 1e3:.0f} ms")
         msg += f"; drop-in bodies (host/obj_adapter.hpp) vs the reference's: {'EQUAL' if s.obj_adapter_check(f) == 1 else 'DIFFERENT'}"
         print(msg, flush=True)
-        lines.append(msg)
-    with open(os.path.join(ROOT, "profiles", "r2_obj_loader.txt"), "w") as f:
-        f.write(f"host cores: {os.cpu_count()}\n" + "\n".join(lines) + "\n")
+    print(f"host cores: {os.cpu_count()}")

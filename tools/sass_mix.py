@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """Static SASS opcode mix of the hot kernels, straight from the built library (cuobjdump -sass): which
-instructions the sm_100a code consists of. usage: sass_mix.py [kernel-name-substring ...] > profiles/..."""
+instructions the sm_90a code consists of. usage: sass_mix.py [kernel-name-substring ...]"""
 import collections, os, re, subprocess, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 lib = os.path.join(ROOT, "monte-carlo-ray-tracer_b200", "libmcrt_b200.so")
@@ -21,7 +21,7 @@ for ln in out.splitlines():
         m = re.match(r"\s+/\*[0-9a-f]+\*/\s+(?:@!?U?P\d+\s+)?([A-Z0-9_.]+)", ln)
         if m:
             mix[cur][1][m.group(1).split(".")[0]] += 1
-print("Static SASS opcode mix (instruction counts in the kernel image, not execution counts), sm_100a, cuobjdump -sass of libmcrt_b200.so")
+print("Static SASS opcode mix (instruction counts in the kernel image, not execution counts), sm_90a, cuobjdump -sass of libmcrt_b200.so")
 print("LDG/STG = global memory, LDL/STL = local memory (stacks, spills), DADD/DMUL/DFMA = float64 pipe, FFMA/FMNMX = the float32 box tests,")
 print("REDUX/SHFL/VOTE/MATCH = warp collectives, ATOMG/RED = global atomics (queue appends, film)\n")
 for key, (name, c) in mix.items():
