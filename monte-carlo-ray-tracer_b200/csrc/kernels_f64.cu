@@ -46,7 +46,7 @@ namespace mcrt
         static bool attr_set = false;
         if (!attr_set)
         {
-            const int max_smem = (int)knnSharedBytes(1024);   // k > 768 exceeds the default 48 KB
+            const int max_smem = (int)knnSharedBytes(1024);   // k > 672 exceeds the default 48 KB
             cudaFuncSetAttribute(k_knn_user<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem);
             cudaFuncSetAttribute(k_knn_user<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem);
             cudaFuncSetAttribute(k_knn_user<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem);

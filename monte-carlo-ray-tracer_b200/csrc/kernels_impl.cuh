@@ -63,7 +63,7 @@ namespace mcrt
         }
         const bool lite = (p.scene.material_flags_any & ~SHADE_FEATS_LITE) == 0;
         const int slots = knnSlotsFor(p.pm.k_nearest);
-        // k > 768 needs more than the default 48 KB of dynamic shared memory (knnSharedBytes)
+        // k > 672 needs more than the default 48 KB of dynamic shared memory (knnSharedBytes)
         #define MCRT_KNN_LAUNCH1(SL, FE) \
             do { static bool attr_set = false; \
                  if (!attr_set) { cudaFuncSetAttribute(k_knn<MCRT_REAL, SL, false, FE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)knnSharedBytes(1024)); attr_set = true; } \

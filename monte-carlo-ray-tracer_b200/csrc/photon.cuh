@@ -319,10 +319,10 @@ namespace mcrt
                 {
                     const uint32_t slot = n_frontier + __popc(ballot & ((1u << lane) - 1u));
                     if (slot < (uint32_t)KNN_FRONTIER) { sh.fr_d2[slot] = d2; sh.fr_node[slot] = child; }
-                    else *overflow = 1;
                 }
                 n_frontier += __popc(ballot);
-                if (n_frontier > (uint32_t)KNN_FRONTIER) n_frontier = KNN_FRONTIER;
+                // set in every lane: the callers report lane 0's flag, and the dropped children may be any lanes'
+                if (n_frontier > (uint32_t)KNN_FRONTIER) { *overflow = 1; n_frontier = KNN_FRONTIER; }
                 // tighten with the farthest corner of any accepted child holding >= k photons
                 double m = md2;
                 for (int off = 4; off > 0; off >>= 1) m = fmin(m, __shfl_xor_sync(0xFFFFFFFFu, m, off));
