@@ -46,7 +46,7 @@ namespace
     template <class R> struct WaveBuffers
     {
         PathBuffer<R> buf[2];
-        ShadowQueue<R> shadow;
+        ShadowRecord<R>* shadow = nullptr;
         V4<R>* hits = nullptr;
         uint32_t capacity = 0;
     };
@@ -557,10 +557,7 @@ namespace
             if ((rc = devAlloc(ctx, track, &w.buf[b].meta, n))) return rc;
             if ((rc = devAlloc(ctx, track, &w.buf[b].meta2, n))) return rc;
         }
-        if ((rc = devAlloc(ctx, track, &w.shadow.o, n))) return rc;
-        if ((rc = devAlloc(ctx, track, &w.shadow.d, n))) return rc;
-        if ((rc = devAlloc(ctx, track, &w.shadow.k, n))) return rc;
-        if ((rc = devAlloc(ctx, track, &w.shadow.meta, n))) return rc;
+        if ((rc = devAlloc(ctx, track, &w.shadow, n))) return rc;
         if ((rc = devAlloc(ctx, track, &w.hits, n))) return rc;
         w.capacity = ctx->pool_paths;
         return MCRT_OK;

@@ -93,13 +93,19 @@ namespace mcrt
         uint4* meta2;    // ls.light as light index, ior_count | dirac<<8, film_index, source prim (fast mode)
     };
 
-    template <class R> struct ShadowQueue
+    // One shadow ray. k_shadow reads the queue through the ray-coherence sort, i.e. at random positions,
+    // so the fields it always needs (o, d, meta) share one line instead of being three scattered reads;
+    // k comes last because it is read only when the light is visible. float64: one 128-byte line, with
+    // 16 bytes of padding after meta; float: one 64-byte half-line.
+    template <class R> struct alignas(16 * sizeof(R)) ShadowRecord
     {
-        V4<R>* o;        // start.xyz, bsdf_pdf
-        V4<R>* d;        // direction.xyz, area * cos_light
-        V4<R>* k;        // bsdf_absIdotN * Le * throughput, select_probability
-        uint4* meta;     // light prim, film_index, source prim, -
+        V4<R> o;         // start.xyz, bsdf_pdf
+        V4<R> d;         // direction.xyz, area * cos_light
+        uint4 meta;      // light prim, film_index, source prim, sample
+        V4<R> k;         // bsdf_absIdotN * Le * throughput, select_probability
     };
+    static_assert(sizeof(ShadowRecord<double>) == 128 && sizeof(ShadowRecord<float>) == 64, "one shadow record per line");
+    static_assert(offsetof(ShadowRecord<double>, k) == 96, "the float64 padding is the 16-byte chunk 5 (k_shade writes it)");
 
     // Ray-coherence sort. Incoherent secondary rays run the traversal kernels at ~10 of 32 lanes
     // active (ncu, r1 baseline) while coherent primary rays reach 31; so every queue is re-ordered
@@ -220,7 +226,7 @@ namespace mcrt
         DeviceScene<R> scene;
         DeviceCamera<R> camera;
         PathBuffer<R> buf[2];
-        ShadowQueue<R> shadow;
+        ShadowRecord<R>* shadow;
         V4<R>* hits;           // t,u,v,prim
         Counters* counters;
         double* film;          // [n_film][3]
@@ -877,11 +883,14 @@ namespace mcrt
             }
             if (want_shadow)
             {
-                stStream(&p.shadow.o[sslot], V4<R>(sh_o, sh_bsdf_pdf));
-                stStream(&p.shadow.d[sslot], V4<R>(sh_d, sh_area_cos));
-                stStream(&p.shadow.k[sslot], V4<R>(sh_k, sh_select));
-                stStream(&p.shadow.meta[sslot], make_uint4(sh_light, meta2.z,
-                                                           sc.shade[hit_prim].type == PRIM_TRIANGLE ? hit_prim : NO_PRIM, meta.y));
+                ShadowRecord<R>& srec = p.shadow[sslot];
+                stStream(&srec.o, V4<R>(sh_o, sh_bsdf_pdf));
+                stStream(&srec.d, V4<R>(sh_d, sh_area_cos));
+                stStream(&srec.meta, make_uint4(sh_light, meta2.z, sc.shade[hit_prim].type == PRIM_TRIANGLE ? hit_prim : NO_PRIM, meta.y));
+                // float64: also write the padding after meta, so that no 32-byte sector of the record is left half
+                // written (without this store the C2 shade stage measured 930 instead of 744 ms per frame)
+                if constexpr (sizeof(R) == 8) stStream(reinterpret_cast<uint4*>(&srec) + 5, make_uint4(0u, 0u, 0u, 0u));
+                stStream(&srec.k, V4<R>(sh_k, sh_select));
                 if (sorting) { p.sort.shadow_key[sslot] = skey; p.sort.shadow_rank[sslot] = srank; }
             }
 
@@ -917,19 +926,20 @@ namespace mcrt
                 [&](uint32_t ii, RayQ<R>& r, uint32_t& target)
                 {
                     const uint32_t i = order ? order[ii] : ii;
-                    const V4<R> so = ldStream(&p.shadow.o[i]), sd = ldStream(&p.shadow.d[i]);
+                    const V4<R> so = ldStream(&p.shadow[i].o), sd = ldStream(&p.shadow[i].d);
                     r.o = so.xyz(); r.d = sd.xyz();
                     if constexpr (PRIMS == PRIMS_ALL) r.inv_d = R(1) / r.d;
-                    target = p.shadow.meta[i].x;
+                    target = p.shadow[i].meta.x;
                     return i;
                 },
                 [&](uint32_t i, const RayQ<R>&, const Hit<R>& h)
                 {
                     rays++;
-                    const uint4 sm = p.shadow.meta[i];
+                    const ShadowRecord<R>& srec = p.shadow[i];
+                    const uint4 sm = srec.meta;
                     if (h.prim == sm.x)   // integrator.cpp:70-86: visible iff the closest hit is that very light primitive
                     {
-                        const V4<R> so = p.shadow.o[i], sd = p.shadow.d[i], sk = p.shadow.k[i];
+                        const V4<R> so = srec.o, sd = srec.d, sk = srec.k;
                         R light_pdf = pow2(h.t) / sd.w;
                         R mis_weight = powerHeuristic(light_pdf, so.w);
                         depositRadiance<FILM>(p, sm.y, pixelOfFilmIndex(p, sm.y), sm.w, sk.xyz() * (mis_weight / (light_pdf * sk.w)));
@@ -941,8 +951,9 @@ namespace mcrt
         for (uint32_t ii = blockIdx.x * blockDim.x + threadIdx.x; ii < n; ii += gridDim.x * blockDim.x)
         {
             const uint32_t i = order ? order[ii] : ii;
-            const V4<R> so = ldStream(&p.shadow.o[i]), sd = ldStream(&p.shadow.d[i]);
-            const uint4 sm = ldStream(&p.shadow.meta[i]);
+            const ShadowRecord<R>& srec = p.shadow[i];
+            const V4<R> so = ldStream(&srec.o), sd = ldStream(&srec.d);
+            const uint4 sm = ldStream(&srec.meta);
             Hit<R> h;
             if constexpr (Mode<R>::parity && FAST != 0) h = traceVisible<PRIMS>(p.scene, so.xyz(), sd.xyz(), sm.x, cnt, overflow);
             else h = traceClosest<PRIMS, false>(p.scene, so.xyz(), sd.xyz(), sm.z, cnt, overflow);
@@ -950,7 +961,7 @@ namespace mcrt
             // integrator.cpp:70-86: visible iff the closest hit is that very light primitive
             if (h.prim == sm.x)
             {
-                const V4<R> sk = p.shadow.k[i];
+                const V4<R> sk = srec.k;
                 R light_pdf = pow2(h.t) / sd.w;
                 R mis_weight = powerHeuristic(light_pdf, so.w);
                 depositRadiance<FILM>(p, sm.y, pixelOfFilmIndex(p, sm.y), sm.w, sk.xyz() * (mis_weight / (light_pdf * sk.w)));
