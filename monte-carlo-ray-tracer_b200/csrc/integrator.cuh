@@ -49,8 +49,8 @@
 #ifndef MCRT_SHADE_MINBLOCKS
 #define MCRT_SHADE_MINBLOCKS 3
 #endif
-#ifndef MCRT_SHADE_MINBLOCKS_LITE   // k_shade without the GGX / Oren-Nayar / conductor code needs fewer registers
-#define MCRT_SHADE_MINBLOCKS_LITE 4
+#ifndef MCRT_SHADE_MINBLOCKS_LITE   // k_shade without the GGX / Oren-Nayar / conductor code: 166 registers, so 3 CTAs
+#define MCRT_SHADE_MINBLOCKS_LITE 3  // hold it without spills; on the H100 that beat 4, 5 and 6 CTAs, which spill (DESIGN.md §10)
 #endif
 #ifndef MCRT_SORT_ORIGIN_BITS
 #define MCRT_SORT_ORIGIN_BITS 4
