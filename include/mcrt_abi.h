@@ -366,13 +366,38 @@ int mcrt_render_rows_strided_peers(mcrt_ctx* ctx, const mcrt_camera* camera, uin
                                    mcrt_stats* stats);
 /* Reconstruction filters across row shards (film.cpp:61-79): with a filter set by mcrt_set_film a sample splats
  * into neighbouring rows, so a rank that renders rows y_first + k*y_step accumulates into whole-frame buffers and
- * returns them UNRESOLVED: rgb_sum_dev[height*width][3] and weight_sum_dev[height*width] (device, float64). The
+ * returns them UNRESOLVED: rgb_sum_dev[height*width][3] and weight_sum_dev[height*width] (device, float64; zeroed
+ * first, then accumulated as mcrt_render_accumulate_dev does). The
  * host adds them over the ranks (an all-reduce) and calls mcrt_film_resolve_dev, Film::Splat::get (film.cpp:106-113). */
 int mcrt_render_film_sums_strided_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_t y_first, uint32_t y_step,
                                       uint32_t n_rows, uint32_t sqrtspp, uint32_t global_seed, int integrator_kind,
                                       int precision, double* rgb_sum_dev, double* weight_sum_dev, mcrt_stats* stats);
 int mcrt_film_resolve_dev(mcrt_ctx* ctx, const double* rgb_sum_dev, const double* weight_sum_dev, uint64_t n_pixels,
                           double* out_rgb_dev);
+
+/* Progressive rendering. Sample s of pixel p traces the same path whichever call renders it, so sums over disjoint
+ * sample ranges add up to the one-shot frame's sums (up to the order of the float64 film additions).
+ * mcrt_render_accumulate_dev adds samples [sample_first, sample_first + sample_count) of every pixel of rows
+ * y_first + k*y_step, k < n_rows, into caller-owned device sums (not zeroed, not resolved). Box film:
+ * rgb_sum_dev[n_rows*W][3], weight_sum_dev NULL (the weight is the sample count). Reconstruction filter
+ * (mcrt_set_film): whole-frame rgb_sum_dev[H*W][3] and weight_sum_dev[H*W]; any set of rows may be accumulated.
+ * MCRT_ERR_INVALID: sample_count 0, sample_first + sample_count > 2^32, a weight pointer with the box film or
+ * none with a filter, and every argument mcrt_render_rows_strided_dev refuses. */
+int mcrt_render_accumulate_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_t y_first, uint32_t y_step, uint32_t n_rows,
+                               uint32_t sample_first, uint32_t sample_count, uint32_t global_seed, int integrator_kind,
+                               int precision, double* rgb_sum_dev, double* weight_sum_dev, mcrt_stats* stats);
+/* Resolves two sets of sums A and B (a_samples / b_samples samples per pixel) into out_rgb_dev[rows*width][3] =
+ * max((A+B)/(wA+wB), 0), with w the sample count (box film, weight pointers NULL) or the weight sums (filter; the
+ * pixel is 0 where the weight is 0), and estimates the remaining noise. Per pixel and channel
+ * v = (A/wA - B/wB)^2 * nA*nB/(nA+nB)^2, unbiased for the variance of the combined mean if the halves are independent
+ * (pixels where a half has zero weight contribute no v). tile_error_dev[ceil(rows/tile)][ceil(width/tile)]
+ * (optional) and *frame_error (optional) = sqrt(sum v / sum I^2) over the tile / the frame, I the resolved value;
+ * 0 where sum v is 0, +inf where sum I^2 is 0 < sum v. A half may be empty (samples 0, sums NULL): the frame is
+ * resolved and every error is +inf. MCRT_ERR_INVALID: tile 0, no samples in either half. */
+int mcrt_progressive_resolve_dev(mcrt_ctx* ctx, const double* a_rgb_dev, const double* a_weight_dev, uint64_t a_samples,
+                                 const double* b_rgb_dev, const double* b_weight_dev, uint64_t b_samples,
+                                 uint32_t width, uint32_t rows, uint32_t tile, double* out_rgb_dev,
+                                 double* tile_error_dev, double* frame_error);
 
 /* A device buffer that other processes on the node can map: *dev_ptr (zero-filled) and its 64-byte CUDA IPC
  * handle, to be sent to the peers by whatever channel the host uses (torch.distributed in this repository). */

@@ -36,6 +36,7 @@ ABI_SYMBOLS = [
     "mcrt_render_film_sums_strided_dev", "mcrt_film_resolve_dev",
     "mcrt_bvh4_host", "mcrt_bvh4_host_free",
     "mcrt_fp64_peak", "mcrt_photon_emit_total", "mcrt_photon_emit_range", "mcrt_photon_build_dev",
+    "mcrt_render_accumulate_dev", "mcrt_progressive_resolve_dev",
 ]
 
 
@@ -208,6 +209,10 @@ def lib():
         L.mcrt_render_film_sums_strided_dev.argtypes = [C.c_void_p, C.POINTER(CameraRec), C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
                                                         C.c_uint32, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.POINTER(Stats)]
         L.mcrt_film_resolve_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]
+        L.mcrt_render_accumulate_dev.argtypes = [C.c_void_p, C.POINTER(CameraRec), C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
+                                                 C.c_uint32, C.c_uint32, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.POINTER(Stats)]
+        L.mcrt_progressive_resolve_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64,
+                                                   C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.POINTER(C.c_double)]
         L.mcrt_photon_emit_total.argtypes = [C.c_void_p, C.POINTER(PhotonEmitParams), C.POINTER(C.c_uint64)]
         L.mcrt_photon_emit_range.argtypes = [C.c_void_p, C.POINTER(PhotonEmitParams), C.c_int, C.c_uint64, C.c_uint64, C.POINTER(C.c_void_p),
                                              C.POINTER(C.c_uint64), C.POINTER(C.c_void_p), C.POINTER(C.c_uint64), C.POINTER(Stats)]
@@ -561,6 +566,31 @@ class Integrator:
     def film_resolve_dev(self, rgb_sum_ptr, weight_sum_ptr, n_pixels, out_ptr):
         self._check(lib().mcrt_film_resolve_dev(self.ctx, C.c_void_p(rgb_sum_ptr), C.c_void_p(weight_sum_ptr), n_pixels, C.c_void_p(out_ptr)))
 
+    # -- progressive rendering (see Progressive)
+    def render_accumulate_dev(self, camera, rgb_sum_ptr, weight_sum_ptr, sample_first, sample_count, y_first=0, y_step=1,
+                              n_rows=None, precision=None):
+        """Adds samples [sample_first, sample_first + sample_count) of rows y_first + k*y_step into device sums
+        (mcrt_render_accumulate_dev). weight_sum_ptr: None with the box film, whole-frame weight sums with a filter."""
+        self.set_film(camera)
+        n_rows = len(range(y_first, camera.height, y_step)) if n_rows is None else n_rows
+        st = Stats()
+        self._check(lib().mcrt_render_accumulate_dev(self.ctx, C.byref(camera.rec), y_first, y_step, n_rows, sample_first, sample_count,
+                                                     self.global_seed, self.kind, self.precision if precision is None else precision,
+                                                     C.c_void_p(rgb_sum_ptr), C.c_void_p(weight_sum_ptr) if weight_sum_ptr else None,
+                                                     C.byref(st)))
+        self.last_stats = st.as_dict()
+        return self.last_stats
+
+    def progressive_resolve_dev(self, a_rgb_ptr, a_weight_ptr, a_samples, b_rgb_ptr, b_weight_ptr, b_samples, width, rows, tile,
+                                out_ptr, tile_error_ptr=None):
+        """mcrt_progressive_resolve_dev: resolves A+B into out_ptr, per-tile errors into tile_error_ptr -> frame error."""
+        def p(x):
+            return C.c_void_p(x) if x else None
+        err = C.c_double()
+        self._check(lib().mcrt_progressive_resolve_dev(self.ctx, p(a_rgb_ptr), p(a_weight_ptr), a_samples, p(b_rgb_ptr), p(b_weight_ptr),
+                                                       b_samples, width, rows, tile, p(out_ptr), p(tile_error_ptr), C.byref(err)))
+        return err.value
+
     def frame_alloc(self, nbytes):
         """-> (device pointer, 64-byte CUDA IPC handle) of a zero-filled buffer other ranks can map"""
         ptr = C.c_void_p(); h = (C.c_ubyte * 64)()
@@ -862,6 +892,141 @@ def bvh4_host(scene, max_leaf=0xFFFFFFFF):
         return np.frombuffer(buf, dtype=BVH4_NODE_DTYPE).copy()
     finally:
         lib().mcrt_bvh4_host_free(h)
+
+
+class Progressive:
+    """A frame rendered in sample passes: it can be extended, stopped once it is good enough, checkpointed and resumed.
+
+    Pass k adds the next range of samples of every pixel into sums A (even k) or B (odd k), torch CUDA tensors this
+    object owns. Sample s of pixel p traces the same path whichever pass renders it, so the resolved frame equals the
+    one-shot frame of the same samples up to the order of the float64 film additions. The difference between the two
+    halves estimates the remaining noise (mcrt_progressive_resolve_dev). With the box film the sums cover the rows
+    y_first + k*y_step, k < n_rows; with a reconstruction filter they, the frame and the tiles span the whole frame."""
+
+    _STATS = ("paths", "extension_rays", "shadow_rays")
+
+    def __init__(self, integrator, camera, y_first=0, y_step=1, n_rows=None, tile=16):
+        import torch
+        self.integrator, self.camera = integrator, camera
+        self.y_first, self.y_step = int(y_first), int(y_step)
+        self.n_rows = len(range(self.y_first, camera.height, self.y_step)) if n_rows is None else int(n_rows)
+        self.tile = int(tile)
+        rec = camera.film_rec()
+        self.filtered = rec is not None and not (rec.filter == FILM_FILTERS["box"] and rec.radius in (0.0, 0.5))
+        self.rows = camera.height if self.filtered else self.n_rows   # rows of the sums and of the resolved frame
+        dev = torch.device("cuda", integrator.device)
+        self.rgb = [torch.zeros((self.rows, camera.width, 3), dtype=torch.float64, device=dev) for _ in range(2)]
+        self.wsum = [torch.zeros((self.rows, camera.width), dtype=torch.float64, device=dev) for _ in range(2)] if self.filtered else None
+        torch.cuda.synchronize(dev)   # the library renders on its own stream
+        self.counts = [0, 0]          # samples per pixel in A and B
+        self.passes = 0
+        self.stats = dict.fromkeys(self._STATS, 0)
+        self._resolved = None
+
+    @property
+    def samples(self):
+        return self.counts[0] + self.counts[1]
+
+    def add(self, samples):
+        """Renders samples [self.samples, self.samples + samples) into A (even pass) or B (odd pass)."""
+        half = self.passes % 2
+        st = self.integrator.render_accumulate_dev(self.camera, self.rgb[half].data_ptr(),
+                                                   self.wsum[half].data_ptr() if self.filtered else None, self.samples,
+                                                   int(samples), self.y_first, self.y_step, self.n_rows)
+        self.counts[half] += int(samples)
+        self.passes += 1
+        for k in self._STATS:
+            self.stats[k] += st[k]
+        self._resolved = None
+        return st
+
+    def _resolve(self):
+        import torch
+        if self._resolved is None:
+            t = self.tile
+            out = torch.empty_like(self.rgb[0])
+            tiles = torch.empty((-(-self.rows // t), -(-self.camera.width // t)), dtype=torch.float64, device=out.device)
+            ptrs = []
+            for h in (0, 1):
+                has = self.counts[h] > 0
+                ptrs += [self.rgb[h].data_ptr() if has else None,
+                         self.wsum[h].data_ptr() if has and self.filtered else None, self.counts[h]]
+            err = self.integrator.progressive_resolve_dev(*ptrs, self.camera.width, self.rows, t, out.data_ptr(), tiles.data_ptr())
+            self._resolved = (out.cpu().numpy(), err, tiles.cpu().numpy())
+        return self._resolved
+
+    def frame(self):
+        """The resolved frame, float64 [rows, width, 3]."""
+        return self._resolve()[0]
+
+    def error(self):
+        """-> (frame relative error, per-tile relative errors [tiles_y, tiles_x]); +inf until both halves have samples."""
+        _, err, tiles = self._resolve()
+        return err, tiles
+
+    def render(self, pass_samples, max_samples, target_error=None):
+        """Adds passes of pass_samples samples until max_samples, or until the first pass after which the frame error is
+        at or below target_error. -> the frame."""
+        while self.samples < max_samples:
+            self.add(min(int(pass_samples), max_samples - self.samples))
+            if target_error is not None and self.error()[0] <= target_error:
+                break
+        return self.frame()
+
+    # -- checkpoint / resume
+    def _identity(self):
+        """What a resumed render must match: every input that changes the samples' paths or where they land."""
+        import hashlib
+        ig, cam = self.integrator, self.camera
+        h = hashlib.sha256()
+        for k in Scene._ARRAYS:
+            a = np.ascontiguousarray(ig.scene.a[k])
+            h.update(k.encode() + str(a.dtype).encode() + str(a.shape).encode() + a.tobytes())
+        h.update(np.float64(ig.scene.ior).tobytes())
+        ident = {"seed": np.uint32(ig.global_seed), "precision": np.int32(ig.precision), "integrator": np.int32(ig.kind),
+                 "camera": np.frombuffer(bytes(cam.rec), np.uint8),
+                 "film": np.frombuffer(bytes(cam.film_rec()), np.uint8) if cam.film_rec() is not None else np.zeros(0, np.uint8),
+                 "row_set": np.array([self.y_first, self.y_step, self.n_rows], np.int64),
+                 "scene_digest": np.array(h.hexdigest())}
+        if ig.kind == INTEGRATOR_PHOTON:
+            caustic, glob, k, dv = ig._maps
+            ph = hashlib.sha256(np.array([k, dv], np.int64).tobytes())
+            for m in (caustic, glob):
+                rows = np.ascontiguousarray(np.asarray(m["photons"], np.float32).reshape(-1, 8)).view(np.dtype((np.void, 32))).ravel()
+                ph.update(np.int64(len(rows)).tobytes() + np.sort(rows).tobytes())   # a set: order inside a leaf may differ
+            ident["photon_digest"] = np.array(ph.hexdigest())
+        return ident
+
+    def save(self, path):
+        """Writes an .npz checkpoint: the sums, the sample counts, the pass index and the render's identity."""
+        data = dict(self._identity(), counts=np.array(self.counts, np.int64), passes=np.int64(self.passes), tile=np.int64(self.tile),
+                    rgb_a=self.rgb[0].cpu().numpy(), rgb_b=self.rgb[1].cpu().numpy())
+        if self.filtered:
+            data.update(wsum_a=self.wsum[0].cpu().numpy(), wsum_b=self.wsum[1].cpu().numpy())
+        with open(path, "wb") as f:
+            np.savez(f, **data)
+
+    @classmethod
+    def load(cls, path, integrator, camera):
+        """Resumes a checkpoint written by save() with `integrator` and `camera`. Raises McrtError, and resumes nothing,
+        when the seed, precision, integrator kind, camera, film, scene or photon maps differ from the checkpoint's."""
+        import torch
+        with np.load(path) as z:
+            data = {k: z[k] for k in z.files}
+        y_first, y_step, n_rows = (int(v) for v in data["row_set"])
+        p = cls(integrator, camera, y_first, y_step, n_rows, int(data["tile"]))
+        ident = p._identity()
+        for k, want in ident.items():
+            if k not in data or not np.array_equal(data[k], want):
+                raise McrtError(f"checkpoint {path}: {k} differs from this render's; not resuming")
+        for name, dst in (("rgb_a", p.rgb[0]), ("rgb_b", p.rgb[1])) + ((("wsum_a", p.wsum[0]), ("wsum_b", p.wsum[1])) if p.filtered else ()):
+            if data[name].shape != tuple(dst.shape):
+                raise McrtError(f"checkpoint {path}: {name} has shape {data[name].shape}, expected {tuple(dst.shape)}")
+            dst.copy_(torch.from_numpy(data[name]))
+        torch.cuda.synchronize(p.rgb[0].device)
+        p.counts = [int(c) for c in data["counts"]]
+        p.passes = int(data["passes"])
+        return p
 
 
 def shard_rows(height, rank, world_size):

@@ -67,7 +67,6 @@ struct mcrt_ctx
     uint32_t n_bvh4_nodes = 0;
     uint32_t bvh4_max_leaf = 0xFFFFFFFFu;   // auto; 0: keep the reference's leaves; n: cut larger leaves into runs of n (option / MCRT_BVH4_MAX_LEAF)
     int dynamic_fetch = -1;       // -1 auto (scenes with >= 2048 BVH4 nodes), 0 off, 1 on
-    double* film_raw_rgb = nullptr; double* film_raw_wsum = nullptr;   // != null: the next filtered render leaves its unresolved sums here (mcrt_render_film_sums_strided_dev)
     PeerFrames peer_out{};   // n_frames != 0: the next resolve writes into these frames (mcrt_render_rows_strided_peers)
     int exact_traversal = 0;   // 1: every ray takes the reference-order replay (traverseReferenceOrder)
 
@@ -88,6 +87,8 @@ struct mcrt_ctx
     double* d_film_cache = nullptr;
     double* d_host_out = nullptr;      // staging of mcrt_render_rows (host-buffer entry point)
     size_t host_out_values = 0;
+    double* d_resolve_scratch = nullptr;   // per-tile noise sums of mcrt_progressive_resolve_dev (grow-only)
+    size_t resolve_scratch_values = 0;
     cudaEvent_t ev_start = nullptr, ev_stop = nullptr, ev_poll[2] = { nullptr, nullptr };
 
     // photon maps (PhotonMapper::caustic_map / global_map) + k-NN query queues
@@ -636,12 +637,23 @@ namespace
         st->replayed_rays = c.replayed_rays;
     }
 
-    // The wavefront loop shared by mcrt_render_rows(_dev) and mcrt_sample_rays.
+    // Accumulate mode of runWavefront: the samples are added into the caller's device sums, which are neither
+    // zeroed before the render nor resolved after it (mcrt_render_accumulate_dev, mcrt_render_film_sums_strided_dev).
+    struct FilmSums
+    {
+        double* rgb;    // box film [n_pixels][3] in film_index order; filtered film [height*width][3]
+        double* wsum;   // filtered film [height*width]; null with the box film
+    };
+
+    // The wavefront loop shared by mcrt_render_rows(_dev) and mcrt_sample_rays. Camera work item w is sample
+    // sample_first + w / n_pixels of pixel w % n_pixels. accum == null: the film lives in the context, is zeroed
+    // first and resolved into out_dev at the end.
     template <class R>
     int runWavefront(mcrt_ctx* ctx, const mcrt_camera* cam, uint32_t row_first, uint32_t row_step, uint32_t n_pixels, uint32_t spp,
                      uint64_t total_work, uint32_t global_seed, int integrator, const double* d_user_rays,
                      const uint32_t* d_user_pixel, const uint32_t* d_user_sample, size_t film_pixels,
-                     double film_weight, double* out_dev, mcrt_stats* stats)
+                     double film_weight, double* out_dev, mcrt_stats* stats, uint32_t sample_first = 0,
+                     const FilmSums* accum = nullptr)
     {
         if (!ctx->has_scene) { ctx->error = "no scene uploaded"; return MCRT_ERR_NO_SCENE; }
         if (integrator == MCRT_INTEGRATOR_PHOTON && !ctx->has_photons)
@@ -652,9 +664,9 @@ namespace
         WaveBuffers<R>& wb = waveOf<R>(ctx);
         int rc;
         if ((rc = ensureWave(ctx, wb, waveAllocsOf<R>(ctx)))) return rc;
-        if ((rc = ensureFilm(ctx, film_pixels * 3))) return rc;
+        if (!accum && (rc = ensureFilm(ctx, film_pixels * 3))) return rc;
         const bool filtered = cam && !d_user_rays && !ctx->film_default && integrator != MCRT_INTERNAL_EMIT;
-        if (filtered && ctx->film_wsum_values < film_pixels)
+        if (filtered && !accum && ctx->film_wsum_values < film_pixels)
         {
             if (ctx->d_film_wsum) cudaFree(ctx->d_film_wsum);
             ctx->d_film_wsum = nullptr; ctx->film_wsum_values = 0;
@@ -697,11 +709,13 @@ namespace
         p.hits = wb.hits;
         p.counters = ctx->d_counters;
         p.sobol_bytes = ctx->d_sobol_bytes;
-        p.film = ctx->d_film;
+        double* const film_rgb = accum ? accum->rgb : ctx->d_film;
+        double* const film_wsum = accum ? accum->wsum : ctx->d_film_wsum;
+        p.film = film_rgb;
         p.filmp.is_default_box = filtered ? 0u : 1u;
         if (filtered)
         {
-            p.filmp.rgb = ctx->d_film; p.filmp.wsum = ctx->d_film_wsum;
+            p.filmp.rgb = film_rgb; p.filmp.wsum = film_wsum;
             p.filmp.cache = ctx->film.cache_size ? ctx->d_film_cache : nullptr;
             p.filmp.radius = ctx->film.radius;
             p.filmp.two_inv_radius = 2.0 / ctx->film.radius;
@@ -762,12 +776,22 @@ namespace
         Counters init;
         std::memset(&init, 0, sizeof(init));
         init.total_work = total_work;
+        if (sample_first)
+        {
+            // work item w is sample w / n_pixels of pixel w % n_pixels: starting the work index at sample_first * n_pixels
+            // renders samples sample_first.. without a kernel change (< 2^64: both factors are below 2^32)
+            init.next_work = (uint64_t)sample_first * n_pixels;
+            init.total_work = init.next_work + total_work;
+        }
         if (integrator == MCRT_INTERNAL_EMIT) { init.next_work = ctx->emit_work_first; init.total_work = ctx->emit_work_first + total_work; }
         ctx->h_counters[0] = init;
         CK(cudaEventRecord(ctx->ev_start, s));   // the timed region includes the counter upload and the film / histogram memsets
         CK(cudaMemcpyAsync(ctx->d_counters, &ctx->h_counters[0], sizeof(Counters), cudaMemcpyHostToDevice, s));
-        CK(cudaMemsetAsync(ctx->d_film, 0, film_pixels * 3 * sizeof(double), s));
-        if (filtered) CK(cudaMemsetAsync(ctx->d_film_wsum, 0, film_pixels * sizeof(double), s));
+        if (!accum)
+        {
+            CK(cudaMemsetAsync(ctx->d_film, 0, film_pixels * 3 * sizeof(double), s));
+            if (filtered) CK(cudaMemsetAsync(ctx->d_film_wsum, 0, film_pixels * sizeof(double), s));
+        }
         const bool sorting = ctx->sort_rays != 0;
         if (sorting)
         {
@@ -872,15 +896,9 @@ namespace
             slot = other;
         }
 
-        if (!emitting)
+        if (!emitting && !accum)
         {
-            if (filtered && ctx->film_raw_rgb)
-            {
-                // row-sharded filtered film: the caller sums these over ranks, then mcrt_film_resolve_dev
-                CK(cudaMemcpyAsync(ctx->film_raw_rgb, ctx->d_film, film_pixels * 3 * sizeof(double), cudaMemcpyDeviceToDevice, s));
-                CK(cudaMemcpyAsync(ctx->film_raw_wsum, ctx->d_film_wsum, film_pixels * sizeof(double), cudaMemcpyDeviceToDevice, s));
-            }
-            else if (filtered) launchResolveFilmWeighted(ctx->d_film, ctx->d_film_wsum, out_dev, film_pixels, grid, s);
+            if (filtered) launchResolveFilmWeighted(ctx->d_film, ctx->d_film_wsum, out_dev, film_pixels, grid, s);
             else if (ctx->peer_out.n_frames) launchResolveFilmPeers(ctx->d_film, ctx->peer_out, film_pixels * 3, film_weight, grid, s);
             else launchResolveFilm(ctx->d_film, out_dev, film_pixels * 3, film_weight, grid, s);
             launches += 1;
@@ -933,17 +951,24 @@ namespace
 
     // ---------------------------------------------------------------------------------------
     // Octree<Photon> + LinearOctree::compact on the host (octree.cpp:34-81, linear-octree.cpp:201-244).
+    // Samples [sample_first, sample_first + spp) of every pixel of rows y_first + k*y_step, k < n_rows: resolved into
+    // out_dev, or added into the caller's sums when accum is given.
     int renderDispatch(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_t y_first, uint32_t y_step, uint32_t n_rows,
-                       uint32_t sqrtspp, uint32_t global_seed, int integrator_kind, int precision, double* out_dev,
-                       mcrt_stats* stats)
+                       uint32_t sample_first, uint64_t spp, uint32_t global_seed, int integrator_kind, int precision,
+                       double* out_dev, mcrt_stats* stats, const FilmSums* accum = nullptr)
     {
-        if (!camera || n_rows == 0 || y_step == 0 || sqrtspp == 0 || camera->width == 0 || sqrtspp > 65535u ||
+        if (!camera || n_rows == 0 || y_step == 0 || spp == 0 || camera->width == 0 ||
             (uint64_t)y_first + (uint64_t)(n_rows - 1) * y_step >= camera->height)
         {
-            ctx->error = "mcrt_render_rows: invalid camera / row range / sqrtspp";
+            ctx->error = "mcrt_render_rows: invalid camera / row range / sample count";
             return MCRT_ERR_INVALID;
         }
-        if (!ctx->film_default && !ctx->film_raw_rgb && (y_first != 0 || y_step != 1 || n_rows != camera->height))
+        if ((uint64_t)sample_first + spp > 0x100000000ull)
+        {
+            ctx->error = "sample range beyond 2^32 samples per pixel";
+            return MCRT_ERR_INVALID;
+        }
+        if (!ctx->film_default && !accum && (y_first != 0 || y_step != 1 || n_rows != camera->height))
         {
             ctx->error = "a reconstruction filter other than the default box splats across rows: render the whole frame in one call";
             return MCRT_ERR_UNSUPPORTED;
@@ -951,18 +976,31 @@ namespace
         const uint64_t n_pixels64 = (uint64_t)camera->width * n_rows;
         if (n_pixels64 > 0xFFFFFFFFull) { ctx->error = "row block too large"; return MCRT_ERR_INVALID; }
         const uint32_t n_pixels = (uint32_t)n_pixels64;
-        const uint32_t spp = sqrtspp * sqrtspp;
         const uint64_t total = (uint64_t)n_pixels * spp;
         // a filtered film accumulates at image positions (samples splat across rows): its buffers span the whole frame
         const size_t film_pixels = ctx->film_default ? (size_t)n_pixels : (size_t)camera->width * camera->height;
         if (precision == MCRT_PRECISION_F64)
-            return runWavefront<double>(ctx, camera, y_first, y_step, n_pixels, spp, total, global_seed, integrator_kind,
-                                        nullptr, nullptr, nullptr, film_pixels, (double)spp, out_dev, stats);
+            return runWavefront<double>(ctx, camera, y_first, y_step, n_pixels, (uint32_t)spp, total, global_seed, integrator_kind,
+                                        nullptr, nullptr, nullptr, film_pixels, (double)spp, out_dev, stats, sample_first, accum);
         if (precision == MCRT_PRECISION_F32)
-            return runWavefront<float>(ctx, camera, y_first, y_step, n_pixels, spp, total, global_seed, integrator_kind,
-                                       nullptr, nullptr, nullptr, film_pixels, (double)spp, out_dev, stats);
+            return runWavefront<float>(ctx, camera, y_first, y_step, n_pixels, (uint32_t)spp, total, global_seed, integrator_kind,
+                                       nullptr, nullptr, nullptr, film_pixels, (double)spp, out_dev, stats, sample_first, accum);
         ctx->error = "unknown precision";
         return MCRT_ERR_INVALID;
+    }
+
+    // One-shot frame: sqrtspp² samples per pixel (Camera::sampleImage)
+    int renderFrame(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_t y_first, uint32_t y_step, uint32_t n_rows,
+                    uint32_t sqrtspp, uint32_t global_seed, int integrator_kind, int precision, double* out_dev,
+                    mcrt_stats* stats, const FilmSums* accum = nullptr)
+    {
+        if (sqrtspp == 0 || sqrtspp > 65535u)
+        {
+            ctx->error = "mcrt_render_rows: invalid camera / row range / sqrtspp";
+            return MCRT_ERR_INVALID;
+        }
+        return renderDispatch(ctx, camera, y_first, y_step, n_rows, 0u, (uint64_t)sqrtspp * sqrtspp, global_seed,
+                              integrator_kind, precision, out_dev, stats, accum);
     }
 }
 
@@ -1020,6 +1058,7 @@ void mcrt_destroy(mcrt_ctx* ctx)
     if (ctx->d_film_wsum) cudaFree(ctx->d_film_wsum);
     if (ctx->d_film_cache) cudaFree(ctx->d_film_cache);
     if (ctx->d_host_out) cudaFree(ctx->d_host_out);
+    if (ctx->d_resolve_scratch) cudaFree(ctx->d_resolve_scratch);
     if (ctx->d_counters) cudaFree(ctx->d_counters);
     if (ctx->d_sobol_bytes) cudaFree(ctx->d_sobol_bytes);
     if (ctx->h_counters) cudaFreeHost(ctx->h_counters);
@@ -1467,7 +1506,7 @@ int mcrt_render_rows_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_t y0, 
     if (!out_rgb_dev) { ctx->error = "null output"; return MCRT_ERR_INVALID; }
     CK(cudaSetDevice(ctx->device));
     if (y1 <= y0) { ctx->error = "empty row range"; return MCRT_ERR_INVALID; }
-    return renderDispatch(ctx, camera, y0, 1, y1 - y0, sqrtspp, global_seed, integrator_kind, precision, out_rgb_dev, stats);
+    return renderFrame(ctx, camera, y0, 1, y1 - y0, sqrtspp, global_seed, integrator_kind, precision, out_rgb_dev, stats);
 }
 
 int mcrt_image_tonemap_dev(mcrt_ctx* ctx, const double* rgb_dev, uint32_t width, uint32_t height,
@@ -1563,7 +1602,7 @@ int mcrt_render_rows_strided_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uint3
     if (!ctx) return MCRT_ERR_INVALID;
     if (!out_rgb_dev) { ctx->error = "null output"; return MCRT_ERR_INVALID; }
     CK(cudaSetDevice(ctx->device));
-    return renderDispatch(ctx, camera, y_first, y_step, n_rows, sqrtspp, global_seed, integrator_kind, precision, out_rgb_dev, stats);
+    return renderFrame(ctx, camera, y_first, y_step, n_rows, sqrtspp, global_seed, integrator_kind, precision, out_rgb_dev, stats);
 }
 
 int mcrt_render_rows_strided_peers(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_t y_first, uint32_t y_step,
@@ -1579,7 +1618,7 @@ int mcrt_render_rows_strided_peers(mcrt_ctx* ctx, const mcrt_camera* camera, uin
     pf.n_frames = n_frames; pf.as_float = frame_is_float32 ? 1u : 0u;
     pf.y_first = y_first; pf.y_step = y_step; pf.row_values = camera->width * 3u;
     ctx->peer_out = pf;
-    const int rc = renderDispatch(ctx, camera, y_first, y_step, n_rows, sqrtspp, global_seed, integrator_kind, precision,
+    const int rc = renderFrame(ctx, camera, y_first, y_step, n_rows, sqrtspp, global_seed, integrator_kind, precision,
                                   static_cast<double*>(frames[0]), stats);
     ctx->peer_out.n_frames = 0;
     return rc;
@@ -1593,10 +1632,84 @@ int mcrt_render_film_sums_strided_dev(mcrt_ctx* ctx, const mcrt_camera* camera, 
     if (!rgb_sum_dev || !weight_sum_dev) { ctx->error = "null output"; return MCRT_ERR_INVALID; }
     if (ctx->film_default) { ctx->error = "mcrt_render_film_sums_strided_dev is for reconstruction filters (mcrt_set_film); the default box film shards by rows directly"; return MCRT_ERR_INVALID; }
     CK(cudaSetDevice(ctx->device));
-    ctx->film_raw_rgb = rgb_sum_dev; ctx->film_raw_wsum = weight_sum_dev;
-    const int rc = renderDispatch(ctx, camera, y_first, y_step, n_rows, sqrtspp, global_seed, integrator_kind, precision, rgb_sum_dev, stats);
-    ctx->film_raw_rgb = nullptr; ctx->film_raw_wsum = nullptr;
-    return rc;
+    if (!camera) { ctx->error = "null camera"; return MCRT_ERR_INVALID; }
+    const size_t film_pixels = (size_t)camera->width * camera->height;
+    CK(cudaMemsetAsync(rgb_sum_dev, 0, film_pixels * 3 * sizeof(double), ctx->stream));
+    CK(cudaMemsetAsync(weight_sum_dev, 0, film_pixels * sizeof(double), ctx->stream));
+    const FilmSums sums = { rgb_sum_dev, weight_sum_dev };
+    return renderFrame(ctx, camera, y_first, y_step, n_rows, sqrtspp, global_seed, integrator_kind, precision, nullptr, stats, &sums);
+}
+
+int mcrt_render_accumulate_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_t y_first, uint32_t y_step, uint32_t n_rows,
+                               uint32_t sample_first, uint32_t sample_count, uint32_t global_seed, int integrator_kind,
+                               int precision, double* rgb_sum_dev, double* weight_sum_dev, mcrt_stats* stats)
+{
+    if (!ctx) return MCRT_ERR_INVALID;
+    if (!rgb_sum_dev) { ctx->error = "mcrt_render_accumulate_dev: null rgb sums"; return MCRT_ERR_INVALID; }
+    if (sample_count == 0) { ctx->error = "mcrt_render_accumulate_dev: sample_count is 0"; return MCRT_ERR_INVALID; }
+    if (ctx->film_default && weight_sum_dev)
+    {
+        ctx->error = "mcrt_render_accumulate_dev: the box film is weighted by the sample count; weight_sum_dev must be NULL";
+        return MCRT_ERR_INVALID;
+    }
+    if (!ctx->film_default && !weight_sum_dev)
+    {
+        ctx->error = "mcrt_render_accumulate_dev: a reconstruction filter needs weight_sum_dev";
+        return MCRT_ERR_INVALID;
+    }
+    CK(cudaSetDevice(ctx->device));
+    const FilmSums sums = { rgb_sum_dev, weight_sum_dev };
+    return renderDispatch(ctx, camera, y_first, y_step, n_rows, sample_first, sample_count, global_seed, integrator_kind,
+                          precision, nullptr, stats, &sums);
+}
+
+int mcrt_progressive_resolve_dev(mcrt_ctx* ctx, const double* a_rgb_dev, const double* a_weight_dev, uint64_t a_samples,
+                                 const double* b_rgb_dev, const double* b_weight_dev, uint64_t b_samples,
+                                 uint32_t width, uint32_t rows, uint32_t tile, double* out_rgb_dev,
+                                 double* tile_error_dev, double* frame_error)
+{
+    if (!ctx) return MCRT_ERR_INVALID;
+    if (!out_rgb_dev || width == 0 || rows == 0 || (uint64_t)width * rows > 0xFFFFFFFFull)
+    {
+        ctx->error = "mcrt_progressive_resolve_dev: null output, empty frame or more than 2^32 pixels";
+        return MCRT_ERR_INVALID;
+    }
+    if (tile == 0) { ctx->error = "mcrt_progressive_resolve_dev: tile is 0"; return MCRT_ERR_INVALID; }
+    if (a_samples + b_samples == 0) { ctx->error = "mcrt_progressive_resolve_dev: no samples to resolve"; return MCRT_ERR_INVALID; }
+    if ((a_samples && !a_rgb_dev) || (b_samples && !b_rgb_dev))
+    {
+        ctx->error = "mcrt_progressive_resolve_dev: null sums for a half with samples";
+        return MCRT_ERR_INVALID;
+    }
+    const bool weighted = a_weight_dev || b_weight_dev;
+    if (weighted && ((a_samples && !a_weight_dev) || (b_samples && !b_weight_dev)))
+    {
+        ctx->error = "mcrt_progressive_resolve_dev: weight sums must be given for both halves or for neither";
+        return MCRT_ERR_INVALID;
+    }
+    CK(cudaSetDevice(ctx->device));
+    const uint64_t tiles_x = (width + tile - 1) / tile, tiles_y = (rows + tile - 1) / tile;
+    const uint64_t n_tiles = tiles_x * tiles_y;
+    // scratch: {sum v, sum I^2} per tile, then the frame's
+    const size_t scratch_values = 2 * (n_tiles + 1);
+    if (ctx->resolve_scratch_values < scratch_values)
+    {
+        if (ctx->d_resolve_scratch) cudaFree(ctx->d_resolve_scratch);
+        ctx->d_resolve_scratch = nullptr; ctx->resolve_scratch_values = 0;
+        CK(cudaMalloc((void**)&ctx->d_resolve_scratch, scratch_values * sizeof(double)));
+        ctx->resolve_scratch_values = scratch_values;
+    }
+    ProgressiveHalf a = { a_samples ? a_rgb_dev : nullptr, a_samples ? a_weight_dev : nullptr, (double)a_samples };
+    ProgressiveHalf b = { b_samples ? b_rgb_dev : nullptr, b_samples ? b_weight_dev : nullptr, (double)b_samples };
+    CK(cudaMemsetAsync(ctx->d_resolve_scratch, 0, scratch_values * sizeof(double), ctx->stream));
+    launchProgressiveResolve(a, b, weighted, width, rows, tile, (uint32_t)tiles_x, out_rgb_dev, ctx->d_resolve_scratch, tile_error_dev,
+                             (uint32_t)n_tiles, ctx->sm_count * ctx->blocks_per_sm, ctx->stream);
+    double frame_sums[2] = { 0.0, 0.0 };
+    CK(cudaMemcpyAsync(frame_sums, ctx->d_resolve_scratch + 2 * n_tiles, sizeof(frame_sums), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    CK(cudaGetLastError());
+    if (frame_error) *frame_error = progressiveRelativeError(frame_sums[0], frame_sums[1], a_samples && b_samples);
+    return MCRT_OK;
 }
 
 int mcrt_film_resolve_dev(mcrt_ctx* ctx, const double* rgb_sum_dev, const double* weight_sum_dev, uint64_t n_pixels, double* out_rgb_dev)
@@ -1708,7 +1821,7 @@ int mcrt_render_rows(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_t y0, uint
         CK(cudaMalloc((void**)&ctx->d_host_out, values * sizeof(double)));
         ctx->host_out_values = values;
     }
-    int rc = renderDispatch(ctx, camera, y0, 1, y1 - y0, sqrtspp, global_seed, integrator_kind, precision, ctx->d_host_out, stats);
+    int rc = renderFrame(ctx, camera, y0, 1, y1 - y0, sqrtspp, global_seed, integrator_kind, precision, ctx->d_host_out, stats);
     if (rc == MCRT_OK)
     {
         cudaError_t e = cudaMemcpyAsync(out_rgb, ctx->d_host_out, values * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream);

@@ -462,6 +462,7 @@ namespace mcrt
             {
                 // sample-major over this rank's pixels: adjacent lanes = adjacent pixels
                 const uint32_t local = (uint32_t)(w % p.n_pixels);
+                // a progressive pass starts at work item sample_first * n_pixels (runWavefront)
                 sample = (uint32_t)(w / p.n_pixels);
                 const uint32_t row = local / p.camera.width, col = local - row * p.camera.width;
                 pixel = (p.row_first + row * p.row_step) * p.camera.width + col;
@@ -1478,6 +1479,23 @@ namespace mcrt
         }
         const double r = ((a0 + a1) + (a2 + a3)) + ((a4 + a5) + (a6 + a7));
         if (r == 12345.678) sink[0] = r;   // never true: keeps the chains alive
+    }
+
+    // One half of a progressive render (mcrt_progressive_resolve_dev): unresolved sums over a set of sample passes.
+    struct ProgressiveHalf
+    {
+        const double* rgb;    // [pixels][3]; null when the half has no samples
+        const double* wsum;   // [pixels] weight sums of a reconstruction filter; null with the box film
+        double samples;       // samples per pixel in this half (the box film's weight)
+    };
+
+    // Relative error sqrt(sum v / sum I^2) of a region. +inf while one half has no samples; 0 where the halves agree
+    // exactly (a region that is black in both halves included).
+    MCRT_HD double progressiveRelativeError(double sum_v, double sum_i2, bool both_halves)
+    {
+        if (!both_halves) return HUGE_VAL;
+        if (sum_v == 0.0) return 0.0;
+        return sum_i2 > 0.0 ? sqrt(sum_v / sum_i2) : HUGE_VAL;
     }
 
     static __global__ void k_resolve_film(const double* film, double* out, size_t n_values, double weight)

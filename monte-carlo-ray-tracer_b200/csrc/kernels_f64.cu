@@ -33,6 +33,96 @@ namespace mcrt
         k_resolve_film_peers<<<grid, 256, 0, s>>>(film, pf, n_values, weight);
     }
 
+    // Progressive resolve: frame = max((A+B) / (wA+wB), 0) as Film::Splat::get (film.cpp:106-113), and per pixel and
+    // channel v = (I_A - I_B)^2 nA nB / (nA+nB)^2 with I_A = A/wA, I_B = B/wB: for independent halves an unbiased
+    // estimate of the variance of the combined mean. v and I^2 are summed per tile x tile block of the buffer's
+    // rows x width (one atomic per warp and tile) and over the frame (one atomic per warp).
+    static __global__ void __launch_bounds__(256) k_progressive_resolve(ProgressiveHalf a, ProgressiveHalf b, uint32_t weighted,
+                                                                        uint32_t width, uint32_t rows, uint32_t tile,
+                                                                        uint32_t tiles_x, uint32_t n_tiles, double* out, double* sums)
+    {
+        const uint64_t n = (uint64_t)width * rows;
+        const bool both = a.samples > 0.0 && b.samples > 0.0;
+        const double scale = both ? a.samples * b.samples / ((a.samples + b.samples) * (a.samples + b.samples)) : 0.0;
+        const unsigned lane = threadIdx.x & 31u;
+        // stride and bound are multiples of 32: the lanes of a warp leave the loop together
+        const uint64_t n_rounded = (n + 31u) & ~31ull;
+        for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n_rounded; i += (uint64_t)gridDim.x * blockDim.x)
+        {
+            double v = 0.0, i2 = 0.0;
+            uint32_t key = 0xFFFFFFFFu;
+            if (i < n)
+            {
+                const double wa = !a.rgb ? 0.0 : (weighted ? a.wsum[i] : a.samples);
+                const double wb = !b.rgb ? 0.0 : (weighted ? b.wsum[i] : b.samples);
+                const double w = wa + wb;
+                const bool compare = both && wa != 0.0 && wb != 0.0;
+                for (int c = 0; c < 3; c++)
+                {
+                    const double sa = a.rgb ? a.rgb[3 * i + c] : 0.0, sb = b.rgb ? b.rgb[3 * i + c] : 0.0;
+                    double value = w == 0.0 ? 0.0 : (sa + sb) / w;
+                    value = value < 0.0 ? 0.0 : value;
+                    out[3 * i + c] = value;
+                    i2 += value * value;
+                    if (compare)
+                    {
+                        const double d = sa / wa - sb / wb;
+                        v += d * d * scale;
+                    }
+                }
+                const uint32_t y = (uint32_t)(i / width), x = (uint32_t)(i - (uint64_t)y * width);
+                key = (y / tile) * tiles_x + x / tile;
+            }
+            double fv = v, fi = i2;
+            for (int off = 16; off > 0; off >>= 1)
+            {
+                fv += __shfl_xor_sync(0xFFFFFFFFu, fv, off);
+                fi += __shfl_xor_sync(0xFFFFFFFFu, fi, off);
+            }
+            if (lane == 0)
+            {
+                if (fv != 0.0) atomicAdd(&sums[2 * (size_t)n_tiles], fv);
+                if (fi != 0.0) atomicAdd(&sums[2 * (size_t)n_tiles + 1], fi);
+            }
+            // one group of lanes per tile the warp touches
+            unsigned pending = __ballot_sync(0xFFFFFFFFu, key != 0xFFFFFFFFu);
+            while (pending)
+            {
+                const int leader = __ffs(pending) - 1;
+                const uint32_t k = __shfl_sync(0xFFFFFFFFu, key, leader);
+                const bool mine = key == k;
+                double gv = mine ? v : 0.0, gi = mine ? i2 : 0.0;
+                for (int off = 16; off > 0; off >>= 1)
+                {
+                    gv += __shfl_xor_sync(0xFFFFFFFFu, gv, off);
+                    gi += __shfl_xor_sync(0xFFFFFFFFu, gi, off);
+                }
+                if ((int)lane == leader)
+                {
+                    if (gv != 0.0) atomicAdd(&sums[2 * (size_t)k], gv);
+                    if (gi != 0.0) atomicAdd(&sums[2 * (size_t)k + 1], gi);
+                }
+                pending &= ~__ballot_sync(0xFFFFFFFFu, mine);
+            }
+        }
+    }
+
+    static __global__ void k_progressive_tile_error(const double* sums, uint32_t n_tiles, bool both_halves, double* tile_error)
+    {
+        for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < n_tiles; t += gridDim.x * blockDim.x)
+            tile_error[t] = progressiveRelativeError(sums[2 * (size_t)t], sums[2 * (size_t)t + 1], both_halves);
+    }
+
+    void launchProgressiveResolve(const ProgressiveHalf& a, const ProgressiveHalf& b, bool weighted, uint32_t width, uint32_t rows,
+                                  uint32_t tile, uint32_t tiles_x, double* out, double* sums, double* tile_error, uint32_t n_tiles,
+                                  int grid, cudaStream_t s)
+    {
+        k_progressive_resolve<<<grid, 256, 0, s>>>(a, b, weighted ? 1u : 0u, width, rows, tile, tiles_x, n_tiles, out, sums);
+        if (tile_error)
+            k_progressive_tile_error<<<(n_tiles + 255) / 256 < (uint32_t)grid ? (n_tiles + 255) / 256 : (uint32_t)grid, 256, 0, s>>>(
+                sums, n_tiles, a.samples > 0.0 && b.samples > 0.0, tile_error);
+    }
+
     void launchFp64Peak(double* sink, int iterations, int grid, cudaStream_t s)
     {
         k_fp64_peak<<<grid, 256, 0, s>>>(sink, iterations);
