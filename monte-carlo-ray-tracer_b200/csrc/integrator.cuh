@@ -37,8 +37,8 @@
 #ifndef MCRT_TRACE_MINBLOCKS_F64_PRUNED   // double traversal without quadric code needs ~100 registers instead of 128
 #define MCRT_TRACE_MINBLOCKS_F64_PRUNED 4
 #endif
-#ifndef MCRT_TRACE_MINBLOCKS_FAST          // order-free search (bvh4.cuh)
-#define MCRT_TRACE_MINBLOCKS_FAST 3
+#ifndef MCRT_TRACE_MINBLOCKS_FAST          // order-free search (bvh4.cuh). 2 CTAs of 256: no spills; measured on C2, H100, DESIGN §10.6
+#define MCRT_TRACE_MINBLOCKS_FAST 2
 #endif
 #ifndef MCRT_TRACE_MINBLOCKS_DYN           // order-free search with dynamic fetch (measured on the spaceship: 64 registers beat 80)
 #define MCRT_TRACE_MINBLOCKS_DYN 4
