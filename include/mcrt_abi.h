@@ -399,6 +399,29 @@ int mcrt_progressive_resolve_dev(mcrt_ctx* ctx, const double* a_rgb_dev, const d
                                  uint32_t width, uint32_t rows, uint32_t tile, double* out_rgb_dev,
                                  double* tile_error_dev, double* frame_error);
 
+/* Adaptive sampling. The n_rows x width grid of a row set is cut into tile x tile blocks (the last row and column of
+ * blocks may be smaller); active_tiles (HOST) holds one byte per block, [ceil(n_rows/tile)][ceil(width/tile)],
+ * nonzero = active. mcrt_render_accumulate_tiles_dev adds samples [sample_first, sample_first + sample_count) of
+ * every pixel of the active blocks into caller-owned sums, exactly as mcrt_render_accumulate_dev does for all pixels
+ * (same sums layout; the other pixels' sums are not touched). MCRT_ERR_INVALID: tile 0, a null mask, a mask with no
+ * active block, and every argument mcrt_render_accumulate_dev refuses. MCRT_ERR_UNSUPPORTED: a reconstruction filter
+ * with a row set other than the whole frame (its splats cross blocks, whose resolve spans the whole frame). */
+int mcrt_render_accumulate_tiles_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_t y_first, uint32_t y_step, uint32_t n_rows,
+                                     uint32_t tile, const uint8_t* active_tiles, uint32_t sample_first, uint32_t sample_count,
+                                     uint32_t global_seed, int integrator_kind, int precision, double* rgb_sum_dev,
+                                     double* weight_sum_dev, mcrt_stats* stats);
+/* mcrt_progressive_resolve_dev with per-tile sample counts: tile_samples (HOST) [ceil(rows/tile)][ceil(width/tile)][2]
+ * = {nA, nB} of each tile's pixels; they set a box-film pixel's weights and every pixel's scale nA*nB/(nA+nB)^2.
+ * With a filter, a pixel near a tile border also holds splats of samples of neighbouring tiles, which may have other
+ * counts: its own tile's counts in the scale are then an approximation. A tile with an empty half has error +inf,
+ * and so does the frame if any tile has one. tile_sums_dev (optional, device) receives {sum v, sum I^2} of each tile,
+ * [n_tiles][2]. MCRT_ERR_INVALID: a null tile_samples and every argument mcrt_progressive_resolve_dev refuses (a half
+ * "has samples" when any tile has samples in it). */
+int mcrt_progressive_resolve_tiles_dev(mcrt_ctx* ctx, const double* a_rgb_dev, const double* a_weight_dev,
+                                       const double* b_rgb_dev, const double* b_weight_dev, const uint32_t* tile_samples,
+                                       uint32_t width, uint32_t rows, uint32_t tile, double* out_rgb_dev,
+                                       double* tile_error_dev, double* tile_sums_dev, double* frame_error);
+
 /* A device buffer that other processes on the node can map: *dev_ptr (zero-filled) and its 64-byte CUDA IPC
  * handle, to be sent to the peers by whatever channel the host uses (torch.distributed in this repository). */
 int mcrt_frame_alloc(mcrt_ctx* ctx, uint64_t bytes, void** dev_ptr, unsigned char ipc_handle[64]);

@@ -37,6 +37,7 @@ ABI_SYMBOLS = [
     "mcrt_bvh4_host", "mcrt_bvh4_host_free",
     "mcrt_fp64_peak", "mcrt_photon_emit_total", "mcrt_photon_emit_range", "mcrt_photon_build_dev",
     "mcrt_render_accumulate_dev", "mcrt_progressive_resolve_dev",
+    "mcrt_render_accumulate_tiles_dev", "mcrt_progressive_resolve_tiles_dev",
 ]
 
 
@@ -213,6 +214,12 @@ def lib():
                                                  C.c_uint32, C.c_uint32, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.POINTER(Stats)]
         L.mcrt_progressive_resolve_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64,
                                                    C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.POINTER(C.c_double)]
+        L.mcrt_render_accumulate_tiles_dev.argtypes = [C.c_void_p, C.POINTER(CameraRec), C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
+                                                       C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int, C.c_int, C.c_void_p,
+                                                       C.c_void_p, C.POINTER(Stats)]
+        L.mcrt_progressive_resolve_tiles_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                         C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                         C.POINTER(C.c_double)]
         L.mcrt_photon_emit_total.argtypes = [C.c_void_p, C.POINTER(PhotonEmitParams), C.POINTER(C.c_uint64)]
         L.mcrt_photon_emit_range.argtypes = [C.c_void_p, C.POINTER(PhotonEmitParams), C.c_int, C.c_uint64, C.c_uint64, C.POINTER(C.c_void_p),
                                              C.POINTER(C.c_uint64), C.POINTER(C.c_void_p), C.POINTER(C.c_uint64), C.POINTER(Stats)]
@@ -591,6 +598,40 @@ class Integrator:
                                                        b_samples, width, rows, tile, p(out_ptr), p(tile_error_ptr), C.byref(err)))
         return err.value
 
+    # -- adaptive sampling (see Progressive.render_adaptive)
+    def render_accumulate_tiles_dev(self, camera, rgb_sum_ptr, weight_sum_ptr, sample_first, sample_count, tile, active,
+                                    y_first=0, y_step=1, n_rows=None, precision=None):
+        """mcrt_render_accumulate_tiles_dev: render_accumulate_dev restricted to the pixels of the active tiles.
+        active: bool [ceil(n_rows / tile), ceil(width / tile)] over the row set's n_rows x width grid."""
+        self.set_film(camera)
+        n_rows = len(range(y_first, camera.height, y_step)) if n_rows is None else n_rows
+        mask = np.ascontiguousarray(active, dtype=np.uint8)
+        if mask.shape != tile_grid(n_rows, camera.width, tile):
+            raise McrtError(f"tile mask has shape {mask.shape}, expected {tile_grid(n_rows, camera.width, tile)}")
+        st = Stats()
+        self._check(lib().mcrt_render_accumulate_tiles_dev(self.ctx, C.byref(camera.rec), y_first, y_step, n_rows, tile,
+                                                           mask.ctypes.data_as(C.c_void_p), sample_first, sample_count,
+                                                           self.global_seed, self.kind, self.precision if precision is None else precision,
+                                                           C.c_void_p(rgb_sum_ptr), C.c_void_p(weight_sum_ptr) if weight_sum_ptr else None,
+                                                           C.byref(st)))
+        self.last_stats = st.as_dict()
+        return self.last_stats
+
+    def progressive_resolve_tiles_dev(self, a_rgb_ptr, a_weight_ptr, b_rgb_ptr, b_weight_ptr, tile_samples, width, rows, tile,
+                                      out_ptr, tile_error_ptr=None, tile_sums_ptr=None):
+        """mcrt_progressive_resolve_tiles_dev: progressive_resolve_dev with per-tile counts tile_samples
+        [tiles_y, tiles_x, 2] = {nA, nB}; tile_sums_ptr (optional) receives {sum v, sum I^2} per tile -> frame error."""
+        def p(x):
+            return C.c_void_p(x) if x else None
+        counts = np.ascontiguousarray(tile_samples, dtype=np.uint32)
+        if counts.shape != tile_grid(rows, width, tile) + (2,):
+            raise McrtError(f"tile_samples has shape {counts.shape}, expected {tile_grid(rows, width, tile) + (2,)}")
+        err = C.c_double()
+        self._check(lib().mcrt_progressive_resolve_tiles_dev(self.ctx, p(a_rgb_ptr), p(a_weight_ptr), p(b_rgb_ptr), p(b_weight_ptr),
+                                                             counts.ctypes.data_as(C.c_void_p), width, rows, tile, p(out_ptr),
+                                                             p(tile_error_ptr), p(tile_sums_ptr), C.byref(err)))
+        return err.value
+
     def frame_alloc(self, nbytes):
         """-> (device pointer, 64-byte CUDA IPC handle) of a zero-filled buffer other ranks can map"""
         ptr = C.c_void_p(); h = (C.c_ubyte * 64)()
@@ -894,6 +935,43 @@ def bvh4_host(scene, max_leaf=0xFFFFFFFF):
         lib().mcrt_bvh4_host_free(h)
 
 
+def tile_grid(rows, width, tile):
+    """(tiles_y, tiles_x) of the tile x tile blocks of a rows x width grid; the last row and column of blocks may be
+    smaller than tile x tile."""
+    return -(-int(rows) // int(tile)), -(-int(width) // int(tile))
+
+
+def tile_pixel_counts(rows, width, tile):
+    """Pixels of each tile of a rows x width grid, int64 [tiles_y, tiles_x]."""
+    ty, tx = tile_grid(rows, width, tile)
+    h = np.minimum(tile, rows - np.arange(ty, dtype=np.int64) * tile)
+    w = np.minimum(tile, width - np.arange(tx, dtype=np.int64) * tile)
+    return np.outer(h, w)
+
+
+def add_tile_samples(tile_counts, active, half, samples):
+    """Per-tile sample counts [tiles_y, tiles_x, 2] after a pass of `samples` samples into half `half` (0: A, 1: B)
+    over the active tiles; retired tiles keep theirs."""
+    out = np.array(tile_counts, dtype=np.int64, copy=True)
+    out[np.asarray(active, bool), half] += int(samples)
+    return out
+
+
+def adaptive_retire(active, tile_counts, tile_sums, tile_pixels, target_error, min_samples):
+    """The retirement rule of Progressive.render_adaptive -> bool [tiles_y, tiles_x], the active tiles to retire.
+
+    A tile retires when both its halves have samples, it has at least min_samples samples, and its share of the
+    noise is within its share of the target: sum v_t <= target^2 * sum I^2 (frame) * n_t / N, with n_t and N the
+    pixels of the tile and of the frame and sum I^2 of the frame the total of the tiles'. If every tile meets it,
+    sum over t of sum v_t <= target^2 * sum I^2: the frame meets the target."""
+    counts = np.asarray(tile_counts, np.int64)
+    sums = np.asarray(tile_sums, np.float64)
+    n_t = np.asarray(tile_pixels, np.float64)
+    bound = float(target_error) ** 2 * sums[..., 1].sum() * n_t / n_t.sum()
+    return (np.asarray(active, bool) & (counts[..., 0] > 0) & (counts[..., 1] > 0) & (counts.sum(-1) >= min_samples)
+            & (sums[..., 0] <= bound))
+
+
 class Progressive:
     """A frame rendered in sample passes: it can be extended, stopped once it is good enough, checkpointed and resumed.
 
@@ -901,7 +979,13 @@ class Progressive:
     object owns. Sample s of pixel p traces the same path whichever pass renders it, so the resolved frame equals the
     one-shot frame of the same samples up to the order of the float64 film additions. The difference between the two
     halves estimates the remaining noise (mcrt_progressive_resolve_dev). With the box film the sums cover the rows
-    y_first + k*y_step, k < n_rows; with a reconstruction filter they, the frame and the tiles span the whole frame."""
+    y_first + k*y_step, k < n_rows; with a reconstruction filter they, the frame and the tiles span the whole frame.
+
+    Adaptive sampling (render_adaptive, retire): tiles of tile x tile pixels can be retired, and a retired tile never
+    comes back. Passes then render only the active tiles (mcrt_render_accumulate_tiles_dev), so every active tile has
+    `counts` samples and a retired tile keeps the counts it had (`tile_counts`); the frame is resolved with those
+    per-tile counts (mcrt_progressive_resolve_tiles_dev). While every tile is active, add, frame and error run the
+    uniform entry points. With a reconstruction filter, adaptive passes need the whole frame as the row set."""
 
     _STATS = ("paths", "extension_rays", "shadow_rays")
 
@@ -918,41 +1002,63 @@ class Progressive:
         self.rgb = [torch.zeros((self.rows, camera.width, 3), dtype=torch.float64, device=dev) for _ in range(2)]
         self.wsum = [torch.zeros((self.rows, camera.width), dtype=torch.float64, device=dev) for _ in range(2)] if self.filtered else None
         torch.cuda.synchronize(dev)   # the library renders on its own stream
-        self.counts = [0, 0]          # samples per pixel in A and B
+        self.counts = [0, 0]          # samples per pixel in A and B (of the active tiles)
         self.passes = 0
         self.stats = dict.fromkeys(self._STATS, 0)
         self._resolved = None
+        grid = tile_grid(self.rows, camera.width, self.tile)
+        self.active = np.ones(grid, bool)                          # tiles that still receive samples
+        self.tile_counts = np.zeros(grid + (2,), np.int64)          # samples per pixel of each tile in A and B
+        self.history = []                                           # one record per render_adaptive pass
+        self.stop_reason = None                                     # why the last render_adaptive stopped
 
     @property
     def samples(self):
         return self.counts[0] + self.counts[1]
 
     def add(self, samples):
-        """Renders samples [self.samples, self.samples + samples) into A (even pass) or B (odd pass)."""
+        """Renders samples [self.samples, self.samples + samples) of the active tiles into A (even pass) or B (odd pass)."""
         half = self.passes % 2
-        st = self.integrator.render_accumulate_dev(self.camera, self.rgb[half].data_ptr(),
-                                                   self.wsum[half].data_ptr() if self.filtered else None, self.samples,
-                                                   int(samples), self.y_first, self.y_step, self.n_rows)
+        wsum = self.wsum[half].data_ptr() if self.filtered else None
+        if self.active.all():
+            st = self.integrator.render_accumulate_dev(self.camera, self.rgb[half].data_ptr(), wsum, self.samples,
+                                                       int(samples), self.y_first, self.y_step, self.n_rows)
+        else:
+            st = self.integrator.render_accumulate_tiles_dev(self.camera, self.rgb[half].data_ptr(), wsum, self.samples, int(samples),
+                                                             self.tile, self.active, self.y_first, self.y_step, self.n_rows)
         self.counts[half] += int(samples)
+        self.tile_counts = add_tile_samples(self.tile_counts, self.active, half, samples)
         self.passes += 1
         for k in self._STATS:
             self.stats[k] += st[k]
         self._resolved = None
         return st
 
-    def _resolve(self):
+    def _resolve(self, sums=False):
+        """-> (frame, frame error, tile errors, tile sums {sum v, sum I^2} [tiles_y, tiles_x, 2] or None). sums: resolve
+        through the per-tile entry point, which reports the tile sums, even while every tile is active."""
         import torch
-        if self._resolved is None:
+        if self._resolved is None or (sums and self._resolved[3] is None):
             t = self.tile
             out = torch.empty_like(self.rgb[0])
-            tiles = torch.empty((-(-self.rows // t), -(-self.camera.width // t)), dtype=torch.float64, device=out.device)
-            ptrs = []
-            for h in (0, 1):
-                has = self.counts[h] > 0
-                ptrs += [self.rgb[h].data_ptr() if has else None,
-                         self.wsum[h].data_ptr() if has and self.filtered else None, self.counts[h]]
-            err = self.integrator.progressive_resolve_dev(*ptrs, self.camera.width, self.rows, t, out.data_ptr(), tiles.data_ptr())
-            self._resolved = (out.cpu().numpy(), err, tiles.cpu().numpy())
+            tiles = torch.empty(self.active.shape, dtype=torch.float64, device=out.device)
+            if self.active.all() and not sums:
+                ptrs = []
+                for h in (0, 1):
+                    has = self.counts[h] > 0
+                    ptrs += [self.rgb[h].data_ptr() if has else None,
+                             self.wsum[h].data_ptr() if has and self.filtered else None, self.counts[h]]
+                err = self.integrator.progressive_resolve_dev(*ptrs, self.camera.width, self.rows, t, out.data_ptr(), tiles.data_ptr())
+                self._resolved = (out.cpu().numpy(), err, tiles.cpu().numpy(), None)
+            else:
+                tile_sums = torch.empty(self.active.shape + (2,), dtype=torch.float64, device=out.device)
+                ptrs = []
+                for h in (0, 1):
+                    has = bool(self.tile_counts[..., h].any())
+                    ptrs += [self.rgb[h].data_ptr() if has else None, self.wsum[h].data_ptr() if has and self.filtered else None]
+                err = self.integrator.progressive_resolve_tiles_dev(*ptrs, self.tile_counts, self.camera.width, self.rows, t,
+                                                                    out.data_ptr(), tiles.data_ptr(), tile_sums.data_ptr())
+                self._resolved = (out.cpu().numpy(), err, tiles.cpu().numpy(), tile_sums.cpu().numpy())
         return self._resolved
 
     def frame(self):
@@ -961,8 +1067,12 @@ class Progressive:
 
     def error(self):
         """-> (frame relative error, per-tile relative errors [tiles_y, tiles_x]); +inf until both halves have samples."""
-        _, err, tiles = self._resolve()
+        _, err, tiles, _ = self._resolve()
         return err, tiles
+
+    def tile_sums(self):
+        """-> {sum v, sum I^2} of each tile, float64 [tiles_y, tiles_x, 2] (mcrt_progressive_resolve_tiles_dev)."""
+        return self._resolve(sums=True)[3]
 
     def render(self, pass_samples, max_samples, target_error=None):
         """Adds passes of pass_samples samples until max_samples, or until the first pass after which the frame error is
@@ -971,6 +1081,48 @@ class Progressive:
             self.add(min(int(pass_samples), max_samples - self.samples))
             if target_error is not None and self.error()[0] <= target_error:
                 break
+        return self.frame()
+
+    # -- adaptive sampling
+    def retire(self, mask):
+        """Retires the tiles where mask (bool [tiles_y, tiles_x]) is True: later passes skip them. A retired tile never
+        comes back. The sums are unchanged, so the resolved frame is too."""
+        mask = np.asarray(mask, bool)
+        if mask.shape != self.active.shape:
+            raise McrtError(f"tile mask has shape {mask.shape}, expected {self.active.shape}")
+        self.active &= ~mask
+
+    def render_adaptive(self, pass_samples, max_samples, target_error, min_samples=16):
+        """Adds passes of pass_samples samples to the active tiles. After each pass it stops if the frame error is at
+        or below target_error, as render does; otherwise it retires every active tile that adaptive_retire selects.
+        It stops when no tile is active or the active tiles have max_samples samples. Each pass is recorded in
+        self.history ({first, count, active, error, tile_counts, tile_sums, retired}); self.stop_reason says why it
+        stopped ("target", "no active tile" or "max_samples"). -> the frame.
+
+        Known limits: the criterion compares a tile's absolute noise with the frame's signal, so dark tiles retire
+        early. A tile's estimate from few samples is itself noisy, which is what min_samples guards against. The two
+        Owen-scrambled halves are not independent: with two large passes the estimate has read about 10 % low."""
+        tile_pixels = tile_pixel_counts(self.rows, self.camera.width, self.tile)
+        while True:
+            if not self.active.any():
+                self.stop_reason = "no active tile"
+                break
+            if self.samples >= max_samples:
+                self.stop_reason = "max_samples"
+                break
+            first, count, n_active = self.samples, min(int(pass_samples), max_samples - self.samples), int(self.active.sum())
+            self.add(count)
+            _, err, _, sums = self._resolve(sums=True)
+            entry = {"first": first, "count": count, "active": n_active, "error": err,
+                     "tile_counts": self.tile_counts.copy(), "tile_sums": sums}
+            if err <= target_error:
+                entry["retired"] = np.zeros_like(self.active)
+                self.history.append(entry)
+                self.stop_reason = "target"
+                break
+            entry["retired"] = adaptive_retire(self.active, self.tile_counts, sums, tile_pixels, target_error, min_samples)
+            self.retire(entry["retired"])
+            self.history.append(entry)
         return self.frame()
 
     # -- checkpoint / resume
@@ -987,6 +1139,7 @@ class Progressive:
                  "camera": np.frombuffer(bytes(cam.rec), np.uint8),
                  "film": np.frombuffer(bytes(cam.film_rec()), np.uint8) if cam.film_rec() is not None else np.zeros(0, np.uint8),
                  "row_set": np.array([self.y_first, self.y_step, self.n_rows], np.int64),
+                 "tile": np.int64(self.tile),   # the tile masks' shapes depend on it
                  "scene_digest": np.array(h.hexdigest())}
         if ig.kind == INTEGRATOR_PHOTON:
             caustic, glob, k, dv = ig._maps
@@ -998,8 +1151,10 @@ class Progressive:
         return ident
 
     def save(self, path):
-        """Writes an .npz checkpoint: the sums, the sample counts, the pass index and the render's identity."""
-        data = dict(self._identity(), counts=np.array(self.counts, np.int64), passes=np.int64(self.passes), tile=np.int64(self.tile),
+        """Writes an .npz checkpoint: the sums, the sample counts, the pass index, the active tiles and the per-tile
+        counts, and the render's identity."""
+        data = dict(self._identity(), counts=np.array(self.counts, np.int64), passes=np.int64(self.passes),
+                    active=self.active.copy(), tile_counts=self.tile_counts.copy(),
                     rgb_a=self.rgb[0].cpu().numpy(), rgb_b=self.rgb[1].cpu().numpy())
         if self.filtered:
             data.update(wsum_a=self.wsum[0].cpu().numpy(), wsum_b=self.wsum[1].cpu().numpy())
@@ -1007,14 +1162,15 @@ class Progressive:
             np.savez(f, **data)
 
     @classmethod
-    def load(cls, path, integrator, camera):
-        """Resumes a checkpoint written by save() with `integrator` and `camera`. Raises McrtError, and resumes nothing,
-        when the seed, precision, integrator kind, camera, film, scene or photon maps differ from the checkpoint's."""
+    def load(cls, path, integrator, camera, tile=None):
+        """Resumes a checkpoint written by save() with `integrator` and `camera` (and `tile`, the checkpoint's if None).
+        Raises McrtError, and resumes nothing, when the seed, precision, integrator kind, camera, film, tile, scene or
+        photon maps differ from the checkpoint's. A checkpoint without tile state resumes with every tile active."""
         import torch
         with np.load(path) as z:
             data = {k: z[k] for k in z.files}
         y_first, y_step, n_rows = (int(v) for v in data["row_set"])
-        p = cls(integrator, camera, y_first, y_step, n_rows, int(data["tile"]))
+        p = cls(integrator, camera, y_first, y_step, n_rows, int(data["tile"]) if tile is None else int(tile))
         ident = p._identity()
         for k, want in ident.items():
             if k not in data or not np.array_equal(data[k], want):
@@ -1023,9 +1179,17 @@ class Progressive:
             if data[name].shape != tuple(dst.shape):
                 raise McrtError(f"checkpoint {path}: {name} has shape {data[name].shape}, expected {tuple(dst.shape)}")
             dst.copy_(torch.from_numpy(data[name]))
+        for name, want in (("active", p.active.shape), ("tile_counts", p.tile_counts.shape)):
+            if name in data and data[name].shape != want:
+                raise McrtError(f"checkpoint {path}: {name} has shape {data[name].shape}, expected {want}")
         torch.cuda.synchronize(p.rgb[0].device)
         p.counts = [int(c) for c in data["counts"]]
         p.passes = int(data["passes"])
+        if "active" in data:
+            p.active = data["active"].astype(bool)
+            p.tile_counts = data["tile_counts"].astype(np.int64)
+        else:
+            p.tile_counts[...] = p.counts   # written before adaptive sampling: every tile has the uniform counts
         return p
 
 

@@ -2,6 +2,7 @@
 // the float64 parity layout and the float32 wide-node layout from the flattened reference scene),
 // the wavefront render loop and the batched sampleRay / Scene::intersect / sampler entry points.
 // There is deliberately no CPU fallback: without a CUDA device every entry point fails.
+#include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -89,6 +90,9 @@ struct mcrt_ctx
     size_t host_out_values = 0;
     double* d_resolve_scratch = nullptr;   // per-tile noise sums of mcrt_progressive_resolve_dev (grow-only)
     size_t resolve_scratch_values = 0;
+    uint32_t* d_pixel_list = nullptr;      // pixels of the active tiles of mcrt_render_accumulate_tiles_dev (grow-only)
+    size_t pixel_list_values = 0;
+    std::vector<uint32_t> h_pixel_list;
     cudaEvent_t ev_start = nullptr, ev_stop = nullptr, ev_poll[2] = { nullptr, nullptr };
 
     // photon maps (PhotonMapper::caustic_map / global_map) + k-NN query queues
@@ -646,14 +650,15 @@ namespace
     };
 
     // The wavefront loop shared by mcrt_render_rows(_dev) and mcrt_sample_rays. Camera work item w is sample
-    // sample_first + w / n_pixels of pixel w % n_pixels. accum == null: the film lives in the context, is zeroed
-    // first and resolved into out_dev at the end.
+    // sample_first + w / n_pixels of pixel w % n_pixels, or of pixel d_pixel_list[w % n_pixels] when a list is given
+    // (n_pixels is then its length). accum == null: the film lives in the context, is zeroed first and resolved into
+    // out_dev at the end.
     template <class R>
     int runWavefront(mcrt_ctx* ctx, const mcrt_camera* cam, uint32_t row_first, uint32_t row_step, uint32_t n_pixels, uint32_t spp,
                      uint64_t total_work, uint32_t global_seed, int integrator, const double* d_user_rays,
                      const uint32_t* d_user_pixel, const uint32_t* d_user_sample, size_t film_pixels,
                      double film_weight, double* out_dev, mcrt_stats* stats, uint32_t sample_first = 0,
-                     const FilmSums* accum = nullptr)
+                     const FilmSums* accum = nullptr, const uint32_t* d_pixel_list = nullptr)
     {
         if (!ctx->has_scene) { ctx->error = "no scene uploaded"; return MCRT_ERR_NO_SCENE; }
         if (integrator == MCRT_INTEGRATOR_PHOTON && !ctx->has_photons)
@@ -724,6 +729,7 @@ namespace
             p.filmp.width = cam->width; p.filmp.height = cam->height;
         }
         p.user_rays = d_user_rays; p.user_pixel = d_user_pixel; p.user_sample = d_user_sample;
+        p.pixel_list = d_pixel_list;
         p.capacity = wb.capacity;
         p.global_seed = global_seed;
         p.spp = spp;
@@ -952,10 +958,12 @@ namespace
     // ---------------------------------------------------------------------------------------
     // Octree<Photon> + LinearOctree::compact on the host (octree.cpp:34-81, linear-octree.cpp:201-244).
     // Samples [sample_first, sample_first + spp) of every pixel of rows y_first + k*y_step, k < n_rows: resolved into
-    // out_dev, or added into the caller's sums when accum is given.
+    // out_dev, or added into the caller's sums when accum is given. d_pixel_list (accumulate mode only): only the n_list
+    // pixels it lists (positions in the n_rows x width grid) are rendered.
     int renderDispatch(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_t y_first, uint32_t y_step, uint32_t n_rows,
                        uint32_t sample_first, uint64_t spp, uint32_t global_seed, int integrator_kind, int precision,
-                       double* out_dev, mcrt_stats* stats, const FilmSums* accum = nullptr)
+                       double* out_dev, mcrt_stats* stats, const FilmSums* accum = nullptr,
+                       const uint32_t* d_pixel_list = nullptr, uint32_t n_list = 0)
     {
         if (!camera || n_rows == 0 || y_step == 0 || spp == 0 || camera->width == 0 ||
             (uint64_t)y_first + (uint64_t)(n_rows - 1) * y_step >= camera->height)
@@ -976,15 +984,18 @@ namespace
         const uint64_t n_pixels64 = (uint64_t)camera->width * n_rows;
         if (n_pixels64 > 0xFFFFFFFFull) { ctx->error = "row block too large"; return MCRT_ERR_INVALID; }
         const uint32_t n_pixels = (uint32_t)n_pixels64;
-        const uint64_t total = (uint64_t)n_pixels * spp;
+        const uint32_t n_work = d_pixel_list ? n_list : n_pixels;   // pixels the camera work covers
+        const uint64_t total = (uint64_t)n_work * spp;
         // a filtered film accumulates at image positions (samples splat across rows): its buffers span the whole frame
         const size_t film_pixels = ctx->film_default ? (size_t)n_pixels : (size_t)camera->width * camera->height;
         if (precision == MCRT_PRECISION_F64)
-            return runWavefront<double>(ctx, camera, y_first, y_step, n_pixels, (uint32_t)spp, total, global_seed, integrator_kind,
-                                        nullptr, nullptr, nullptr, film_pixels, (double)spp, out_dev, stats, sample_first, accum);
+            return runWavefront<double>(ctx, camera, y_first, y_step, n_work, (uint32_t)spp, total, global_seed, integrator_kind,
+                                        nullptr, nullptr, nullptr, film_pixels, (double)spp, out_dev, stats, sample_first, accum,
+                                        d_pixel_list);
         if (precision == MCRT_PRECISION_F32)
-            return runWavefront<float>(ctx, camera, y_first, y_step, n_pixels, (uint32_t)spp, total, global_seed, integrator_kind,
-                                       nullptr, nullptr, nullptr, film_pixels, (double)spp, out_dev, stats, sample_first, accum);
+            return runWavefront<float>(ctx, camera, y_first, y_step, n_work, (uint32_t)spp, total, global_seed, integrator_kind,
+                                       nullptr, nullptr, nullptr, film_pixels, (double)spp, out_dev, stats, sample_first, accum,
+                                       d_pixel_list);
         ctx->error = "unknown precision";
         return MCRT_ERR_INVALID;
     }
@@ -1001,6 +1012,26 @@ namespace
         }
         return renderDispatch(ctx, camera, y_first, y_step, n_rows, 0u, (uint64_t)sqrtspp * sqrtspp, global_seed,
                               integrator_kind, precision, out_dev, stats, accum);
+    }
+
+    // Arguments of the accumulate entry points: a sample count and sums that match the film
+    int checkAccumulateSums(mcrt_ctx* ctx, const char* fn, uint32_t sample_count, const double* rgb_sum_dev,
+                            const double* weight_sum_dev)
+    {
+        const std::string name(fn);
+        if (!rgb_sum_dev) { ctx->error = name + ": null rgb sums"; return MCRT_ERR_INVALID; }
+        if (sample_count == 0) { ctx->error = name + ": sample_count is 0"; return MCRT_ERR_INVALID; }
+        if (ctx->film_default && weight_sum_dev)
+        {
+            ctx->error = name + ": the box film is weighted by the sample count; weight_sum_dev must be NULL";
+            return MCRT_ERR_INVALID;
+        }
+        if (!ctx->film_default && !weight_sum_dev)
+        {
+            ctx->error = name + ": a reconstruction filter needs weight_sum_dev";
+            return MCRT_ERR_INVALID;
+        }
+        return MCRT_OK;
     }
 }
 
@@ -1059,6 +1090,7 @@ void mcrt_destroy(mcrt_ctx* ctx)
     if (ctx->d_film_cache) cudaFree(ctx->d_film_cache);
     if (ctx->d_host_out) cudaFree(ctx->d_host_out);
     if (ctx->d_resolve_scratch) cudaFree(ctx->d_resolve_scratch);
+    if (ctx->d_pixel_list) cudaFree(ctx->d_pixel_list);
     if (ctx->d_counters) cudaFree(ctx->d_counters);
     if (ctx->d_sobol_bytes) cudaFree(ctx->d_sobol_bytes);
     if (ctx->h_counters) cudaFreeHost(ctx->h_counters);
@@ -1645,22 +1677,140 @@ int mcrt_render_accumulate_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_
                                int precision, double* rgb_sum_dev, double* weight_sum_dev, mcrt_stats* stats)
 {
     if (!ctx) return MCRT_ERR_INVALID;
-    if (!rgb_sum_dev) { ctx->error = "mcrt_render_accumulate_dev: null rgb sums"; return MCRT_ERR_INVALID; }
-    if (sample_count == 0) { ctx->error = "mcrt_render_accumulate_dev: sample_count is 0"; return MCRT_ERR_INVALID; }
-    if (ctx->film_default && weight_sum_dev)
-    {
-        ctx->error = "mcrt_render_accumulate_dev: the box film is weighted by the sample count; weight_sum_dev must be NULL";
-        return MCRT_ERR_INVALID;
-    }
-    if (!ctx->film_default && !weight_sum_dev)
-    {
-        ctx->error = "mcrt_render_accumulate_dev: a reconstruction filter needs weight_sum_dev";
-        return MCRT_ERR_INVALID;
-    }
+    int rc;
+    if ((rc = checkAccumulateSums(ctx, "mcrt_render_accumulate_dev", sample_count, rgb_sum_dev, weight_sum_dev))) return rc;
     CK(cudaSetDevice(ctx->device));
     const FilmSums sums = { rgb_sum_dev, weight_sum_dev };
     return renderDispatch(ctx, camera, y_first, y_step, n_rows, sample_first, sample_count, global_seed, integrator_kind,
                           precision, nullptr, stats, &sums);
+}
+
+int mcrt_render_accumulate_tiles_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_t y_first, uint32_t y_step, uint32_t n_rows,
+                                     uint32_t tile, const uint8_t* active_tiles, uint32_t sample_first, uint32_t sample_count,
+                                     uint32_t global_seed, int integrator_kind, int precision, double* rgb_sum_dev,
+                                     double* weight_sum_dev, mcrt_stats* stats)
+{
+    if (!ctx) return MCRT_ERR_INVALID;
+    int rc;
+    if ((rc = checkAccumulateSums(ctx, "mcrt_render_accumulate_tiles_dev", sample_count, rgb_sum_dev, weight_sum_dev))) return rc;
+    if (tile == 0) { ctx->error = "mcrt_render_accumulate_tiles_dev: tile is 0"; return MCRT_ERR_INVALID; }
+    if (!active_tiles) { ctx->error = "mcrt_render_accumulate_tiles_dev: null tile mask"; return MCRT_ERR_INVALID; }
+    // the mask's size follows from the row set: check it before reading the mask
+    if (!camera || n_rows == 0 || y_step == 0 || camera->width == 0 ||
+        (uint64_t)y_first + (uint64_t)(n_rows - 1) * y_step >= camera->height)
+    {
+        ctx->error = "mcrt_render_accumulate_tiles_dev: invalid camera / row range";
+        return MCRT_ERR_INVALID;
+    }
+    if ((uint64_t)camera->width * n_rows > 0xFFFFFFFFull) { ctx->error = "row block too large"; return MCRT_ERR_INVALID; }
+    if (!ctx->film_default && (y_first != 0 || y_step != 1 || n_rows != camera->height))
+    {
+        // a filter splats across tiles: the resolve's tiles span the whole frame, so the row set must be the whole frame
+        ctx->error = "mcrt_render_accumulate_tiles_dev: with a reconstruction filter the row set must be the whole frame";
+        return MCRT_ERR_UNSUPPORTED;
+    }
+    // tile-major, row-major inside a tile: adjacent lanes of k_generate take adjacent pixels of one tile
+    const uint32_t width = camera->width;
+    const uint32_t tiles_x = (width + tile - 1) / tile, tiles_y = (n_rows + tile - 1) / tile;
+    std::vector<uint32_t>& list = ctx->h_pixel_list;
+    list.clear();
+    for (uint32_t ty = 0; ty < tiles_y; ty++)
+        for (uint32_t tx = 0; tx < tiles_x; tx++)
+        {
+            if (!active_tiles[(size_t)ty * tiles_x + tx]) continue;
+            const uint32_t y1 = std::min(n_rows, (ty + 1) * tile), x1 = std::min(width, (tx + 1) * tile);
+            for (uint32_t y = ty * tile; y < y1; y++)
+                for (uint32_t x = tx * tile; x < x1; x++) list.push_back(y * width + x);
+        }
+    if (list.empty()) { ctx->error = "mcrt_render_accumulate_tiles_dev: no active tile"; return MCRT_ERR_INVALID; }
+    CK(cudaSetDevice(ctx->device));
+    if (ctx->pixel_list_values < list.size())
+    {
+        if (ctx->d_pixel_list) cudaFree(ctx->d_pixel_list);
+        ctx->d_pixel_list = nullptr; ctx->pixel_list_values = 0;
+        CK(cudaMalloc((void**)&ctx->d_pixel_list, list.size() * sizeof(uint32_t)));
+        ctx->pixel_list_values = list.size();
+    }
+    CK(cudaMemcpyAsync(ctx->d_pixel_list, list.data(), list.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+    const FilmSums sums = { rgb_sum_dev, weight_sum_dev };
+    return renderDispatch(ctx, camera, y_first, y_step, n_rows, sample_first, sample_count, global_seed, integrator_kind,
+                          precision, nullptr, stats, &sums, ctx->d_pixel_list, (uint32_t)list.size());
+}
+
+namespace
+{
+    // Shared by mcrt_progressive_resolve_dev (tile_samples null: every pixel has a_samples / b_samples) and
+    // mcrt_progressive_resolve_tiles_dev (tile_samples: HOST {nA, nB}[n_tiles]).
+    int progressiveResolve(mcrt_ctx* ctx, const char* fn, const double* a_rgb_dev, const double* a_weight_dev, uint64_t a_samples,
+                           const double* b_rgb_dev, const double* b_weight_dev, uint64_t b_samples, const uint32_t* tile_samples,
+                           uint32_t width, uint32_t rows, uint32_t tile, double* out_rgb_dev, double* tile_error_dev,
+                           double* tile_sums_dev, double* frame_error)
+    {
+        const std::string name(fn);
+        if (!out_rgb_dev || width == 0 || rows == 0 || (uint64_t)width * rows > 0xFFFFFFFFull)
+        {
+            ctx->error = name + ": null output, empty frame or more than 2^32 pixels";
+            return MCRT_ERR_INVALID;
+        }
+        if (tile == 0) { ctx->error = name + ": tile is 0"; return MCRT_ERR_INVALID; }
+        const uint64_t tiles_x = (width + tile - 1) / tile, tiles_y = (rows + tile - 1) / tile;
+        const uint64_t n_tiles = tiles_x * tiles_y;
+        bool both = a_samples && b_samples;   // the frame error is finite only if every tile has both halves
+        if (tile_samples)
+        {
+            both = true;
+            for (uint64_t t = 0; t < n_tiles; t++)
+            {
+                a_samples += tile_samples[2 * t] != 0; b_samples += tile_samples[2 * t + 1] != 0;
+                both = both && tile_samples[2 * t] != 0 && tile_samples[2 * t + 1] != 0;
+            }
+        }
+        if (a_samples + b_samples == 0) { ctx->error = name + ": no samples to resolve"; return MCRT_ERR_INVALID; }
+        if ((a_samples && !a_rgb_dev) || (b_samples && !b_rgb_dev))
+        {
+            ctx->error = name + ": null sums for a half with samples";
+            return MCRT_ERR_INVALID;
+        }
+        const bool weighted = a_weight_dev || b_weight_dev;
+        if (weighted && ((a_samples && !a_weight_dev) || (b_samples && !b_weight_dev)))
+        {
+            ctx->error = name + ": weight sums must be given for both halves or for neither";
+            return MCRT_ERR_INVALID;
+        }
+        CK(cudaSetDevice(ctx->device));
+        // scratch: {sum v, sum I^2} per tile, then the frame's; then the tiles' {nA, nB} when they are given
+        const size_t sums_values = 2 * (n_tiles + 1);
+        const size_t scratch_values = sums_values + (tile_samples ? 2 * n_tiles : 0);
+        if (ctx->resolve_scratch_values < scratch_values)
+        {
+            if (ctx->d_resolve_scratch) cudaFree(ctx->d_resolve_scratch);
+            ctx->d_resolve_scratch = nullptr; ctx->resolve_scratch_values = 0;
+            CK(cudaMalloc((void**)&ctx->d_resolve_scratch, scratch_values * sizeof(double)));
+            ctx->resolve_scratch_values = scratch_values;
+        }
+        double* d_counts = nullptr;
+        std::vector<double> counts;
+        if (tile_samples)
+        {
+            counts.assign(tile_samples, tile_samples + 2 * n_tiles);
+            d_counts = ctx->d_resolve_scratch + sums_values;
+            CK(cudaMemcpyAsync(d_counts, counts.data(), counts.size() * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+        }
+        // with per-tile counts the halves' scalar counts are unused: only whether a half has samples anywhere matters
+        ProgressiveHalf a = { a_samples ? a_rgb_dev : nullptr, a_samples ? a_weight_dev : nullptr, tile_samples ? 0.0 : (double)a_samples };
+        ProgressiveHalf b = { b_samples ? b_rgb_dev : nullptr, b_samples ? b_weight_dev : nullptr, tile_samples ? 0.0 : (double)b_samples };
+        CK(cudaMemsetAsync(ctx->d_resolve_scratch, 0, sums_values * sizeof(double), ctx->stream));
+        launchProgressiveResolve(a, b, weighted, width, rows, tile, (uint32_t)tiles_x, out_rgb_dev, ctx->d_resolve_scratch, tile_error_dev,
+                                 (uint32_t)n_tiles, ctx->sm_count * ctx->blocks_per_sm, ctx->stream, d_counts);
+        if (tile_sums_dev)
+            CK(cudaMemcpyAsync(tile_sums_dev, ctx->d_resolve_scratch, 2 * n_tiles * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
+        double frame_sums[2] = { 0.0, 0.0 };
+        CK(cudaMemcpyAsync(frame_sums, ctx->d_resolve_scratch + 2 * n_tiles, sizeof(frame_sums), cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+        CK(cudaGetLastError());
+        if (frame_error) *frame_error = progressiveRelativeError(frame_sums[0], frame_sums[1], both);
+        return MCRT_OK;
+    }
 }
 
 int mcrt_progressive_resolve_dev(mcrt_ctx* ctx, const double* a_rgb_dev, const double* a_weight_dev, uint64_t a_samples,
@@ -1669,47 +1819,19 @@ int mcrt_progressive_resolve_dev(mcrt_ctx* ctx, const double* a_rgb_dev, const d
                                  double* tile_error_dev, double* frame_error)
 {
     if (!ctx) return MCRT_ERR_INVALID;
-    if (!out_rgb_dev || width == 0 || rows == 0 || (uint64_t)width * rows > 0xFFFFFFFFull)
-    {
-        ctx->error = "mcrt_progressive_resolve_dev: null output, empty frame or more than 2^32 pixels";
-        return MCRT_ERR_INVALID;
-    }
-    if (tile == 0) { ctx->error = "mcrt_progressive_resolve_dev: tile is 0"; return MCRT_ERR_INVALID; }
-    if (a_samples + b_samples == 0) { ctx->error = "mcrt_progressive_resolve_dev: no samples to resolve"; return MCRT_ERR_INVALID; }
-    if ((a_samples && !a_rgb_dev) || (b_samples && !b_rgb_dev))
-    {
-        ctx->error = "mcrt_progressive_resolve_dev: null sums for a half with samples";
-        return MCRT_ERR_INVALID;
-    }
-    const bool weighted = a_weight_dev || b_weight_dev;
-    if (weighted && ((a_samples && !a_weight_dev) || (b_samples && !b_weight_dev)))
-    {
-        ctx->error = "mcrt_progressive_resolve_dev: weight sums must be given for both halves or for neither";
-        return MCRT_ERR_INVALID;
-    }
-    CK(cudaSetDevice(ctx->device));
-    const uint64_t tiles_x = (width + tile - 1) / tile, tiles_y = (rows + tile - 1) / tile;
-    const uint64_t n_tiles = tiles_x * tiles_y;
-    // scratch: {sum v, sum I^2} per tile, then the frame's
-    const size_t scratch_values = 2 * (n_tiles + 1);
-    if (ctx->resolve_scratch_values < scratch_values)
-    {
-        if (ctx->d_resolve_scratch) cudaFree(ctx->d_resolve_scratch);
-        ctx->d_resolve_scratch = nullptr; ctx->resolve_scratch_values = 0;
-        CK(cudaMalloc((void**)&ctx->d_resolve_scratch, scratch_values * sizeof(double)));
-        ctx->resolve_scratch_values = scratch_values;
-    }
-    ProgressiveHalf a = { a_samples ? a_rgb_dev : nullptr, a_samples ? a_weight_dev : nullptr, (double)a_samples };
-    ProgressiveHalf b = { b_samples ? b_rgb_dev : nullptr, b_samples ? b_weight_dev : nullptr, (double)b_samples };
-    CK(cudaMemsetAsync(ctx->d_resolve_scratch, 0, scratch_values * sizeof(double), ctx->stream));
-    launchProgressiveResolve(a, b, weighted, width, rows, tile, (uint32_t)tiles_x, out_rgb_dev, ctx->d_resolve_scratch, tile_error_dev,
-                             (uint32_t)n_tiles, ctx->sm_count * ctx->blocks_per_sm, ctx->stream);
-    double frame_sums[2] = { 0.0, 0.0 };
-    CK(cudaMemcpyAsync(frame_sums, ctx->d_resolve_scratch + 2 * n_tiles, sizeof(frame_sums), cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-    CK(cudaGetLastError());
-    if (frame_error) *frame_error = progressiveRelativeError(frame_sums[0], frame_sums[1], a_samples && b_samples);
-    return MCRT_OK;
+    return progressiveResolve(ctx, "mcrt_progressive_resolve_dev", a_rgb_dev, a_weight_dev, a_samples, b_rgb_dev, b_weight_dev,
+                              b_samples, nullptr, width, rows, tile, out_rgb_dev, tile_error_dev, nullptr, frame_error);
+}
+
+int mcrt_progressive_resolve_tiles_dev(mcrt_ctx* ctx, const double* a_rgb_dev, const double* a_weight_dev,
+                                       const double* b_rgb_dev, const double* b_weight_dev, const uint32_t* tile_samples,
+                                       uint32_t width, uint32_t rows, uint32_t tile, double* out_rgb_dev,
+                                       double* tile_error_dev, double* tile_sums_dev, double* frame_error)
+{
+    if (!ctx) return MCRT_ERR_INVALID;
+    if (!tile_samples) { ctx->error = "mcrt_progressive_resolve_tiles_dev: null tile_samples"; return MCRT_ERR_INVALID; }
+    return progressiveResolve(ctx, "mcrt_progressive_resolve_tiles_dev", a_rgb_dev, a_weight_dev, 0, b_rgb_dev, b_weight_dev, 0,
+                              tile_samples, width, rows, tile, out_rgb_dev, tile_error_dev, tile_sums_dev, frame_error);
 }
 
 int mcrt_film_resolve_dev(mcrt_ctx* ctx, const double* rgb_sum_dev, const double* weight_sum_dev, uint64_t n_pixels, double* out_rgb_dev)

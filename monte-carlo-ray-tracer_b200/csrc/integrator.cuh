@@ -234,6 +234,9 @@ namespace mcrt
         const double* user_rays;
         const uint32_t* user_pixel;
         const uint32_t* user_sample;
+        // camera work over a subset of the pixels (k_generate<R, FILM, true>): the pixels' positions in the
+        // n_rows x width grid, tile-major and row-major inside a tile; n_pixels is then the list's length
+        const uint32_t* pixel_list;
         uint32_t capacity;
         uint32_t global_seed;
         uint32_t spp;
@@ -426,7 +429,9 @@ namespace mcrt
         }
     }
 
-    template <class R, bool FILM>
+    // LIST: camera work item w is sample w / n_pixels of pixel pixel_list[w % n_pixels] (adaptive sampling);
+    // otherwise of pixel w % n_pixels
+    template <class R, bool FILM, bool LIST>
     __global__ void __launch_bounds__(256) k_generate(WaveParams<R> p, int next)
     {
         Counters* c = p.counters;
@@ -461,7 +466,8 @@ namespace mcrt
             else
             {
                 // sample-major over this rank's pixels: adjacent lanes = adjacent pixels
-                const uint32_t local = (uint32_t)(w % p.n_pixels);
+                uint32_t local = (uint32_t)(w % p.n_pixels);
+                if constexpr (LIST) local = p.pixel_list[local];
                 // a progressive pass starts at work item sample_first * n_pixels (runWavefront)
                 sample = (uint32_t)(w / p.n_pixels);
                 const uint32_t row = local / p.camera.width, col = local - row * p.camera.width;

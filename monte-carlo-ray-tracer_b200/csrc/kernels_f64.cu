@@ -37,9 +37,14 @@ namespace mcrt
     // channel v = (I_A - I_B)^2 nA nB / (nA+nB)^2 with I_A = A/wA, I_B = B/wB: for independent halves an unbiased
     // estimate of the variance of the combined mean. v and I^2 are summed per tile x tile block of the buffer's
     // rows x width (one atomic per warp and tile) and over the frame (one atomic per warp).
+    // TILE_COUNTS (adaptive sampling): nA, nB are those of the pixel's tile, tile_counts[tile][2], instead of
+    // a.samples, b.samples. With a filter a pixel near a tile's border also holds splats of samples of neighbouring
+    // tiles, which may have other counts; its own tile's counts in the scale are then an approximation.
+    template <bool TILE_COUNTS>
     static __global__ void __launch_bounds__(256) k_progressive_resolve(ProgressiveHalf a, ProgressiveHalf b, uint32_t weighted,
                                                                         uint32_t width, uint32_t rows, uint32_t tile,
-                                                                        uint32_t tiles_x, uint32_t n_tiles, double* out, double* sums)
+                                                                        uint32_t tiles_x, uint32_t n_tiles, double* out, double* sums,
+                                                                        const double* tile_counts)
     {
         const uint64_t n = (uint64_t)width * rows;
         const bool both = a.samples > 0.0 && b.samples > 0.0;
@@ -53,10 +58,20 @@ namespace mcrt
             uint32_t key = 0xFFFFFFFFu;
             if (i < n)
             {
-                const double wa = !a.rgb ? 0.0 : (weighted ? a.wsum[i] : a.samples);
-                const double wb = !b.rgb ? 0.0 : (weighted ? b.wsum[i] : b.samples);
+                double na = a.samples, nb = b.samples, pixel_scale = scale;
+                bool pixel_both = both;
+                if constexpr (TILE_COUNTS)
+                {
+                    const uint32_t y = (uint32_t)(i / width), x = (uint32_t)(i - (uint64_t)y * width);
+                    const size_t t = (size_t)(y / tile) * tiles_x + x / tile;
+                    na = tile_counts[2 * t]; nb = tile_counts[2 * t + 1];
+                    pixel_both = na > 0.0 && nb > 0.0;
+                    pixel_scale = pixel_both ? na * nb / ((na + nb) * (na + nb)) : 0.0;
+                }
+                const double wa = !a.rgb ? 0.0 : (weighted ? a.wsum[i] : na);
+                const double wb = !b.rgb ? 0.0 : (weighted ? b.wsum[i] : nb);
                 const double w = wa + wb;
-                const bool compare = both && wa != 0.0 && wb != 0.0;
+                const bool compare = pixel_both && wa != 0.0 && wb != 0.0;
                 for (int c = 0; c < 3; c++)
                 {
                     const double sa = a.rgb ? a.rgb[3 * i + c] : 0.0, sb = b.rgb ? b.rgb[3 * i + c] : 0.0;
@@ -67,7 +82,7 @@ namespace mcrt
                     if (compare)
                     {
                         const double d = sa / wa - sb / wb;
-                        v += d * d * scale;
+                        v += d * d * pixel_scale;
                     }
                 }
                 const uint32_t y = (uint32_t)(i / width), x = (uint32_t)(i - (uint64_t)y * width);
@@ -107,20 +122,31 @@ namespace mcrt
         }
     }
 
-    static __global__ void k_progressive_tile_error(const double* sums, uint32_t n_tiles, bool both_halves, double* tile_error)
+    // TILE_COUNTS: a tile has both halves when its own counts tile_counts[t][2] are both nonzero
+    template <bool TILE_COUNTS>
+    static __global__ void k_progressive_tile_error(const double* sums, uint32_t n_tiles, bool both_halves, double* tile_error,
+                                                    const double* tile_counts)
     {
         for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < n_tiles; t += gridDim.x * blockDim.x)
-            tile_error[t] = progressiveRelativeError(sums[2 * (size_t)t], sums[2 * (size_t)t + 1], both_halves);
+        {
+            bool both = both_halves;
+            if constexpr (TILE_COUNTS) both = tile_counts[2 * (size_t)t] > 0.0 && tile_counts[2 * (size_t)t + 1] > 0.0;
+            tile_error[t] = progressiveRelativeError(sums[2 * (size_t)t], sums[2 * (size_t)t + 1], both);
+        }
     }
 
     void launchProgressiveResolve(const ProgressiveHalf& a, const ProgressiveHalf& b, bool weighted, uint32_t width, uint32_t rows,
                                   uint32_t tile, uint32_t tiles_x, double* out, double* sums, double* tile_error, uint32_t n_tiles,
-                                  int grid, cudaStream_t s)
+                                  int grid, cudaStream_t s, const double* tile_counts)
     {
-        k_progressive_resolve<<<grid, 256, 0, s>>>(a, b, weighted ? 1u : 0u, width, rows, tile, tiles_x, n_tiles, out, sums);
-        if (tile_error)
-            k_progressive_tile_error<<<(n_tiles + 255) / 256 < (uint32_t)grid ? (n_tiles + 255) / 256 : (uint32_t)grid, 256, 0, s>>>(
-                sums, n_tiles, a.samples > 0.0 && b.samples > 0.0, tile_error);
+        const uint32_t w = weighted ? 1u : 0u;
+        if (tile_counts) k_progressive_resolve<true><<<grid, 256, 0, s>>>(a, b, w, width, rows, tile, tiles_x, n_tiles, out, sums, tile_counts);
+        else k_progressive_resolve<false><<<grid, 256, 0, s>>>(a, b, w, width, rows, tile, tiles_x, n_tiles, out, sums, nullptr);
+        if (!tile_error) return;
+        const uint32_t tile_grid = (n_tiles + 255) / 256 < (uint32_t)grid ? (n_tiles + 255) / 256 : (uint32_t)grid;
+        const bool both = a.samples > 0.0 && b.samples > 0.0;
+        if (tile_counts) k_progressive_tile_error<true><<<tile_grid, 256, 0, s>>>(sums, n_tiles, both, tile_error, tile_counts);
+        else k_progressive_tile_error<false><<<tile_grid, 256, 0, s>>>(sums, n_tiles, both, tile_error, nullptr);
     }
 
     void launchFp64Peak(double* sink, int iterations, int grid, cudaStream_t s)

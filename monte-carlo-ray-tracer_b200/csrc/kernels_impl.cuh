@@ -5,8 +5,14 @@ namespace mcrt
 {
     template <> void Launch<MCRT_REAL>::generate(const WaveParams<MCRT_REAL>& p, int next, int grid, cudaStream_t s)
     {
-        if (p.filmp.is_default_box) k_generate<MCRT_REAL, false><<<grid, 256, 0, s>>>(p, next);
-        else k_generate<MCRT_REAL, true><<<grid, 256, 0, s>>>(p, next);
+        if (p.pixel_list)
+        {
+            if (p.filmp.is_default_box) k_generate<MCRT_REAL, false, true><<<grid, 256, 0, s>>>(p, next);
+            else k_generate<MCRT_REAL, true, true><<<grid, 256, 0, s>>>(p, next);
+            return;
+        }
+        if (p.filmp.is_default_box) k_generate<MCRT_REAL, false, false><<<grid, 256, 0, s>>>(p, next);
+        else k_generate<MCRT_REAL, true, false><<<grid, 256, 0, s>>>(p, next);
     }
     template <> void Launch<MCRT_REAL>::extend(const WaveParams<MCRT_REAL>& p, int cur, int grid, cudaStream_t s)
     {

@@ -30,9 +30,10 @@ namespace mcrt
     void launchResolveFilmPeers(const double* film, const PeerFrames& pf, size_t n_values, double weight, int grid, cudaStream_t s);
     // Resolves a+b into out and adds {sum v, sum I^2} of each tile into sums[2*tile..] and of the frame into
     // sums[2*n_tiles..] (zeroed by the caller); tile_error (optional) receives the per-tile relative errors.
+    // tile_counts (device, optional): per-tile {nA, nB}[n_tiles] in place of a.samples, b.samples.
     void launchProgressiveResolve(const ProgressiveHalf& a, const ProgressiveHalf& b, bool weighted, uint32_t width, uint32_t rows,
                                   uint32_t tile, uint32_t tiles_x, double* out, double* sums, double* tile_error, uint32_t n_tiles,
-                                  int grid, cudaStream_t s);
+                                  int grid, cudaStream_t s, const double* tile_counts = nullptr);
     void launchFp64Peak(double* sink, int iterations, int grid, cudaStream_t s);
     void launchKnnUser(const DevicePhotonMap& map, uint32_t k, const double* points, size_t n, uint32_t* out_index,
                        double* out_d2, uint32_t* out_count, uint32_t* overflow_flag, int grid, cudaStream_t s);
