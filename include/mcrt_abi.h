@@ -422,6 +422,47 @@ int mcrt_progressive_resolve_tiles_dev(mcrt_ctx* ctx, const double* a_rgb_dev, c
                                        uint32_t width, uint32_t rows, uint32_t tile, double* out_rgb_dev,
                                        double* tile_error_dev, double* tile_sums_dev, double* frame_error);
 
+/* Denoising a progressive frame (mcrt_denoise_dev) needs per-pixel guides: the first hits of the camera rays of samples
+ * [sample_first, sample_first + sample_count) of every pixel of the whole width x height frame add
+ * {albedo.rgb, shading normal.xyz, t, 1} per hit into features_dev [height*width][8] (device, float64); a miss adds
+ * nothing. Albedo is the specular reflectance of perfect mirrors and complex-IOR materials, the reflectance of every
+ * other material; the shading normal faces the ray. The sums are added to, never zeroed; each pixel adds its samples
+ * in increasing order, so consecutive ranges accumulate bit-identically to their union. The guides are per pixel
+ * (a box footprint) whatever film is set, and depend on the scene, camera, seed and sample range only.
+ * MCRT_ERR_INVALID: a null camera or buffer, sample_count 0, sample_first + sample_count > 2^32, an empty frame or
+ * more than 2^32 pixels, an unknown precision. MCRT_ERR_NO_SCENE before mcrt_scene_upload. */
+int mcrt_render_features_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_t sample_first, uint32_t sample_count,
+                             uint32_t global_seed, int precision, double* features_dev, mcrt_stats* stats);
+
+/* Parameters of mcrt_denoise_dev; a NULL pointer selects the MCRT_DENOISE_DEFAULT_* values. */
+typedef struct mcrt_denoise_params {
+    uint32_t iterations;   /* 0..10 a-trous passes of steps 1, 2, 4, ...; 0 = the two halves' plain resolve */
+    uint32_t _pad;
+    double sigma_color, sigma_normal, sigma_depth, sigma_albedo;   /* >= 0, finite; 0 switches the term off */
+} mcrt_denoise_params;
+
+#define MCRT_DENOISE_MAX_ITERATIONS 10
+#define MCRT_DENOISE_DEFAULT_ITERATIONS 5
+#define MCRT_DENOISE_DEFAULT_SIGMA_COLOR 1.0
+#define MCRT_DENOISE_DEFAULT_SIGMA_NORMAL 64.0
+#define MCRT_DENOISE_DEFAULT_SIGMA_DEPTH 0.1
+#define MCRT_DENOISE_DEFAULT_SIGMA_ALBEDO 0.1
+
+/* Cross-filtered a-trous denoiser over the two halves of a progressive frame (whole frame, float64). The sums and
+ * weights are those mcrt_progressive_resolve_tiles_dev takes, with tile_samples (HOST) {nA, nB}[n_tiles] (uniform
+ * renders pass equal counts); features_dev are mcrt_render_features_dev's sums. Each half is filtered with edge-stopping
+ * weights from the guides (normal, relative depth, albedo) and a colour term measured on the other half, so the
+ * difference of the filtered halves still estimates the residual noise: out_rgb_dev [height*width][3] receives
+ * max(0, (wA A' + wB B') / (wA + wB)) and *frame_error sqrt(sum v' / sum out^2) with v' = sum_c (A' - B')^2 wA wB /
+ * (wA + wB)^2 (0 if sum v' = 0, +inf if sum out^2 = 0 < sum v'). A pixel with zero weight in a half is output as its
+ * plain resolve. Device buffers except tile_samples, params and frame_error. MCRT_ERR_INVALID: a null buffer, an
+ * empty frame or more than 2^32 pixels, tile 0, a tile with an empty half, weight sums given for one half only,
+ * iterations > MCRT_DENOISE_MAX_ITERATIONS, a negative or non-finite sigma. */
+int mcrt_denoise_dev(mcrt_ctx* ctx, const double* a_rgb_dev, const double* a_weight_dev,
+                     const double* b_rgb_dev, const double* b_weight_dev, const uint32_t* tile_samples,
+                     uint32_t tile, const double* features_dev, uint32_t width, uint32_t height,
+                     const mcrt_denoise_params* params, double* out_rgb_dev, double* frame_error);
+
 /* A device buffer that other processes on the node can map: *dev_ptr (zero-filled) and its 64-byte CUDA IPC
  * handle, to be sent to the peers by whatever channel the host uses (torch.distributed in this repository). */
 int mcrt_frame_alloc(mcrt_ctx* ctx, uint64_t bytes, void** dev_ptr, unsigned char ipc_handle[64]);

@@ -38,6 +38,7 @@ ABI_SYMBOLS = [
     "mcrt_fp64_peak", "mcrt_photon_emit_total", "mcrt_photon_emit_range", "mcrt_photon_build_dev",
     "mcrt_render_accumulate_dev", "mcrt_progressive_resolve_dev",
     "mcrt_render_accumulate_tiles_dev", "mcrt_progressive_resolve_tiles_dev",
+    "mcrt_render_features_dev", "mcrt_denoise_dev",
 ]
 
 
@@ -46,6 +47,15 @@ class McrtError(RuntimeError):
 
 
 # ------------------------------------------------------------------------------------ ctypes structs
+class DenoiseParams(C.Structure):
+    _fields_ = [("iterations", C.c_uint32), ("_pad", C.c_uint32), ("sigma_color", C.c_double), ("sigma_normal", C.c_double),
+                ("sigma_depth", C.c_double), ("sigma_albedo", C.c_double)]
+
+
+# MCRT_DENOISE_DEFAULT_* of mcrt_abi.h
+DENOISE_DEFAULTS = {"iterations": 5, "sigma_color": 1.0, "sigma_normal": 64.0, "sigma_depth": 0.1, "sigma_albedo": 0.1}
+
+
 class MaterialRec(C.Structure):
     _fields_ = [("reflectance", C.c_double * 3), ("specular_reflectance", C.c_double * 3),
                 ("transmittance", C.c_double * 3), ("emittance", C.c_double * 3),
@@ -220,6 +230,11 @@ def lib():
         L.mcrt_progressive_resolve_tiles_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                                          C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p,
                                                          C.POINTER(C.c_double)]
+        L.mcrt_render_features_dev.argtypes = [C.c_void_p, C.POINTER(CameraRec), C.c_uint32, C.c_uint32, C.c_uint32, C.c_int,
+                                               C.c_void_p, C.POINTER(Stats)]
+        L.mcrt_denoise_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32,
+                                       C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(DenoiseParams), C.c_void_p,
+                                       C.POINTER(C.c_double)]
         L.mcrt_photon_emit_total.argtypes = [C.c_void_p, C.POINTER(PhotonEmitParams), C.POINTER(C.c_uint64)]
         L.mcrt_photon_emit_range.argtypes = [C.c_void_p, C.POINTER(PhotonEmitParams), C.c_int, C.c_uint64, C.c_uint64, C.POINTER(C.c_void_p),
                                              C.POINTER(C.c_uint64), C.POINTER(C.c_void_p), C.POINTER(C.c_uint64), C.POINTER(Stats)]
@@ -632,6 +647,32 @@ class Integrator:
                                                              p(tile_error_ptr), p(tile_sums_ptr), C.byref(err)))
         return err.value
 
+    # -- denoising (see Progressive.denoise)
+    def render_features_dev(self, camera, features_ptr, sample_first, sample_count, precision=None):
+        """mcrt_render_features_dev: adds the first-hit guides {albedo.rgb, normal.xyz, t, hits} of samples
+        [sample_first, sample_first + sample_count) of every pixel into device sums [height, width, 8]."""
+        st = Stats()
+        self._check(lib().mcrt_render_features_dev(self.ctx, C.byref(camera.rec), sample_first, sample_count, self.global_seed,
+                                                   self.precision if precision is None else precision,
+                                                   C.c_void_p(features_ptr) if features_ptr else None, C.byref(st)))
+        self.last_stats = st.as_dict()
+        return self.last_stats
+
+    def denoise_dev(self, a_rgb_ptr, a_weight_ptr, b_rgb_ptr, b_weight_ptr, tile_samples, tile, features_ptr, width, height,
+                    out_ptr, params=None):
+        """mcrt_denoise_dev: the denoised frame of halves A and B into out_ptr [height, width, 3] -> its residual error.
+        tile_samples: {nA, nB} per tile [tiles_y, tiles_x, 2]; params: a DenoiseParams, or None for the defaults."""
+        def p(x):
+            return C.c_void_p(x) if x else None
+        counts = np.ascontiguousarray(tile_samples, dtype=np.uint32)
+        if counts.shape != tile_grid(height, width, tile) + (2,):
+            raise McrtError(f"tile_samples has shape {counts.shape}, expected {tile_grid(height, width, tile) + (2,)}")
+        err = C.c_double()
+        self._check(lib().mcrt_denoise_dev(self.ctx, p(a_rgb_ptr), p(a_weight_ptr), p(b_rgb_ptr), p(b_weight_ptr),
+                                           counts.ctypes.data_as(C.c_void_p), tile, p(features_ptr), width, height,
+                                           C.byref(params) if params is not None else None, p(out_ptr), C.byref(err)))
+        return err.value
+
     def frame_alloc(self, nbytes):
         """-> (device pointer, 64-byte CUDA IPC handle) of a zero-filled buffer other ranks can map"""
         ptr = C.c_void_p(); h = (C.c_ubyte * 64)()
@@ -1011,6 +1052,7 @@ class Progressive:
         self.tile_counts = np.zeros(grid + (2,), np.int64)          # samples per pixel of each tile in A and B
         self.history = []                                           # one record per render_adaptive pass
         self.stop_reason = None                                     # why the last render_adaptive stopped
+        self._features = None                                       # (samples, device sums [height, width, 8]) of features()
 
     @property
     def samples(self):
@@ -1124,6 +1166,59 @@ class Progressive:
             self.retire(entry["retired"])
             self.history.append(entry)
         return self.frame()
+
+    # -- denoising
+    def _feature_sums(self, samples):
+        """Device feature sums of samples [0, samples), computed once per sample count."""
+        import torch
+        samples = int(samples)
+        if self._features is None or self._features[0] != samples:
+            f = torch.zeros((self.camera.height, self.camera.width, 8), dtype=torch.float64, device=self.rgb[0].device)
+            torch.cuda.synchronize(f.device)   # the library renders on its own stream
+            self.integrator.render_features_dev(self.camera, f.data_ptr(), 0, samples)
+            self._features = (samples, f)
+        return self._features[1]
+
+    def features(self, samples=8):
+        """First-hit guides of the camera rays of samples [0, samples) of every pixel of the whole frame, as numpy:
+        {albedo [H,W,3], normal [H,W,3] (normalised mean, 0 where nothing was hit), depth [H,W] (mean hit distance),
+        coverage [H,W] (hits / samples)}. The device sums are kept and recomputed only when `samples` changes."""
+        f = self._feature_sums(samples).cpu().numpy()
+        hits = f[..., 7]
+        with np.errstate(invalid="ignore", divide="ignore"):
+            albedo = np.where(hits[..., None] > 0, f[..., 0:3] / hits[..., None], 0.0)
+            depth = np.where(hits > 0, f[..., 6] / hits, 0.0)
+            length = np.sqrt((f[..., 3:6] ** 2).sum(-1, keepdims=True))
+            normal = np.where(length > 0, f[..., 3:6] / length, 0.0)
+        return {"albedo": albedo, "normal": normal, "depth": depth, "coverage": hits / float(samples)}
+
+    def denoise(self, iterations=None, sigma_color=None, sigma_normal=None, sigma_depth=None, sigma_albedo=None,
+                feature_samples=8):
+        """The frame denoised by the cross-filtered a-trous filter of mcrt_denoise_dev, guided by features(feature_samples)
+        -> (frame float64 [H, W, 3], residual error). The error is estimated like error()'s, from the difference of the
+        two filtered halves: it measures the remaining noise, not the filter's bias. Arguments left None take the
+        defaults of DENOISE_DEFAULTS. Uses the per-tile counts, so it works after adaptive retirement too.
+        Raises McrtError unless the row set is the whole frame and every tile has samples in both halves.
+
+        Known limits: the guides come from the first hit only, so glass and mirrors are guided by their own surface,
+        not by what they show; the feature samples [0, F) also feed half A; the Owen-scrambled halves are not
+        independent, so the residual estimate can read about 10 % low."""
+        import torch
+        if (self.y_first, self.y_step, self.n_rows) != (0, 1, self.camera.height):
+            raise McrtError("denoise needs the whole frame as the row set (y_first 0, y_step 1, n_rows = height)")
+        if not (self.tile_counts > 0).all():
+            raise McrtError("denoise needs samples in both halves of every tile")
+        given = {"iterations": iterations, "sigma_color": sigma_color, "sigma_normal": sigma_normal,
+                 "sigma_depth": sigma_depth, "sigma_albedo": sigma_albedo}
+        v = {k: DENOISE_DEFAULTS[k] if x is None else x for k, x in given.items()}
+        params = DenoiseParams(int(v["iterations"]), 0, float(v["sigma_color"]), float(v["sigma_normal"]),
+                               float(v["sigma_depth"]), float(v["sigma_albedo"]))
+        feats = self._feature_sums(feature_samples)
+        out = torch.empty_like(self.rgb[0])
+        w = (self.wsum[0].data_ptr(), self.wsum[1].data_ptr()) if self.filtered else (None, None)
+        err = self.integrator.denoise_dev(self.rgb[0].data_ptr(), w[0], self.rgb[1].data_ptr(), w[1], self.tile_counts, self.tile,
+                                          feats.data_ptr(), self.camera.width, self.camera.height, out.data_ptr(), params)
+        return out.cpu().numpy(), err
 
     # -- checkpoint / resume
     def _identity(self):

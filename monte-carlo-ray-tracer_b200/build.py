@@ -21,6 +21,7 @@ UNITS = [
     ("bvh_build.cu", ["--fmad=false"]),
     ("image.cu", ["--fmad=false"]),
     ("obj_abi.cu", ["--fmad=false"]),
+    ("denoise.cu", ["--fmad=false"]),
     ("abi.cu", []),
 ]
 

@@ -14,6 +14,7 @@
 #include "launch.h"
 #include "bvh_build.h"
 #include "image.h"
+#include "denoise.h"
 
 using namespace mcrt;
 
@@ -90,6 +91,8 @@ struct mcrt_ctx
     size_t host_out_values = 0;
     double* d_resolve_scratch = nullptr;   // per-tile noise sums of mcrt_progressive_resolve_dev (grow-only)
     size_t resolve_scratch_values = 0;
+    double* d_denoise_scratch = nullptr;   // state, guides, tile counts and sums of mcrt_denoise_dev (grow-only)
+    size_t denoise_scratch_values = 0;
     uint32_t* d_pixel_list = nullptr;      // pixels of the active tiles of mcrt_render_accumulate_tiles_dev (grow-only)
     size_t pixel_list_values = 0;
     std::vector<uint32_t> h_pixel_list;
@@ -641,6 +644,18 @@ namespace
         st->replayed_rays = c.replayed_rays;
     }
 
+    template <class R> DeviceCamera<R> deviceCamera(const mcrt_camera& cam)
+    {
+        DeviceCamera<R> c;
+        std::memset(&c, 0, sizeof(c));
+        c.eye = v3<R>(cam.eye); c.forward = v3<R>(cam.forward);
+        c.left = v3<R>(cam.left); c.up = v3<R>(cam.up);
+        c.focal_length = (R)cam.focal_length; c.sensor_width = (R)cam.sensor_width;
+        c.aperture_radius = (R)cam.aperture_radius; c.focus_distance = (R)cam.focus_distance;
+        c.width = cam.width; c.height = cam.height; c.thin_lens = cam.thin_lens;
+        return c;
+    }
+
     // Accumulate mode of runWavefront: the samples are added into the caller's device sums, which are neither
     // zeroed before the render nor resolved after it (mcrt_render_accumulate_dev, mcrt_render_film_sums_strided_dev).
     struct FilmSums
@@ -701,14 +716,7 @@ namespace
         p.scene = sceneOf<R>(ctx);
         if (ctx->exact_traversal) p.scene.bvh4 = nullptr;
         p.scene.dynamic_fetch = (ctx->dynamic_fetch < 0 ? ctx->n_bvh4_nodes >= 2048u : ctx->dynamic_fetch != 0) ? 1u : 0u;
-        if (cam)
-        {
-            p.camera.eye = v3<R>(cam->eye); p.camera.forward = v3<R>(cam->forward);
-            p.camera.left = v3<R>(cam->left); p.camera.up = v3<R>(cam->up);
-            p.camera.focal_length = (R)cam->focal_length; p.camera.sensor_width = (R)cam->sensor_width;
-            p.camera.aperture_radius = (R)cam->aperture_radius; p.camera.focus_distance = (R)cam->focus_distance;
-            p.camera.width = cam->width; p.camera.height = cam->height; p.camera.thin_lens = cam->thin_lens;
-        }
+        if (cam) p.camera = deviceCamera<R>(*cam);
         p.buf[0] = wb.buf[0]; p.buf[1] = wb.buf[1];
         p.shadow = wb.shadow;
         p.hits = wb.hits;
@@ -1090,6 +1098,7 @@ void mcrt_destroy(mcrt_ctx* ctx)
     if (ctx->d_film_cache) cudaFree(ctx->d_film_cache);
     if (ctx->d_host_out) cudaFree(ctx->d_host_out);
     if (ctx->d_resolve_scratch) cudaFree(ctx->d_resolve_scratch);
+    if (ctx->d_denoise_scratch) cudaFree(ctx->d_denoise_scratch);
     if (ctx->d_pixel_list) cudaFree(ctx->d_pixel_list);
     if (ctx->d_counters) cudaFree(ctx->d_counters);
     if (ctx->d_sobol_bytes) cudaFree(ctx->d_sobol_bytes);
@@ -1832,6 +1841,107 @@ int mcrt_progressive_resolve_tiles_dev(mcrt_ctx* ctx, const double* a_rgb_dev, c
     if (!tile_samples) { ctx->error = "mcrt_progressive_resolve_tiles_dev: null tile_samples"; return MCRT_ERR_INVALID; }
     return progressiveResolve(ctx, "mcrt_progressive_resolve_tiles_dev", a_rgb_dev, a_weight_dev, 0, b_rgb_dev, b_weight_dev, 0,
                               tile_samples, width, rows, tile, out_rgb_dev, tile_error_dev, tile_sums_dev, frame_error);
+}
+
+int mcrt_render_features_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_t sample_first, uint32_t sample_count,
+                             uint32_t global_seed, int precision, double* features_dev, mcrt_stats* stats)
+{
+    if (!ctx) return MCRT_ERR_INVALID;
+    if (!camera || !features_dev) { ctx->error = "mcrt_render_features_dev: null camera or buffer"; return MCRT_ERR_INVALID; }
+    if (sample_count == 0) { ctx->error = "mcrt_render_features_dev: sample_count is 0"; return MCRT_ERR_INVALID; }
+    if ((uint64_t)sample_first + sample_count > 0x100000000ull)
+    {
+        ctx->error = "mcrt_render_features_dev: sample range beyond 2^32 samples per pixel";
+        return MCRT_ERR_INVALID;
+    }
+    const uint64_t n_pixels = (uint64_t)camera->width * camera->height;
+    if (n_pixels == 0 || n_pixels > 0xFFFFFFFFull) { ctx->error = "mcrt_render_features_dev: empty frame or more than 2^32 pixels"; return MCRT_ERR_INVALID; }
+    if (precision != MCRT_PRECISION_F64 && precision != MCRT_PRECISION_F32) { ctx->error = "unknown precision"; return MCRT_ERR_INVALID; }
+    if (!ctx->has_scene) { ctx->error = "no scene uploaded"; return MCRT_ERR_NO_SCENE; }
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t s = ctx->stream;
+    const int grid = ctx->sm_count * ctx->blocks_per_sm;
+    CK(cudaMemsetAsync(ctx->d_counters, 0, sizeof(Counters), s));
+    CK(cudaEventRecord(ctx->ev_start, s));
+    if (precision == MCRT_PRECISION_F64)
+    {
+        DeviceScene<double> sc = ctx->scene64;
+        if (ctx->exact_traversal) sc.bvh4 = nullptr;
+        Launch<double>::features(sc, deviceCamera<double>(*camera), global_seed, sample_first, sample_count, features_dev,
+                                 ctx->d_counters, grid, s);
+    }
+    else Launch<float>::features(ctx->scene32, deviceCamera<float>(*camera), global_seed, sample_first, sample_count, features_dev,
+                                 ctx->d_counters, grid, s);
+    CK(cudaEventRecord(ctx->ev_stop, s));
+    CK(cudaMemcpyAsync(&ctx->h_counters[0], ctx->d_counters, sizeof(Counters), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    CK(cudaGetLastError());
+    float ms = 0.f;
+    cudaEventElapsedTime(&ms, ctx->ev_start, ctx->ev_stop);
+    fillStats(stats, ctx->h_counters[0], 0, 1, ms);
+    if (ctx->h_counters[0].traversal_overflow) { ctx->error = "traversal stack/heap overflow"; return MCRT_ERR_UNSUPPORTED; }
+    return MCRT_OK;
+}
+
+int mcrt_denoise_dev(mcrt_ctx* ctx, const double* a_rgb_dev, const double* a_weight_dev,
+                     const double* b_rgb_dev, const double* b_weight_dev, const uint32_t* tile_samples,
+                     uint32_t tile, const double* features_dev, uint32_t width, uint32_t height,
+                     const mcrt_denoise_params* params, double* out_rgb_dev, double* frame_error)
+{
+    if (!ctx) return MCRT_ERR_INVALID;
+    if (!a_rgb_dev || !b_rgb_dev || !tile_samples || !features_dev || !out_rgb_dev || !frame_error)
+    {
+        ctx->error = "mcrt_denoise_dev: null buffer";
+        return MCRT_ERR_INVALID;
+    }
+    const uint64_t n_pixels = (uint64_t)width * height;
+    if (n_pixels == 0 || n_pixels > 0xFFFFFFFFull) { ctx->error = "mcrt_denoise_dev: empty frame or more than 2^32 pixels"; return MCRT_ERR_INVALID; }
+    if (tile == 0) { ctx->error = "mcrt_denoise_dev: tile is 0"; return MCRT_ERR_INVALID; }
+    if (!a_weight_dev != !b_weight_dev)
+    {
+        ctx->error = "mcrt_denoise_dev: weight sums must be given for both halves or for neither";
+        return MCRT_ERR_INVALID;
+    }
+    mcrt_denoise_params pr = { MCRT_DENOISE_DEFAULT_ITERATIONS, 0u, MCRT_DENOISE_DEFAULT_SIGMA_COLOR, MCRT_DENOISE_DEFAULT_SIGMA_NORMAL,
+                               MCRT_DENOISE_DEFAULT_SIGMA_DEPTH, MCRT_DENOISE_DEFAULT_SIGMA_ALBEDO };
+    if (params) pr = *params;
+    if (pr.iterations > MCRT_DENOISE_MAX_ITERATIONS) { ctx->error = "mcrt_denoise_dev: more than MCRT_DENOISE_MAX_ITERATIONS iterations"; return MCRT_ERR_INVALID; }
+    for (double sg : { pr.sigma_color, pr.sigma_normal, pr.sigma_depth, pr.sigma_albedo })
+        if (!std::isfinite(sg) || sg < 0.0) { ctx->error = "mcrt_denoise_dev: a sigma is negative or not finite"; return MCRT_ERR_INVALID; }
+    const uint64_t tiles_x = (width + tile - 1) / tile, tiles_y = (height + tile - 1) / tile;
+    const uint64_t n_tiles = tiles_x * tiles_y;
+    for (uint64_t t = 0; t < n_tiles; t++)
+        if (tile_samples[2 * t] == 0 || tile_samples[2 * t + 1] == 0)
+        {
+            ctx->error = "mcrt_denoise_dev: a tile has no samples in one half";
+            return MCRT_ERR_INVALID;
+        }
+    CK(cudaSetDevice(ctx->device));
+    // scratch: the denoiser's, then the tiles' {nA, nB}, then {sum v', sum out^2}
+    const size_t dn_values = denoiseScratchValues((size_t)n_pixels);
+    const size_t scratch_values = dn_values + 2 * n_tiles + 2;
+    if (ctx->denoise_scratch_values < scratch_values)
+    {
+        if (ctx->d_denoise_scratch) cudaFree(ctx->d_denoise_scratch);
+        ctx->d_denoise_scratch = nullptr; ctx->denoise_scratch_values = 0;
+        CK(cudaMalloc((void**)&ctx->d_denoise_scratch, scratch_values * sizeof(double)));
+        ctx->denoise_scratch_values = scratch_values;
+    }
+    double* d_counts = ctx->d_denoise_scratch + dn_values;
+    double* d_sums = d_counts + 2 * n_tiles;
+    const std::vector<double> counts(tile_samples, tile_samples + 2 * n_tiles);
+    cudaStream_t s = ctx->stream;
+    CK(cudaMemcpyAsync(d_counts, counts.data(), counts.size() * sizeof(double), cudaMemcpyHostToDevice, s));
+    CK(cudaMemsetAsync(d_sums, 0, 2 * sizeof(double), s));
+    const DenoiseInput in = { a_rgb_dev, a_weight_dev, b_rgb_dev, b_weight_dev, d_counts, features_dev, width, height, tile, (uint32_t)tiles_x };
+    const DenoiseSigmas sg = { pr.sigma_color, pr.sigma_normal, pr.sigma_depth, pr.sigma_albedo };
+    launchDenoise(in, sg, pr.iterations, ctx->d_denoise_scratch, out_rgb_dev, d_sums, s);
+    double sums[2] = { 0.0, 0.0 };
+    CK(cudaMemcpyAsync(sums, d_sums, sizeof(sums), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    CK(cudaGetLastError());
+    *frame_error = progressiveRelativeError(sums[0], sums[1], true);
+    return MCRT_OK;
 }
 
 int mcrt_film_resolve_dev(mcrt_ctx* ctx, const double* rgb_sum_dev, const double* weight_sum_dev, uint64_t n_pixels, double* out_rgb_dev)

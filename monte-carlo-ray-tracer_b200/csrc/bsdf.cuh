@@ -242,6 +242,54 @@ namespace mcrt
         }
     };
 
+    // Surface::normal(position) and the shading normal: the interpolated vertex normal where the triangle has them, the
+    // face normal where it has none or where the two disagree on the side the ray comes from; both are flipped to face
+    // the ray. -> dot(direction, face normal) before the flip. The same computation as buildInteraction's, kept
+    // separate for k_features: calling it from buildInteraction changed the registers and spills of k_shade and
+    // k_emit_shade (DESIGN.md §3).
+    template <class R>
+    MCRT_D R surfaceNormals(const DeviceScene<R>& sc, const PrimShade<R>& ps, const Hit<R>& hit, const V3<R>& position,
+                            const V3<R>& direction, V3<R>& normal, V3<R>& shading_normal)
+    {
+        if (ps.type == PRIM_TRIANGLE)
+        {
+            normal = V3<R>(ps.nx, ps.ny, ps.nz);
+        }
+        else if (ps.type == PRIM_SPHERE)
+        {
+            const V4<R> g0 = sc.geom[3 * hit.prim];
+            const V4<R> g1 = sc.geom[3 * hit.prim + 1];
+            normal = (position - g0.xyz()) / g1.x;
+        }
+        else
+        {
+            const Quadric<R>& q = sc.quadrics[(uint32_t)sc.geom[3 * hit.prim].x];
+            const V3<R>& p = position;
+            // G * vec4(pos, 1): 4x3 matrix, type_mat4x3.inl:474-477
+            normal = normalize(V3<R>(q.G[0] * p.x + q.G[3] * p.y + q.G[6] * p.z + q.G[9] * R(1),
+                                     q.G[1] * p.x + q.G[4] * p.y + q.G[7] * p.z + q.G[10] * R(1),
+                                     q.G[2] * p.x + q.G[5] * p.y + q.G[8] * p.z + q.G[11] * R(1)));
+        }
+
+        const R cos_theta = dot(direction, normal);
+        shading_normal = normal;
+        if (ps.type == PRIM_TRIANGLE && ps.vn_index >= 0)
+        {
+            const V3<R> n0 = sc.vnormals[3 * ps.vn_index + 0].xyz();
+            const V3<R> nA = sc.vnormals[3 * ps.vn_index + 1].xyz();
+            const V3<R> nB = sc.vnormals[3 * ps.vn_index + 2].xyz();
+            shading_normal = normalize((R(1) - hit.u - hit.v) * n0 + hit.u * nA + hit.v * nB);
+            if ((cos_theta < R(0)) != (dot(direction, shading_normal) < R(0))) shading_normal = normal;
+        }
+
+        if (cos_theta > R(0))
+        {
+            normal = -normal;
+            shading_normal = -shading_normal;
+        }
+        return cos_theta;
+    }
+
     // Interaction::Interaction + selectType. `ray_dir`/`ray_start` are the incoming ray.
     // normal_geo: Surface::normal(position); shading normal resolved by the caller's callback data.
     template <uint32_t FEATS = 0xFFFFFFFFu, class R>

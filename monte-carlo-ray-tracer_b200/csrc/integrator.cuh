@@ -1429,6 +1429,48 @@ namespace mcrt
         flushStats(c, cnt, rays, false, overflow);
     }
 
+    // ------------------------------------------------------------------------------------------
+    // First-hit guides of the denoiser (mcrt_render_features_dev). For samples [sample_first, sample_first +
+    // sample_count) of each pixel, in increasing order, the closest hit of the sample's camera ray adds
+    // {albedo.rgb, shading normal.xyz, t, 1} to out[pixel][8]; a miss adds nothing. Albedo is the specular
+    // reflectance of mirrors and conductors and the reflectance of everything else. One thread owns a pixel and
+    // adds its samples in order, so accumulating consecutive ranges is bit-identical to accumulating their union.
+    template <class R, bool FAST>
+    __global__ void __launch_bounds__(256) k_features(DeviceScene<R> sc, DeviceCamera<R> cam, uint32_t global_seed,
+                                                      uint32_t sample_first, uint32_t sample_count, double* out, Counters* c)
+    {
+        TraceCounters cnt = { 0u, 0u, 0u };
+        uint32_t overflow = 0;
+        unsigned long long rays = 0;
+        const uint32_t n = cam.width * cam.height;
+        for (uint32_t pixel = blockIdx.x * blockDim.x + threadIdx.x; pixel < n; pixel += gridDim.x * blockDim.x)
+        {
+            double* f = out + 8 * (size_t)pixel;
+            double sum[8];
+            for (int k = 0; k < 8; k++) sum[k] = f[k];
+            for (uint32_t k = 0; k < sample_count; k++)
+            {
+                const SamplerState smp = SamplerState::make(global_seed, pixel, sample_first + k, 0u);
+                V3<R> start, direction;
+                cameraRay(cam, sc.scene_ior, pixel, smp, start, direction);
+                const Hit<R> h = traceClosest<PRIMS_ALL, FAST>(sc, start, direction, NO_PRIM, cnt, overflow);
+                rays++;
+                if (h.prim == NO_PRIM) continue;
+                const PrimShade<R> ps = sc.shade[h.prim];
+                const Material<R>& m = sc.materials[ps.material];
+                const V3<R> albedo = (m.flags & (MAT_PERFECT_MIRROR | MAT_COMPLEX_IOR)) ? m.specular_reflectance : m.reflectance;
+                V3<R> normal, shading_normal;
+                surfaceNormals(sc, ps, h, start + direction * h.t, direction, normal, shading_normal);
+                sum[0] += (double)albedo.x; sum[1] += (double)albedo.y; sum[2] += (double)albedo.z;
+                sum[3] += (double)shading_normal.x; sum[4] += (double)shading_normal.y; sum[5] += (double)shading_normal.z;
+                sum[6] += (double)h.t;
+                sum[7] += 1.0;
+            }
+            for (int k = 0; k < 8; k++) f[k] = sum[k];
+        }
+        flushStats(c, cnt, rays, false, overflow);
+    }
+
     // Film::Splat::get for the box filter: mean of the samples, clamped at 0 (film.cpp:106-113)
     // Film::Splat::get with accumulated weights (film.cpp:106-113)
     static __global__ void k_resolve_film_weighted(const double* film, const double* wsum, double* out, size_t n_pixels)

@@ -133,4 +133,14 @@ namespace mcrt
         }
         k_trace_user<MCRT_REAL, false><<<grid, 256, 0, s>>>(sc, rays6, n, out_tuv, out_prim, c);
     }
+    template <> void Launch<MCRT_REAL>::features(const DeviceScene<MCRT_REAL>& sc, const DeviceCamera<MCRT_REAL>& cam, uint32_t global_seed,
+                                                 uint32_t sample_first, uint32_t sample_count, double* out, Counters* c, int grid,
+                                                 cudaStream_t s)
+    {
+        if constexpr (Mode<MCRT_REAL>::parity)
+        {
+            if (sc.bvh4) { k_features<MCRT_REAL, true><<<grid, 256, fastStackSharedBytes(256), s>>>(sc, cam, global_seed, sample_first, sample_count, out, c); return; }
+        }
+        k_features<MCRT_REAL, false><<<grid, 256, 0, s>>>(sc, cam, global_seed, sample_first, sample_count, out, c);
+    }
 }

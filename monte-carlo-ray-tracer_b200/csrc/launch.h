@@ -19,6 +19,8 @@ namespace mcrt
         static void shadeKey(const WaveParams<R>& p, int grid, cudaStream_t s);
         static void traceUser(const DeviceScene<R>& sc, const double* rays6, size_t n, double* out_tuv,
                               uint32_t* out_prim, Counters* c, int grid, cudaStream_t s);
+        static void features(const DeviceScene<R>& sc, const DeviceCamera<R>& cam, uint32_t global_seed, uint32_t sample_first,
+                             uint32_t sample_count, double* out, Counters* c, int grid, cudaStream_t s);
     };
 
     void launchAdvance(Counters* c, cudaStream_t s);
