@@ -434,6 +434,21 @@ int mcrt_progressive_resolve_tiles_dev(mcrt_ctx* ctx, const double* a_rgb_dev, c
 int mcrt_render_features_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_t sample_first, uint32_t sample_count,
                              uint32_t global_seed, int precision, double* features_dev, mcrt_stats* stats);
 
+#define MCRT_FEATURES_MAX_SPECULAR_DEPTH 7
+
+/* mcrt_render_features_dev with the guides taken after perfectly specular bounces, so glass and mirrors are guided by
+ * what they show. Each sample follows its own path, exactly as the path tracer traces it (same sampler dimensions,
+ * IOR history, ray offsets), with throughput T = prod f/pdf and distance L = sum t. A hit on a material without
+ * dirac_delta, the hit at depth specular_depth, or a hit whose sampled bounce is rejected or leaves T at 0 is the end
+ * vertex; it adds {T * albedo, shading normal, L + t, 1} with mcrt_render_features_dev's albedo and normal. A miss
+ * anywhere on the chain adds nothing. No Russian roulette: a pure delta chain this short would not roulette. At
+ * specular_depth 0 the sums are mcrt_render_features_dev's bit for bit; accumulation, order and determinism are the
+ * same. Refuses everything mcrt_render_features_dev refuses, and specular_depth > MCRT_FEATURES_MAX_SPECULAR_DEPTH
+ * (MCRT_ERR_INVALID); a refused call launches nothing. */
+int mcrt_render_features_chain_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_t sample_first, uint32_t sample_count,
+                                   uint32_t global_seed, int precision, uint32_t specular_depth, double* features_dev,
+                                   mcrt_stats* stats);
+
 /* Parameters of mcrt_denoise_dev; a NULL pointer selects the MCRT_DENOISE_DEFAULT_* values. */
 typedef struct mcrt_denoise_params {
     uint32_t iterations;   /* 0..10 a-trous passes of steps 1, 2, 4, ...; 0 = the two halves' plain resolve */

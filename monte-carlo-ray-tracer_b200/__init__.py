@@ -38,7 +38,7 @@ ABI_SYMBOLS = [
     "mcrt_fp64_peak", "mcrt_photon_emit_total", "mcrt_photon_emit_range", "mcrt_photon_build_dev",
     "mcrt_render_accumulate_dev", "mcrt_progressive_resolve_dev",
     "mcrt_render_accumulate_tiles_dev", "mcrt_progressive_resolve_tiles_dev",
-    "mcrt_render_features_dev", "mcrt_denoise_dev",
+    "mcrt_render_features_dev", "mcrt_denoise_dev", "mcrt_render_features_chain_dev",
 ]
 
 
@@ -54,6 +54,7 @@ class DenoiseParams(C.Structure):
 
 # MCRT_DENOISE_DEFAULT_* of mcrt_abi.h
 DENOISE_DEFAULTS = {"iterations": 5, "sigma_color": 1.0, "sigma_normal": 64.0, "sigma_depth": 0.1, "sigma_albedo": 0.1}
+FEATURES_MAX_SPECULAR_DEPTH = 7   # MCRT_FEATURES_MAX_SPECULAR_DEPTH
 
 
 class MaterialRec(C.Structure):
@@ -232,6 +233,8 @@ def lib():
                                                          C.POINTER(C.c_double)]
         L.mcrt_render_features_dev.argtypes = [C.c_void_p, C.POINTER(CameraRec), C.c_uint32, C.c_uint32, C.c_uint32, C.c_int,
                                                C.c_void_p, C.POINTER(Stats)]
+        L.mcrt_render_features_chain_dev.argtypes = [C.c_void_p, C.POINTER(CameraRec), C.c_uint32, C.c_uint32, C.c_uint32, C.c_int,
+                                                     C.c_uint32, C.c_void_p, C.POINTER(Stats)]
         L.mcrt_denoise_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32,
                                        C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(DenoiseParams), C.c_void_p,
                                        C.POINTER(C.c_double)]
@@ -648,13 +651,22 @@ class Integrator:
         return err.value
 
     # -- denoising (see Progressive.denoise)
-    def render_features_dev(self, camera, features_ptr, sample_first, sample_count, precision=None):
+    def render_features_dev(self, camera, features_ptr, sample_first, sample_count, precision=None, specular_depth=0):
         """mcrt_render_features_dev: adds the first-hit guides {albedo.rgb, normal.xyz, t, hits} of samples
-        [sample_first, sample_first + sample_count) of every pixel into device sums [height, width, 8]."""
+        [sample_first, sample_first + sample_count) of every pixel into device sums [height, width, 8].
+        specular_depth > 0 (at most FEATURES_MAX_SPECULAR_DEPTH): mcrt_render_features_chain_dev, the guides of the
+        first vertex after up to that many perfectly specular bounces of each sample's own path, with the albedo
+        weighted by the chain's throughput and the depth measured along the chain."""
         st = Stats()
-        self._check(lib().mcrt_render_features_dev(self.ctx, C.byref(camera.rec), sample_first, sample_count, self.global_seed,
-                                                   self.precision if precision is None else precision,
-                                                   C.c_void_p(features_ptr) if features_ptr else None, C.byref(st)))
+        precision = self.precision if precision is None else precision
+        ptr = C.c_void_p(features_ptr) if features_ptr else None
+        if specular_depth:
+            rc = lib().mcrt_render_features_chain_dev(self.ctx, C.byref(camera.rec), sample_first, sample_count, self.global_seed,
+                                                      precision, specular_depth, ptr, C.byref(st))
+        else:
+            rc = lib().mcrt_render_features_dev(self.ctx, C.byref(camera.rec), sample_first, sample_count, self.global_seed,
+                                                precision, ptr, C.byref(st))
+        self._check(rc)
         self.last_stats = st.as_dict()
         return self.last_stats
 
@@ -1052,7 +1064,7 @@ class Progressive:
         self.tile_counts = np.zeros(grid + (2,), np.int64)          # samples per pixel of each tile in A and B
         self.history = []                                           # one record per render_adaptive pass
         self.stop_reason = None                                     # why the last render_adaptive stopped
-        self._features = None                                       # (samples, device sums [height, width, 8]) of features()
+        self._features = None                                       # ((samples, specular_depth), device sums [height, width, 8]) of features()
 
     @property
     def samples(self):
@@ -1168,22 +1180,25 @@ class Progressive:
         return self.frame()
 
     # -- denoising
-    def _feature_sums(self, samples):
-        """Device feature sums of samples [0, samples), computed once per sample count."""
+    def _feature_sums(self, samples, specular_depth=0):
+        """Device feature sums of samples [0, samples), computed once per (sample count, specular depth)."""
         import torch
-        samples = int(samples)
-        if self._features is None or self._features[0] != samples:
+        key = (int(samples), int(specular_depth))
+        if self._features is None or self._features[0] != key:
             f = torch.zeros((self.camera.height, self.camera.width, 8), dtype=torch.float64, device=self.rgb[0].device)
             torch.cuda.synchronize(f.device)   # the library renders on its own stream
-            self.integrator.render_features_dev(self.camera, f.data_ptr(), 0, samples)
-            self._features = (samples, f)
+            self.integrator.render_features_dev(self.camera, f.data_ptr(), 0, key[0], specular_depth=key[1])
+            self._features = (key, f)
         return self._features[1]
 
-    def features(self, samples=8):
+    def features(self, samples=8, specular_depth=0):
         """First-hit guides of the camera rays of samples [0, samples) of every pixel of the whole frame, as numpy:
         {albedo [H,W,3], normal [H,W,3] (normalised mean, 0 where nothing was hit), depth [H,W] (mean hit distance),
-        coverage [H,W] (hits / samples)}. The device sums are kept and recomputed only when `samples` changes."""
-        f = self._feature_sums(samples).cpu().numpy()
+        coverage [H,W] (hits / samples)}. specular_depth > 0 takes them after up to that many perfectly specular
+        bounces of each sample's path (Integrator.render_features_dev): the albedo is weighted by the chain's
+        throughput and the depth is the distance along the chain. The device sums are kept and recomputed only when
+        `samples` or `specular_depth` changes."""
+        f = self._feature_sums(samples, specular_depth).cpu().numpy()
         hits = f[..., 7]
         with np.errstate(invalid="ignore", divide="ignore"):
             albedo = np.where(hits[..., None] > 0, f[..., 0:3] / hits[..., None], 0.0)
@@ -1193,15 +1208,18 @@ class Progressive:
         return {"albedo": albedo, "normal": normal, "depth": depth, "coverage": hits / float(samples)}
 
     def denoise(self, iterations=None, sigma_color=None, sigma_normal=None, sigma_depth=None, sigma_albedo=None,
-                feature_samples=8):
+                feature_samples=8, specular_depth=0):
         """The frame denoised by the cross-filtered a-trous filter of mcrt_denoise_dev, guided by features(feature_samples)
         -> (frame float64 [H, W, 3], residual error). The error is estimated like error()'s, from the difference of the
         two filtered halves: it measures the remaining noise, not the filter's bias. Arguments left None take the
         defaults of DENOISE_DEFAULTS. Uses the per-tile counts, so it works after adaptive retirement too.
         Raises McrtError unless the row set is the whole frame and every tile has samples in both halves.
+        specular_depth > 0 guides the filter by features(feature_samples, specular_depth), taken after up to that
+        many perfectly specular bounces, so glass and mirrors are guided by what they show; on the H100 measurements
+        of DESIGN.md §6 that did not lower the denoised error at 8 feature samples, which is why 0 stays the default.
 
-        Known limits: the guides come from the first hit only, so glass and mirrors are guided by their own surface,
-        not by what they show; the feature samples [0, F) also feed half A; the Owen-scrambled halves are not
+        Known limits: at specular_depth 0 the guides come from the first hit only, so glass and mirrors are guided by
+        their own surface; rough and glossy lobes are never followed; the feature samples [0, F) also feed half A; the Owen-scrambled halves are not
         independent, so the residual estimate can read about 10 % low."""
         import torch
         if (self.y_first, self.y_step, self.n_rows) != (0, 1, self.camera.height):
@@ -1213,7 +1231,7 @@ class Progressive:
         v = {k: DENOISE_DEFAULTS[k] if x is None else x for k, x in given.items()}
         params = DenoiseParams(int(v["iterations"]), 0, float(v["sigma_color"]), float(v["sigma_normal"]),
                                float(v["sigma_depth"]), float(v["sigma_albedo"]))
-        feats = self._feature_sums(feature_samples)
+        feats = self._feature_sums(feature_samples, specular_depth)
         out = torch.empty_like(self.rgb[0])
         w = (self.wsum[0].data_ptr(), self.wsum[1].data_ptr()) if self.filtered else (None, None)
         err = self.integrator.denoise_dev(self.rgb[0].data_ptr(), w[0], self.rgb[1].data_ptr(), w[1], self.tile_counts, self.tile,

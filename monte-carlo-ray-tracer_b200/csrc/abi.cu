@@ -656,6 +656,12 @@ namespace
         return c;
     }
 
+    // offset of spawned rays along the normal: C::EPSILON in parity mode, scale-aware in fast mode
+    template <class R> R rayEps(const mcrt_ctx* ctx)
+    {
+        return Mode<R>::parity ? (R)1e-9 : (R)(ctx->ray_eps_scale * ctx->scene_scale);
+    }
+
     // Accumulate mode of runWavefront: the samples are added into the caller's device sums, which are neither
     // zeroed before the render nor resolved after it (mcrt_render_accumulate_dev, mcrt_render_film_sums_strided_dev).
     struct FilmSums
@@ -745,7 +751,7 @@ namespace
         p.row_step = row_step;
         p.n_pixels = n_pixels;
         p.integrator = (uint32_t)integrator;
-        p.ray_eps = Mode<R>::parity ? (R)1e-9 : (R)(ctx->ray_eps_scale * ctx->scene_scale);
+        p.ray_eps = rayEps<R>(ctx);
         std::memset(&p.sort, 0, sizeof(p.sort));
         if (ctx->sort_rays)
         {
@@ -1843,44 +1849,79 @@ int mcrt_progressive_resolve_tiles_dev(mcrt_ctx* ctx, const double* a_rgb_dev, c
                               tile_samples, width, rows, tile, out_rgb_dev, tile_error_dev, tile_sums_dev, frame_error);
 }
 
+static_assert(MCRT_FEATURES_MAX_SPECULAR_DEPTH + 1 <= IOR_STACK_CAPACITY, "a guide chain must not overflow the IOR stack");
+
+namespace
+{
+    // mcrt_render_features_dev (specular_depth 0: the first-hit kernel) and mcrt_render_features_chain_dev
+    int renderFeatures(const char* fn, mcrt_ctx* ctx, const mcrt_camera* camera, uint32_t sample_first, uint32_t sample_count,
+                       uint32_t global_seed, int precision, uint32_t specular_depth, double* features_dev, mcrt_stats* stats)
+    {
+        if (!ctx) return MCRT_ERR_INVALID;
+        const std::string f = fn;
+        if (!camera || !features_dev) { ctx->error = f + ": null camera or buffer"; return MCRT_ERR_INVALID; }
+        if (sample_count == 0) { ctx->error = f + ": sample_count is 0"; return MCRT_ERR_INVALID; }
+        if ((uint64_t)sample_first + sample_count > 0x100000000ull)
+        {
+            ctx->error = f + ": sample range beyond 2^32 samples per pixel";
+            return MCRT_ERR_INVALID;
+        }
+        const uint64_t n_pixels = (uint64_t)camera->width * camera->height;
+        if (n_pixels == 0 || n_pixels > 0xFFFFFFFFull) { ctx->error = f + ": empty frame or more than 2^32 pixels"; return MCRT_ERR_INVALID; }
+        if (precision != MCRT_PRECISION_F64 && precision != MCRT_PRECISION_F32) { ctx->error = "unknown precision"; return MCRT_ERR_INVALID; }
+        if (specular_depth > MCRT_FEATURES_MAX_SPECULAR_DEPTH)
+        {
+            ctx->error = f + ": specular_depth above MCRT_FEATURES_MAX_SPECULAR_DEPTH";
+            return MCRT_ERR_INVALID;
+        }
+        if (!ctx->has_scene) { ctx->error = "no scene uploaded"; return MCRT_ERR_NO_SCENE; }
+        CK(cudaSetDevice(ctx->device));
+        cudaStream_t s = ctx->stream;
+        const int grid = ctx->sm_count * ctx->blocks_per_sm;
+        CK(cudaMemsetAsync(ctx->d_counters, 0, sizeof(Counters), s));
+        CK(cudaEventRecord(ctx->ev_start, s));
+        if (precision == MCRT_PRECISION_F64)
+        {
+            DeviceScene<double> sc = ctx->scene64;
+            if (ctx->exact_traversal) sc.bvh4 = nullptr;
+            if (specular_depth == 0)
+                Launch<double>::features(sc, deviceCamera<double>(*camera), global_seed, sample_first, sample_count, features_dev,
+                                         ctx->d_counters, grid, s);
+            else
+                Launch<double>::featuresChain(sc, deviceCamera<double>(*camera), global_seed, sample_first, sample_count, specular_depth,
+                                              rayEps<double>(ctx), features_dev, ctx->d_counters, grid, s);
+        }
+        else if (specular_depth == 0)
+            Launch<float>::features(ctx->scene32, deviceCamera<float>(*camera), global_seed, sample_first, sample_count, features_dev,
+                                    ctx->d_counters, grid, s);
+        else
+            Launch<float>::featuresChain(ctx->scene32, deviceCamera<float>(*camera), global_seed, sample_first, sample_count, specular_depth,
+                                         rayEps<float>(ctx), features_dev, ctx->d_counters, grid, s);
+        CK(cudaEventRecord(ctx->ev_stop, s));
+        CK(cudaMemcpyAsync(&ctx->h_counters[0], ctx->d_counters, sizeof(Counters), cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        CK(cudaGetLastError());
+        float ms = 0.f;
+        cudaEventElapsedTime(&ms, ctx->ev_start, ctx->ev_stop);
+        fillStats(stats, ctx->h_counters[0], 0, 1, ms);
+        if (ctx->h_counters[0].traversal_overflow) { ctx->error = "traversal stack/heap overflow"; return MCRT_ERR_UNSUPPORTED; }
+        return MCRT_OK;
+    }
+}
+
 int mcrt_render_features_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_t sample_first, uint32_t sample_count,
                              uint32_t global_seed, int precision, double* features_dev, mcrt_stats* stats)
 {
-    if (!ctx) return MCRT_ERR_INVALID;
-    if (!camera || !features_dev) { ctx->error = "mcrt_render_features_dev: null camera or buffer"; return MCRT_ERR_INVALID; }
-    if (sample_count == 0) { ctx->error = "mcrt_render_features_dev: sample_count is 0"; return MCRT_ERR_INVALID; }
-    if ((uint64_t)sample_first + sample_count > 0x100000000ull)
-    {
-        ctx->error = "mcrt_render_features_dev: sample range beyond 2^32 samples per pixel";
-        return MCRT_ERR_INVALID;
-    }
-    const uint64_t n_pixels = (uint64_t)camera->width * camera->height;
-    if (n_pixels == 0 || n_pixels > 0xFFFFFFFFull) { ctx->error = "mcrt_render_features_dev: empty frame or more than 2^32 pixels"; return MCRT_ERR_INVALID; }
-    if (precision != MCRT_PRECISION_F64 && precision != MCRT_PRECISION_F32) { ctx->error = "unknown precision"; return MCRT_ERR_INVALID; }
-    if (!ctx->has_scene) { ctx->error = "no scene uploaded"; return MCRT_ERR_NO_SCENE; }
-    CK(cudaSetDevice(ctx->device));
-    cudaStream_t s = ctx->stream;
-    const int grid = ctx->sm_count * ctx->blocks_per_sm;
-    CK(cudaMemsetAsync(ctx->d_counters, 0, sizeof(Counters), s));
-    CK(cudaEventRecord(ctx->ev_start, s));
-    if (precision == MCRT_PRECISION_F64)
-    {
-        DeviceScene<double> sc = ctx->scene64;
-        if (ctx->exact_traversal) sc.bvh4 = nullptr;
-        Launch<double>::features(sc, deviceCamera<double>(*camera), global_seed, sample_first, sample_count, features_dev,
-                                 ctx->d_counters, grid, s);
-    }
-    else Launch<float>::features(ctx->scene32, deviceCamera<float>(*camera), global_seed, sample_first, sample_count, features_dev,
-                                 ctx->d_counters, grid, s);
-    CK(cudaEventRecord(ctx->ev_stop, s));
-    CK(cudaMemcpyAsync(&ctx->h_counters[0], ctx->d_counters, sizeof(Counters), cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    CK(cudaGetLastError());
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, ctx->ev_start, ctx->ev_stop);
-    fillStats(stats, ctx->h_counters[0], 0, 1, ms);
-    if (ctx->h_counters[0].traversal_overflow) { ctx->error = "traversal stack/heap overflow"; return MCRT_ERR_UNSUPPORTED; }
-    return MCRT_OK;
+    return renderFeatures("mcrt_render_features_dev", ctx, camera, sample_first, sample_count, global_seed, precision, 0u,
+                          features_dev, stats);
+}
+
+int mcrt_render_features_chain_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_t sample_first, uint32_t sample_count,
+                                   uint32_t global_seed, int precision, uint32_t specular_depth, double* features_dev,
+                                   mcrt_stats* stats)
+{
+    return renderFeatures("mcrt_render_features_chain_dev", ctx, camera, sample_first, sample_count, global_seed, precision,
+                          specular_depth, features_dev, stats);
 }
 
 int mcrt_denoise_dev(mcrt_ctx* ctx, const double* a_rgb_dev, const double* a_weight_dev,

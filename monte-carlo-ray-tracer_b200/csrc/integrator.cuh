@@ -1471,6 +1471,101 @@ namespace mcrt
         flushStats(c, cnt, rays, false, overflow);
     }
 
+    // Guides after perfectly specular bounces (mcrt_render_features_chain_dev). Each sample follows its own path,
+    // exactly as k_generate / k_shade trace it, through at most `specular_depth` hits on MAT_DIRAC_DELTA materials,
+    // with throughput T = prod f/pdf and distance L = sum t. The first hit on any other material, the hit at the
+    // depth cap, or a hit whose sampleBSDF rejects the direction or leaves T at 0, is the end vertex: it adds
+    // {T * albedo, shading normal, L + t, 1}, with k_features' albedo and normal. A miss adds nothing. At depth 0 this
+    // is k_features' sum bit for bit. A pure delta chain has diffuse_depth 0 and depth < 16, so the path would not
+    // roulette there. Each continued vertex pushes at most one IOR, so a depth of at most IOR_STACK_CAPACITY - 1
+    // (MCRT_FEATURES_MAX_SPECULAR_DEPTH, checked in abi.cu) cannot overflow the IOR stack.
+
+    template <class R, bool FAST>
+    __global__ void __launch_bounds__(256) k_features_chain(DeviceScene<R> sc, DeviceCamera<R> cam, uint32_t global_seed,
+                                                            uint32_t sample_first, uint32_t sample_count, uint32_t specular_depth,
+                                                            R ray_eps, double* out, Counters* c)
+    {
+        TraceCounters cnt = { 0u, 0u, 0u };
+        uint32_t overflow = 0;
+        unsigned long long rays = 0;
+        const uint32_t n = cam.width * cam.height;
+        for (uint32_t pixel = blockIdx.x * blockDim.x + threadIdx.x; pixel < n; pixel += gridDim.x * blockDim.x)
+        {
+            double* f = out + 8 * (size_t)pixel;
+            double sum[8];
+            for (int k = 0; k < 8; k++) sum[k] = f[k];
+            for (uint32_t k = 0; k < sample_count; k++)
+            {
+                const uint32_t sample = sample_first + k;
+                PathRay<R> ray;
+                cameraRay(cam, sc.scene_ior, pixel, SamplerState::make(global_seed, pixel, sample, 0u), ray.start, ray.direction);
+                ray.medium_ior = sc.scene_ior; ray.refraction_scale = R(1);
+                ray.depth = 0u; ray.diffuse_depth = 0u; ray.refraction_level = 0;
+                ray.dirac_delta = false; ray.refraction = false;
+                R iors[IOR_STACK_CAPACITY];
+                iors[0] = sc.scene_ior;
+                uint32_t ior_count = 1, skip = NO_PRIM;
+                V3<R> throughput(R(1), R(1), R(1));
+                R distance = R(0);
+                for (uint32_t depth = 0;; depth++)
+                {
+                    const Hit<R> h = traceClosest<PRIMS_ALL, FAST>(sc, ray.start, ray.direction, skip, cnt, overflow);
+                    rays++;
+                    if (h.prim == NO_PRIM) break;
+                    const PrimShade<R> ps = sc.shade[h.prim];
+                    const Material<R>& m = sc.materials[ps.material];
+                    if (depth < specular_depth && (m.flags & MAT_DIRAC_DELTA))
+                    {
+                        // k_shade's bounce at this depth: RefractionHistory::externalIOR, Interaction, sampleBSDF
+                        const SamplerState smp = SamplerState::make(global_seed, pixel, sample, depth + 1u);
+                        int ext_idx = ray.refraction_level - 1;
+                        ext_idx = ext_idx < 0 ? 0 : (ext_idx > (int)ior_count - 1 ? (int)ior_count - 1 : ext_idx);
+                        Interaction<R> ia;
+                        buildInteraction<SHADE_FEATS_ALL>(ia, sc, h, ray, iors[ext_idx], smp);
+                        PathRay<R> nray;
+                        V3<R> bsdf_absIdotN;
+                        R pdf;
+                        if (sampleBSDF(ia, ray, smp, ray_eps, false, bsdf_absIdotN, pdf, nray))
+                        {
+                            const V3<R> next_throughput = throughput * (bsdf_absIdotN / pdf);
+                            if (compMax(next_throughput) != R(0))
+                            {
+                                throughput = next_throughput;
+                                distance += h.t;
+                                // RefractionHistory::update, ray.cpp:80-93
+                                if (nray.refraction_level > 0)
+                                {
+                                    if (nray.refraction_level == (int32_t)ior_count)
+                                    {
+                                        if (ior_count < (uint32_t)IOR_STACK_CAPACITY) iors[ior_count++] = nray.medium_ior;
+                                    }
+                                    else if (nray.refraction_level < (int32_t)ior_count - 1)
+                                    {
+                                        ior_count--;
+                                    }
+                                }
+                                skip = ps.type == PRIM_TRIANGLE ? h.prim : NO_PRIM;   // the source primitive (fast mode)
+                                ray = nray;
+                                ray.refraction = false;
+                                continue;
+                            }
+                        }
+                    }
+                    const V3<R> albedo = throughput * ((m.flags & (MAT_PERFECT_MIRROR | MAT_COMPLEX_IOR)) ? m.specular_reflectance : m.reflectance);
+                    V3<R> normal, shading_normal;
+                    surfaceNormals(sc, ps, h, ray.start + ray.direction * h.t, ray.direction, normal, shading_normal);
+                    sum[0] += (double)albedo.x; sum[1] += (double)albedo.y; sum[2] += (double)albedo.z;
+                    sum[3] += (double)shading_normal.x; sum[4] += (double)shading_normal.y; sum[5] += (double)shading_normal.z;
+                    sum[6] += (double)(distance + h.t);
+                    sum[7] += 1.0;
+                    break;
+                }
+            }
+            for (int k = 0; k < 8; k++) f[k] = sum[k];
+        }
+        flushStats(c, cnt, rays, false, overflow);
+    }
+
     // Film::Splat::get for the box filter: mean of the samples, clamped at 0 (film.cpp:106-113)
     // Film::Splat::get with accumulated weights (film.cpp:106-113)
     static __global__ void k_resolve_film_weighted(const double* film, const double* wsum, double* out, size_t n_pixels)

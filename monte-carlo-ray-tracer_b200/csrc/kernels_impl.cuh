@@ -143,4 +143,19 @@ namespace mcrt
         }
         k_features<MCRT_REAL, false><<<grid, 256, 0, s>>>(sc, cam, global_seed, sample_first, sample_count, out, c);
     }
+    template <> void Launch<MCRT_REAL>::featuresChain(const DeviceScene<MCRT_REAL>& sc, const DeviceCamera<MCRT_REAL>& cam, uint32_t global_seed,
+                                                      uint32_t sample_first, uint32_t sample_count, uint32_t specular_depth,
+                                                      MCRT_REAL ray_eps, double* out, Counters* c, int grid, cudaStream_t s)
+    {
+        if constexpr (Mode<MCRT_REAL>::parity)
+        {
+            if (sc.bvh4)
+            {
+                k_features_chain<MCRT_REAL, true><<<grid, 256, fastStackSharedBytes(256), s>>>(sc, cam, global_seed, sample_first, sample_count,
+                                                                                              specular_depth, ray_eps, out, c);
+                return;
+            }
+        }
+        k_features_chain<MCRT_REAL, false><<<grid, 256, 0, s>>>(sc, cam, global_seed, sample_first, sample_count, specular_depth, ray_eps, out, c);
+    }
 }

@@ -21,6 +21,9 @@ namespace mcrt
                               uint32_t* out_prim, Counters* c, int grid, cudaStream_t s);
         static void features(const DeviceScene<R>& sc, const DeviceCamera<R>& cam, uint32_t global_seed, uint32_t sample_first,
                              uint32_t sample_count, double* out, Counters* c, int grid, cudaStream_t s);
+        static void featuresChain(const DeviceScene<R>& sc, const DeviceCamera<R>& cam, uint32_t global_seed, uint32_t sample_first,
+                                  uint32_t sample_count, uint32_t specular_depth, R ray_eps, double* out, Counters* c, int grid,
+                                  cudaStream_t s);
     };
 
     void launchAdvance(Counters* c, cudaStream_t s);

@@ -2,7 +2,7 @@
 """Cost and benefit of the denoiser on the C2 workload of bench.py (hexagon_room, 1920x1080, parity mode, 32 Mi-path
 pool).
 
-  python tools/denoise_bench.py [--reps 20] [--ref-spp 1024] [--out result.json]
+  python tools/denoise_bench.py [--reps 20] [--ref-spp 1024] [--specular-depth 0,1,2,4] [--out result.json]
 
 Reported: the device time of the feature pass at 8 spp (CUDA events of mcrt_render_features_dev); the device time of
 mcrt_denoise_dev at the default parameters (CUDA events around the call, median of --reps) and per kernel
@@ -12,7 +12,11 @@ Equal-error comparison: noisy frames at 16, 32 and 64 spp with seed s1 and a ref
 relative error sqrt(sum (I - R)^2 / sum R^2) of each noisy and denoised frame against the reference, the denoised
 residual estimate beside it (it sees noise, not the filter's bias), and the spp a noisy render needs to match the
 denoised 16-spp frame, interpolated in log-log between the measured spp. The reference's own noise is included in
-every measured error; it is reported as the reference's two-half estimate."""
+every measured error; it is reported as the reference's two-half estimate.
+
+--specular-depth D1,D2,...: guides taken after up to D perfectly specular bounces (Progressive.denoise(specular_depth=D)).
+For each D, the feature pass at 8 spp is timed and every spp row also reports the denoised error over the pixels whose
+first hit is a dirac_delta material (the ray through the pixel's centre), beside the whole frame's."""
 import argparse
 import importlib
 import json
@@ -37,14 +41,33 @@ def gpu_info():
         return f"nvidia-smi unavailable: {e}"
 
 
+def delta_first_hit(m, tracer, scene, cam):
+    """[H, W] True where the ray through the pixel's centre first hits a dirac_delta material."""
+    r = cam.rec
+    fwd, left, up = (np.array(v[:3]) for v in (r.forward, r.left, r.up))
+    x, y = np.meshgrid(np.arange(cam.width) + 0.5, np.arange(cam.height) + 0.5)
+    size = r.sensor_width / cam.width
+    d = fwd * r.focal_length + left * (size * (cam.width * 0.5 - x))[..., None] + up * (size * (cam.height * 0.5 - y))[..., None]
+    d /= np.linalg.norm(d, axis=-1, keepdims=True)
+    rays = np.concatenate([np.broadcast_to(np.array(r.eye[:3]), d.shape), d], -1).reshape(-1, 6)
+    prim = tracer.intersect(rays)["prim"]
+    a = scene.a
+    hit = prim != m.NO_PRIM
+    out = np.zeros(len(prim), bool)
+    out[hit] = a["materials"]["dirac_delta"][a["prim_material"][prim[hit].astype(np.int64)]] != 0
+    return out.reshape(cam.height, cam.width)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--ref-spp", type=int, default=1024)
     ap.add_argument("--width", type=int, default=1920)
     ap.add_argument("--height", type=int, default=1080)
+    ap.add_argument("--specular-depth", default="0", help="comma-separated guide depths")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
+    depths = [int(d) for d in args.specular_depth.split(",")]
     import torch
     m = importlib.import_module("monte-carlo-ray-tracer_b200")
     scene = m.Scene.from_pack(os.path.join(ROOT, "bench_data", "c2_hexagon_room.mcrtpack"))
@@ -61,8 +84,12 @@ def main():
     ref = ref_prog.frame()
     result["reference"] = {"spp": args.ref_spp, "estimate": ref_prog.error()[0]}
 
-    def rel(x):
-        return float(np.sqrt(np.sum((x - ref) ** 2) / np.sum(ref ** 2)))
+    mask = delta_first_hit(m, tracers[S1], scene, cam)
+    result["delta_first_hit_share"] = float(mask.mean())
+
+    def rel(x, where=None):
+        where = np.ones(mask.shape, bool) if where is None else where
+        return float(np.sqrt(np.sum((x - ref)[where] ** 2) / np.sum(ref[where] ** 2)))
 
     prog = m.Progressive(tracers[S1], cam)
     rows = []
@@ -71,7 +98,12 @@ def main():
         prog.add(pass_spp // 2); prog.add(pass_spp - pass_spp // 2)
         dn, estimate = prog.denoise()
         rows.append({"spp": spp, "noisy": rel(prog.frame()), "noisy_estimate": prog.error()[0], "denoised": rel(dn),
-                     "denoised_estimate": estimate})
+                     "denoised_estimate": estimate, "noisy_delta": rel(prog.frame(), mask)})
+        if depths != [0]:
+            rows[-1]["by_specular_depth"] = {}
+            for d in depths:
+                dnd, _ = prog.denoise(specular_depth=d)
+                rows[-1]["by_specular_depth"][d] = {"denoised": rel(dnd), "denoised_delta": rel(dnd, mask)}
         print(json.dumps(rows[-1]), flush=True)
     result["quality"] = rows
     # spp at which a noisy render matches denoised 16 spp (log-log interpolation / extrapolation over 16..64)
@@ -88,6 +120,16 @@ def main():
         f.zero_(); torch.cuda.synchronize()
         feat_ms.append(tracers[S1].render_features_dev(cam, f.data_ptr(), 0, 8)["gpu_ms_total"])
     result["feature_pass_8spp_ms"] = float(np.median(feat_ms))
+    if depths != [0]:
+        result["feature_pass_8spp_ms_by_specular_depth"] = {}
+        for d in depths:
+            ms = []
+            for _ in range(3):
+                f.zero_(); torch.cuda.synchronize()
+                ms.append(tracers[S1].render_features_dev(cam, f.data_ptr(), 0, 8, specular_depth=d)["gpu_ms_total"])
+            result["feature_pass_8spp_ms_by_specular_depth"][d] = float(np.median(ms))
+        f.zero_(); torch.cuda.synchronize()
+        tracers[S1].render_features_dev(cam, f.data_ptr(), 0, 8)   # the denoiser timing below uses the first-hit guides
 
     # denoiser: CUDA events around the call (the library's stream is synchronised inside the call)
     ptl = tracers[S1]
