@@ -29,7 +29,10 @@ def test_struct_layouts_match_header(mcrt):
 
 @pytest.mark.parametrize("cid", golden_cases())
 def test_scene_pack_is_consistent(cid, mcrt):
-    scene = mcrt.Scene.from_pack(os.path.join(GOLDEN, cid + ".mcrtpack"))
+    check_scene_is_consistent(mcrt, mcrt.Scene.from_pack(os.path.join(GOLDEN, cid + ".mcrtpack")))
+
+
+def check_scene_is_consistent(mcrt, scene):
     a = scene.a
     n = scene.n_prims
     assert n > 0 and a["prim_index"].size == n and a["prim_material"].size == n and a["prim_area"].size == n

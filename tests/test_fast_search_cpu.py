@@ -15,6 +15,42 @@ from oracle import port
 CASES = [c for c in golden_cases() if c != "ior_test_nobvh_64" and not c.startswith("pm_")]
 
 
+def search_rays(mcrt, ps, base, rng, n=20000):
+    """base rays, segments from surface to surface, rays leaving surfaces and axis-parallel rays (the last 600)."""
+    ref0 = ps.trace(base)
+    ok = ref0["prim"] != mcrt.NO_PRIM
+    pts = base[ok, :3] + base[ok, 3:] * ref0["t"][ok, None]
+    a = pts[rng.integers(0, len(pts), n)]
+    b = pts[rng.integers(0, len(pts), n)] + rng.normal(0, 1e-3, (n, 3))
+    d = b - a
+    nrm = np.linalg.norm(d, axis=1, keepdims=True)
+    keep = nrm[:, 0] > 1e-9
+    seg = np.concatenate([a[keep], d[keep] / nrm[keep]], axis=1)              # start exactly on surfaces, aim at surfaces
+    d2 = rng.normal(size=(n, 3)); d2 /= np.linalg.norm(d2, axis=1, keepdims=True)
+    leave = np.concatenate([a + 1e-9 * d2, d2], axis=1)                        # leave surfaces in random directions
+    axis = np.zeros((600, 6)); axis[:, :3] = pts[rng.integers(0, len(pts), 600)] + rng.normal(0, 0.3, (600, 3))
+    axis[np.arange(600), 3 + np.arange(600) % 3] = np.where(np.arange(600) % 2, 1.0, -1.0)   # axis-parallel rays: 1/d = inf in the reference
+    return np.concatenate([base, seg, leave, axis], axis=0)
+
+
+def check_unflagged_answers(mcrt, ps, nodes, rays, max_flagged=0.02):
+    """Every answer of the order-free search that is not flagged equals the reference-order answer; rays with a zero direction
+    component (the last 600 of search_rays) are always flagged, other flags are rare and never on a miss. -> (reference hits, flags)"""
+    scene = ps.scene
+    scale = float(np.float32(np.abs(scene.a["node_bounds"][:6]).max()))      # ctx->scene_scale (float) as mcrt_scene_upload computes it
+    ref = ps.trace(rays)
+    fast, flagged, box, prim = ps.trace_fast(nodes, scale, rays)
+    final = ~flagged
+    for f in ("prim", "t", "u", "v", "interpolate"):
+        assert np.array_equal(fast[f][final], ref[f][final]), (f, int((fast[f][final] != ref[f][final]).sum()))
+    generic = np.ones(len(rays), dtype=bool); generic[-600:] = False          # rays with a zero direction component always go to the replay
+    assert flagged[~generic].all()
+    assert flagged[generic].mean() < max_flagged, flagged[generic].mean()
+    assert not flagged[generic & (ref["prim"] == mcrt.NO_PRIM)].any()          # a generic miss is never ambiguous
+    assert box > 0 and prim > 0
+    return ref, flagged
+
+
 @pytest.mark.parametrize("max_leaf", [0xFFFFFFFF, 0])
 @pytest.mark.parametrize("cid", CASES)
 def test_unflagged_answers_equal_reference_order(cid, max_leaf, mcrt):
@@ -22,35 +58,8 @@ def test_unflagged_answers_equal_reference_order(cid, max_leaf, mcrt):
     g = np.load(os.path.join(GOLDEN, cid + ".npz"))
     ps = port.PortScene(scene)
     try:
-        nodes = mcrt.bvh4_host(scene, max_leaf)
-        scale = float(np.float32(np.abs(scene.a["node_bounds"][:6]).max()))      # ctx->scene_scale (float) as mcrt_scene_upload computes it
-        rng = np.random.default_rng(3)
-        base = g["tr_rays"]
-        ref0 = ps.trace(base)
-        ok = ref0["prim"] != mcrt.NO_PRIM
-        pts = base[ok, :3] + base[ok, 3:] * ref0["t"][ok, None]
-        n = 20000
-        a = pts[rng.integers(0, len(pts), n)]
-        b = pts[rng.integers(0, len(pts), n)] + rng.normal(0, 1e-3, (n, 3))
-        d = b - a
-        nrm = np.linalg.norm(d, axis=1, keepdims=True)
-        keep = nrm[:, 0] > 1e-9
-        seg = np.concatenate([a[keep], d[keep] / nrm[keep]], axis=1)              # start exactly on surfaces, aim at surfaces
-        d2 = rng.normal(size=(n, 3)); d2 /= np.linalg.norm(d2, axis=1, keepdims=True)
-        leave = np.concatenate([a + 1e-9 * d2, d2], axis=1)                        # leave surfaces in random directions
-        axis = np.zeros((600, 6)); axis[:, :3] = pts[rng.integers(0, len(pts), 600)] + rng.normal(0, 0.3, (600, 3))
-        axis[np.arange(600), 3 + np.arange(600) % 3] = np.where(np.arange(600) % 2, 1.0, -1.0)   # axis-parallel rays: 1/d = inf in the reference
-        rays = np.concatenate([base, seg, leave, axis], axis=0)
-        ref = ps.trace(rays)
-        fast, flagged, box, prim = ps.trace_fast(nodes, scale, rays)
-        final = ~flagged
-        for f in ("prim", "t", "u", "v", "interpolate"):
-            assert np.array_equal(fast[f][final], ref[f][final]), (cid, f, int((fast[f][final] != ref[f][final]).sum()))
-        generic = np.ones(len(rays), dtype=bool); generic[-len(axis):] = False    # rays with a zero direction component always go to the replay
-        assert flagged[~generic].all()
-        assert flagged[generic].mean() < 0.02, flagged[generic].mean()
-        assert not flagged[generic & (ref["prim"] == mcrt.NO_PRIM)].any()          # a generic miss is never ambiguous
-        assert box > 0 and prim > 0
+        rays = search_rays(mcrt, ps, g["tr_rays"], np.random.default_rng(3))
+        check_unflagged_answers(mcrt, ps, mcrt.bvh4_host(scene, max_leaf), rays)
     finally:
         ps.close()
 
@@ -131,41 +140,45 @@ def test_occlusion_query_equals_closest_hit_comparison(cid, mcrt):
     g = np.load(os.path.join(GOLDEN, cid + ".npz"))
     ps = port.PortScene(scene)
     try:
-        nodes = mcrt.bvh4_host(scene)
-        scale = float(np.float32(np.abs(scene.a["node_bounds"][:6]).max()))
-        rng = np.random.default_rng(21)
-        base = g["tr_rays"]
-        ref0 = ps.trace(base)
-        ok = ref0["prim"] != mcrt.NO_PRIM
-        pts = base[ok, :3] + base[ok, 3:] * ref0["t"][ok, None]
-        lights = scene.a["light_prim"]
-        assert len(lights) > 0
-        n = 30000
-        tgt = lights[rng.integers(0, len(lights), n)].astype(np.uint32)
-        # a point on each target light: triangle lights by barycentric sampling, sphere lights through their centre
-        a = scene.a
-        lp = np.zeros((n, 3))
-        for j in range(n):
-            t, idx = int(a["prim_type"][tgt[j]]), int(a["prim_index"][tgt[j]])
-            if t == 0:
-                u, v = rng.uniform(0, 1, 2); su = np.sqrt(u)
-                lp[j] = ((1 - su) * a["tri_v0"].reshape(-1, 3)[idx] + (1 - v) * su * a["tri_v1"].reshape(-1, 3)[idx] + v * su * a["tri_v2"].reshape(-1, 3)[idx])
-            else:
-                lp[j] = a["sphere_origin_radius"].reshape(-1, 4)[idx][:3]
-        o = pts[rng.integers(0, len(pts), n)]
-        d = lp - o
-        nrm = np.linalg.norm(d, axis=1, keepdims=True)
-        keep = nrm[:, 0] > 1e-9
-        rays = np.concatenate([o[keep], d[keep] / nrm[keep]], axis=1)
-        tgt = tgt[keep]
-        ref = ps.trace(rays)
-        verdict, t = ps.trace_visible(nodes, scale, rays, tgt)
-        vis, occ = verdict == 0, verdict == 1
-        assert np.array_equal(ref["prim"][vis], tgt[vis]) and np.array_equal(ref["t"][vis], t[vis])
-        assert (ref["prim"][occ] != tgt[occ]).all()
-        assert vis.sum() > 100 and occ.sum() > 100 and (verdict == 2).mean() < 0.02
+        check_occlusion_query(mcrt, ps, mcrt.bvh4_host(scene), g["tr_rays"], np.random.default_rng(21))
     finally:
         ps.close()
+
+
+def check_occlusion_query(mcrt, ps, nodes, base, rng, n=30000):
+    """Rays from surface points (where `base` rays hit) to points on random lights: the occlusion query's verdict against the
+    reference-order closest hit. -> verdicts"""
+    scene = ps.scene
+    scale = float(np.float32(np.abs(scene.a["node_bounds"][:6]).max()))
+    ref0 = ps.trace(base)
+    ok = ref0["prim"] != mcrt.NO_PRIM
+    pts = base[ok, :3] + base[ok, 3:] * ref0["t"][ok, None]
+    lights = scene.a["light_prim"]
+    assert len(lights) > 0
+    tgt = lights[rng.integers(0, len(lights), n)].astype(np.uint32)
+    # a point on each target light: triangle lights by barycentric sampling, sphere lights through their centre
+    a = scene.a
+    lp = np.zeros((n, 3))
+    for j in range(n):
+        t, idx = int(a["prim_type"][tgt[j]]), int(a["prim_index"][tgt[j]])
+        if t == 0:
+            u, v = rng.uniform(0, 1, 2); su = np.sqrt(u)
+            lp[j] = ((1 - su) * a["tri_v0"].reshape(-1, 3)[idx] + (1 - v) * su * a["tri_v1"].reshape(-1, 3)[idx] + v * su * a["tri_v2"].reshape(-1, 3)[idx])
+        else:
+            lp[j] = a["sphere_origin_radius"].reshape(-1, 4)[idx][:3]
+    o = pts[rng.integers(0, len(pts), n)]
+    d = lp - o
+    nrm = np.linalg.norm(d, axis=1, keepdims=True)
+    keep = nrm[:, 0] > 1e-9
+    rays = np.concatenate([o[keep], d[keep] / nrm[keep]], axis=1)
+    tgt = tgt[keep]
+    ref = ps.trace(rays)
+    verdict, t = ps.trace_visible(nodes, scale, rays, tgt)
+    vis, occ = verdict == 0, verdict == 1
+    assert np.array_equal(ref["prim"][vis], tgt[vis]) and np.array_equal(ref["t"][vis], t[vis])
+    assert (ref["prim"][occ] != tgt[occ]).all()
+    assert vis.sum() > 100 and occ.sum() > 100 and (verdict == 2).mean() < 0.02
+    return verdict
 
 
 def _unit(v):
