@@ -247,6 +247,32 @@ int mcrt_photon_emit_range(mcrt_ctx* ctx, const mcrt_photon_emit_params* params,
 int mcrt_photon_build_dev(mcrt_ctx* ctx, const mcrt_photon_emit_params* params, const float* caustic_dev,
                           uint64_t n_caustic, const float* global_dev, uint64_t n_global, double* build_ms);
 
+/* One pass of progressive photon mapping (Knaus & Zwicker, "Progressive photon mapping: a probabilistic
+ * approach", TOG 2011): mcrt_photon_emit, except that light l's emissions are the reference's emission
+ * indices [pass * n_l, (pass + 1) * n_l), n_l being its count in the emission plan. The photon flux stays
+ * light_flux / n_l, so every pass map is a complete map on its own; the index offset continues each light's
+ * Owen-scrambled Sobol sequence, so passes stay stratified against each other, and passes 0..P-1 hold the
+ * photons of one mcrt_photon_emit whose per-light counts are P * n_l (with 1/P of their flux). Pass 0 is
+ * mcrt_photon_emit. MCRT_ERR_INVALID when (pass + 1) * n_l exceeds 2^32 for a light (the sample index is
+ * 32 bits). */
+int mcrt_photon_emit_pass(mcrt_ctx* ctx, const mcrt_photon_emit_params* params, int precision, uint32_t pass,
+                          uint64_t* n_caustic, uint64_t* n_global, mcrt_stats* stats);
+
+/* Fixed-radius photon gather for the following photon-mapped renders of this context, in place of the
+ * reference's k-NN estimate: every photon within r of a query enters it, with the k-NN formulas and r^2 in
+ * place of the k-th distance^2 - caustic 3/(pi r^2) sum flux f/pdf (1 - d/r), global 1/(pi r^2) sum flux f/pdf.
+ * The kernel (k_gather) replaces k_knn; its time is reported in gpu_ms_knn, the same stage slot.
+ * (0, 0) returns to the k-NN estimate, the default; otherwise both radii must be positive and finite
+ * (MCRT_ERR_INVALID). The radii stay set when maps are replaced. */
+int mcrt_photon_gather_radius(mcrt_ctx* ctx, double r_caustic, double r_global);
+
+/* The traversal of the fixed-radius gather on caller points (which: 0 caustic, 1 global map): for each point
+ * out_count[i] photons lie within `radius` (float64 distance2 <= radius^2, inclusive), out_flux_sum[i][3] is the
+ * float64 sum of their float32 flux and out_cone_sum[i][3] the same weighted by max(0, 1 - d / radius).
+ * Host buffers. MCRT_ERR_UNSUPPORTED if a traversal stack overflowed. */
+int mcrt_photon_gather_search(mcrt_ctx* ctx, int which, const double* points_xyz, size_t n, double radius,
+                              uint32_t* out_count, double* out_flux_sum, double* out_cone_sum, mcrt_stats* stats);
+
 /* Host view of the maps built by mcrt_photon_emit (which: 0 caustic, 1 global). The pointers stay
  * valid until the next mcrt_photon_emit / mcrt_destroy. */
 int mcrt_photon_download(mcrt_ctx* ctx, int which, mcrt_photon_map_desc* out);

@@ -39,6 +39,7 @@ ABI_SYMBOLS = [
     "mcrt_render_accumulate_dev", "mcrt_progressive_resolve_dev",
     "mcrt_render_accumulate_tiles_dev", "mcrt_progressive_resolve_tiles_dev",
     "mcrt_render_features_dev", "mcrt_denoise_dev", "mcrt_render_features_chain_dev",
+    "mcrt_photon_emit_pass", "mcrt_photon_gather_radius", "mcrt_photon_gather_search",
 ]
 
 
@@ -197,6 +198,11 @@ def lib():
                                          C.c_uint32, C.c_uint32, C.POINTER(C.c_uint64)]
         L.mcrt_photon_emit.argtypes = [C.c_void_p, C.POINTER(PhotonEmitParams), C.c_int, C.POINTER(C.c_uint64),
                                        C.POINTER(C.c_uint64), C.POINTER(Stats)]
+        L.mcrt_photon_emit_pass.argtypes = [C.c_void_p, C.POINTER(PhotonEmitParams), C.c_int, C.c_uint32, C.POINTER(C.c_uint64),
+                                            C.POINTER(C.c_uint64), C.POINTER(Stats)]
+        L.mcrt_photon_gather_radius.argtypes = [C.c_void_p, C.c_double, C.c_double]
+        L.mcrt_photon_gather_search.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.c_double, C.c_void_p, C.c_void_p,
+                                                C.c_void_p, C.POINTER(Stats)]
         L.mcrt_photon_download.argtypes = [C.c_void_p, C.c_int, C.POINTER(PhotonMapDesc)]
         L.mcrt_octree_build.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p, C.POINTER(C.c_void_p),
                                         C.POINTER(PhotonMapDesc), C.POINTER(C.c_double)]
@@ -813,10 +819,20 @@ class PhotonMapper(Integrator):
     def emit(self, emissions, caustic_factor, max_photons_per_octree_leaf=200, k_nearest_photons=50,
              direct_visualization=False, scene_bounds=None, precision=None):
         """PhotonMapper::PhotonMapper's first pass on the GPU; replaces the uploaded maps."""
+        return self.emit_pass(0, emissions, caustic_factor, max_photons_per_octree_leaf, k_nearest_photons, scene_bounds,
+                              direct_visualization, precision)
+
+    def emit_pass(self, pass_index, emissions, caustic_factor, max_photons_per_octree_leaf=200, k_nearest_photons=50,
+                  scene_bounds=None, direct_visualization=False, precision=None):
+        """Photon pass `pass_index` of progressive photon mapping (mcrt_photon_emit_pass): light l's emissions take the
+        reference's emission indices [pass_index * n_l, (pass_index + 1) * n_l) with the flux of a one-pass map, so every
+        pass map is complete on its own and independent of the others. Pass 0 is emit(). Replaces the uploaded maps."""
+        if not 0 <= int(pass_index) < 1 << 32:
+            raise McrtError(f"pass index {pass_index} is outside [0, 2^32)")
         p = self._emit_params(emissions, caustic_factor, max_photons_per_octree_leaf, k_nearest_photons, direct_visualization, scene_bounds)
         nc, ng, st = C.c_uint64(), C.c_uint64(), Stats()
-        self._check(lib().mcrt_photon_emit(self.ctx, C.byref(p), self.precision if precision is None else precision,
-                                           C.byref(nc), C.byref(ng), C.byref(st)))
+        self._check(lib().mcrt_photon_emit_pass(self.ctx, C.byref(p), self.precision if precision is None else precision,
+                                                int(pass_index), C.byref(nc), C.byref(ng), C.byref(st)))
         self.last_stats = st.as_dict()
         self.k_nearest = int(k_nearest_photons)
         # the maps stay in HBM (octrees are built there too); host copies only when somebody asks
@@ -867,6 +883,25 @@ class PhotonMapper(Integrator):
         st = Stats()
         self._check(lib().mcrt_knn_search(self.ctx, which, _ptr(points), n, _ptr(idx), _ptr(d2), _ptr(cnt), C.byref(st)))
         return idx, d2, cnt
+
+    def gather_radius(self, r_caustic, r_global):
+        """Following renders estimate radiance from every photon within r_caustic / r_global of a query (k_gather), with
+        the k-NN formulas and r^2 in place of the k-th distance^2; (0, 0) returns to the reference's k-NN estimate, the
+        default (mcrt_photon_gather_radius)."""
+        self._check(lib().mcrt_photon_gather_radius(self.ctx, float(r_caustic), float(r_global)))
+        self.gather_radii = (float(r_caustic), float(r_global))
+
+    def gather(self, which, points, radius):
+        """The fixed-radius search on caller points (mcrt_photon_gather_search) -> (count uint32 [n], flux_sum [n, 3],
+        cone_sum [n, 3]): the photons of map `which` (0 caustic, 1 global) within `radius` (distance^2 <= radius^2), and
+        the float64 sums of their flux, plain and weighted by max(0, 1 - d / radius)."""
+        points = np.ascontiguousarray(points, dtype=np.float64).reshape(-1, 3)
+        n = len(points)
+        cnt = np.zeros(n, np.uint32); flux = np.zeros((n, 3)); cone = np.zeros((n, 3))
+        st = Stats()
+        self._check(lib().mcrt_photon_gather_search(self.ctx, which, _ptr(points), n, float(radius), _ptr(cnt), _ptr(flux),
+                                                    _ptr(cone), C.byref(st)))
+        return cnt, flux, cone
 
 
 def _map_arrays(d):
@@ -1255,13 +1290,18 @@ class Progressive:
                  "tile": np.int64(self.tile),   # the tile masks' shapes depend on it
                  "scene_digest": np.array(h.hexdigest())}
         if ig.kind == INTEGRATOR_PHOTON:
-            caustic, glob, k, dv = ig._maps
-            ph = hashlib.sha256(np.array([k, dv], np.int64).tobytes())
-            for m in (caustic, glob):
-                rows = np.ascontiguousarray(np.asarray(m["photons"], np.float32).reshape(-1, 8)).view(np.dtype((np.void, 32))).ravel()
-                ph.update(np.int64(len(rows)).tobytes() + np.sort(rows).tobytes())   # a set: order inside a leaf may differ
-            ident["photon_digest"] = np.array(ph.hexdigest())
+            ident.update(self._photon_identity())
         return ident
+
+    def _photon_identity(self):
+        """The photon maps' part of _identity: a digest of the uploaded maps."""
+        import hashlib
+        caustic, glob, k, dv = self.integrator._maps
+        ph = hashlib.sha256(np.array([k, dv], np.int64).tobytes())
+        for m in (caustic, glob):
+            rows = np.ascontiguousarray(np.asarray(m["photons"], np.float32).reshape(-1, 8)).view(np.dtype((np.void, 32))).ravel()
+            ph.update(np.int64(len(rows)).tobytes() + np.sort(rows).tobytes())   # a set: order inside a leaf may differ
+        return {"photon_digest": np.array(ph.hexdigest())}
 
     def save(self, path):
         """Writes an .npz checkpoint: the sums, the sample counts, the pass index, the active tiles and the per-tile
@@ -1279,30 +1319,145 @@ class Progressive:
         """Resumes a checkpoint written by save() with `integrator` and `camera` (and `tile`, the checkpoint's if None).
         Raises McrtError, and resumes nothing, when the seed, precision, integrator kind, camera, film, tile, scene or
         photon maps differ from the checkpoint's. A checkpoint without tile state resumes with every tile active."""
-        import torch
-        with np.load(path) as z:
-            data = {k: z[k] for k in z.files}
+        data = _read_checkpoint(path)
         y_first, y_step, n_rows = (int(v) for v in data["row_set"])
         p = cls(integrator, camera, y_first, y_step, n_rows, int(data["tile"]) if tile is None else int(tile))
-        ident = p._identity()
+        p._restore(path, data)
+        return p
+
+    def _restore(self, path, data):
+        """Takes over the sums, counts and tile state of checkpoint `data` after checking its identity."""
+        import torch
+        ident = self._identity()
         for k, want in ident.items():
             if k not in data or not np.array_equal(data[k], want):
                 raise McrtError(f"checkpoint {path}: {k} differs from this render's; not resuming")
-        for name, dst in (("rgb_a", p.rgb[0]), ("rgb_b", p.rgb[1])) + ((("wsum_a", p.wsum[0]), ("wsum_b", p.wsum[1])) if p.filtered else ()):
+        for name, dst in (("rgb_a", self.rgb[0]), ("rgb_b", self.rgb[1])) + ((("wsum_a", self.wsum[0]), ("wsum_b", self.wsum[1])) if self.filtered else ()):
             if data[name].shape != tuple(dst.shape):
                 raise McrtError(f"checkpoint {path}: {name} has shape {data[name].shape}, expected {tuple(dst.shape)}")
             dst.copy_(torch.from_numpy(data[name]))
-        for name, want in (("active", p.active.shape), ("tile_counts", p.tile_counts.shape)):
+        for name, want in (("active", self.active.shape), ("tile_counts", self.tile_counts.shape)):
             if name in data and data[name].shape != want:
                 raise McrtError(f"checkpoint {path}: {name} has shape {data[name].shape}, expected {want}")
-        torch.cuda.synchronize(p.rgb[0].device)
-        p.counts = [int(c) for c in data["counts"]]
-        p.passes = int(data["passes"])
+        torch.cuda.synchronize(self.rgb[0].device)
+        self.counts = [int(c) for c in data["counts"]]
+        self.passes = int(data["passes"])
         if "active" in data:
-            p.active = data["active"].astype(bool)
-            p.tile_counts = data["tile_counts"].astype(np.int64)
+            self.active = data["active"].astype(bool)
+            self.tile_counts = data["tile_counts"].astype(np.int64)
         else:
-            p.tile_counts[...] = p.counts   # written before adaptive sampling: every tile has the uniform counts
+            self.tile_counts[...] = self.counts   # written before adaptive sampling: every tile has the uniform counts
+
+
+def _read_checkpoint(path):
+    with np.load(path) as z:
+        return {k: z[k] for k in z.files}
+
+
+def ppm_radii(r1, alpha, n):
+    """The n gather radii of progressive photon mapping (Knaus & Zwicker 2011): r_1 = r1, then
+    r_{i+1}^2 = r_i^2 (i + alpha) / (i + 1). With 0 < alpha < 1 the average of the passes' estimates converges:
+    bias and variance both go to zero. -> float64 [n]."""
+    r1, alpha, n = float(r1), float(alpha), int(n)
+    if not (0.0 < alpha < 1.0):
+        raise McrtError(f"alpha {alpha} is outside (0, 1)")
+    if not (r1 > 0.0 and math.isfinite(r1)):
+        raise McrtError(f"initial radius {r1} is not positive and finite")
+    i = np.arange(1, max(n, 1), dtype=np.float64)
+    r = np.empty(max(n, 0))
+    if n > 0:
+        r[0] = r1
+        r[1:] = r1 * np.sqrt(np.cumprod((i + alpha) / (i + 1.0)))
+    return r
+
+
+class ProgressivePhotonMapping(Progressive):
+    """Probabilistic progressive photon mapping (Knaus & Zwicker, "Progressive photon mapping: a probabilistic
+    approach", TOG 2011) over the passes of Progressive: pass i emits its own photon map (PhotonMapper.emit_pass(i),
+    the next emission indices of every light) and gathers with fixed radii r_i that shrink as ppm_radii, so the frame
+    converges to the image, not to one map's answer. Even passes go to half A and odd ones to B, so the halves come
+    from different maps and error(), render(target_error=...), render_adaptive and denoise() see the maps' noise too.
+
+    radius: None picks the initial radii once from the pass-0 maps - for each map the median, over up to 4096 of its
+    photons chosen with a fixed seed from the photons sorted by position, of the distance to the
+    k_nearest_photons-th nearest photon (PhotonMapper.knn at the photons' positions; in a map of fewer photons, the
+    farthest one); an empty caustic map takes the global radius. A number sets both, a pair (caustic, global) each.
+    With few emissions per pass that radius is large, and its blur dominates the error for many passes: on the
+    golden photon-mapping scene, a quarter of it reached the fixed k-NN map's error within 64 passes and the full
+    radius did not (DESIGN.md section 6).
+
+    Each pass replaces the photon mapper's uploaded maps and leaves it in gather mode (gather_radius(0, 0) returns
+    it to the k-NN estimate). The frame no longer equals a one-shot render; it equals the same sequence of passes.
+    Every sample is weighted equally: with passes of equal size that is Knaus and Zwicker's plain average of the
+    pass estimates, a shorter last pass deviates from it slightly. Checkpoints record the emissions, caustic factor,
+    leaf size, alpha and the initial radii instead of the maps; load() resumes with the map of pass `passes`, which
+    the next add() emits again (the passes are deterministic)."""
+
+    def __init__(self, photon_mapper, camera, emissions, caustic_factor, max_photons_per_octree_leaf=200, alpha=2 / 3,
+                 radius=None, k_nearest_photons=50, tile=16):
+        if not isinstance(photon_mapper, PhotonMapper):
+            raise McrtError("ProgressivePhotonMapping needs a PhotonMapper")
+        ppm_radii(1.0, alpha, 1)   # validates alpha
+        self.emissions, self.caustic_factor = int(emissions), float(caustic_factor)
+        self.max_photons_per_octree_leaf, self.k_nearest_photons = int(max_photons_per_octree_leaf), int(k_nearest_photons)
+        self.alpha = float(alpha)
+        super().__init__(photon_mapper, camera, tile=tile)
+        if radius is None:
+            radius = self._initial_radii()
+        r = (float(radius), float(radius)) if np.ndim(radius) == 0 else tuple(float(x) for x in radius)
+        if len(r) != 2:
+            raise McrtError("radius: None, a number or a (caustic, global) pair")
+        for x in r:
+            ppm_radii(x, self.alpha, 1)   # validates the radius
+        self.radius = r
+
+    def _emit(self, pass_index):
+        return self.integrator.emit_pass(pass_index, self.emissions, self.caustic_factor, self.max_photons_per_octree_leaf,
+                                         self.k_nearest_photons)
+
+    def _initial_radii(self):
+        self._emit(0)
+        ig, radii = self.integrator, [None, None]
+        rng = np.random.default_rng(0x9E3779B9)
+        for which, m in enumerate(ig._maps[:2]):
+            pos = m["photons"].reshape(-1, 8)[:, 3:6].astype(np.float64)
+            if len(pos) == 0:
+                continue
+            pos = pos[np.lexsort(pos.T[::-1])]   # the emission's atomics order the photons; the choice must not depend on it
+            pick = np.sort(rng.choice(len(pos), min(4096, len(pos)), replace=False))
+            _, d2, cnt = ig.knn(which, pos[pick])
+            # the farthest of the cnt results (unsorted); a map with fewer than k photons returns them all, then padding
+            kth = np.where(np.arange(d2.shape[1])[None, :] < cnt[:, None], d2, 0.0).max(axis=1)
+            radii[which] = float(np.median(np.sqrt(kth)))
+        if radii[1] is None:
+            raise McrtError("the pass-0 global photon map is empty: no initial radius")
+        return (radii[1] if radii[0] is None else radii[0], radii[1])
+
+    def pass_radii(self, pass_index):
+        """(caustic, global) gather radii of pass pass_index (0-based)."""
+        return tuple(float(ppm_radii(r, self.alpha, int(pass_index) + 1)[-1]) for r in self.radius)
+
+    def add(self, samples):
+        """Emits the map of pass self.passes, gathers with that pass's radii and renders the next samples (Progressive.add)."""
+        self._emit(self.passes)
+        self.integrator.gather_radius(*self.pass_radii(self.passes))
+        return super().add(samples)
+
+    def _photon_identity(self):
+        return {"ppm_emissions": np.int64(self.emissions), "ppm_caustic_factor": np.float64(self.caustic_factor),
+                "ppm_leaf": np.int64(self.max_photons_per_octree_leaf), "ppm_alpha": np.float64(self.alpha),
+                "ppm_radius": np.array(self.radius, np.float64)}
+
+    @classmethod
+    def load(cls, path, photon_mapper, camera, emissions, caustic_factor, max_photons_per_octree_leaf=200, alpha=2 / 3,
+             radius=None, k_nearest_photons=50, tile=None):
+        """Resumes a checkpoint written by save(). Raises McrtError, and resumes nothing, when the seed, precision,
+        camera, film, tile, scene, emissions, caustic factor, leaf size, alpha or initial radii differ from the
+        checkpoint's (radius None derives them from the pass-0 maps again)."""
+        data = _read_checkpoint(path)
+        p = cls(photon_mapper, camera, emissions, caustic_factor, max_photons_per_octree_leaf, alpha, radius, k_nearest_photons,
+                int(data["tile"]) if tile is None else int(tile))
+        p._restore(path, data)
         return p
 
 

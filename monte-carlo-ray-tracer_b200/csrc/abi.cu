@@ -125,6 +125,8 @@ struct mcrt_ctx
     std::vector<void*> emit_allocs;          // emission buffers (kept until the next emission / mcrt_destroy)
     unsigned long long emit_stored[2] = { 0, 0 };
     unsigned long long emit_work_first = 0;   // first emission index of the range being emitted (mcrt_photon_emit_range)
+    uint32_t emit_pass = 0;                   // photon pass being emitted (mcrt_photon_emit_pass)
+    double gather_r2[2] = { 0.0, 0.0 };       // fixed gather radius^2 of the caustic / global map; 0: k-NN (mcrt_photon_gather_radius)
     double emit_non_caustic_reject = 1.0;
     void* knn_queue64 = nullptr; void* knn_queue32 = nullptr;
     uint32_t knn_capacity64 = 0, knn_capacity32 = 0;
@@ -783,6 +785,7 @@ namespace
             p.emit.photons[0] = ctx->d_emit_photons[0]; p.emit.photons[1] = ctx->d_emit_photons[1];
             p.emit.capacity[0] = ctx->emit_capacity[0]; p.emit.capacity[1] = ctx->emit_capacity[1];
             p.emit.non_caustic_reject = (R)ctx->emit_non_caustic_reject;
+            p.emit.pass = ctx->emit_pass;
         }
         if (integrator == MCRT_INTEGRATOR_PHOTON)
         {
@@ -791,6 +794,7 @@ namespace
             p.pm.k_nearest = ctx->k_nearest;
             p.pm.direct_visualization = ctx->direct_visualization;
             p.pm.query_capacity = knn_capacity;
+            p.pm.gather_r2[0] = ctx->gather_r2[0]; p.pm.gather_r2[1] = ctx->gather_r2[1];
         }
 
         Counters init;
@@ -1353,15 +1357,20 @@ int mcrt_photon_emit_total(mcrt_ctx* ctx, const mcrt_photon_emit_params* params,
     return MCRT_OK;
 }
 
-int mcrt_photon_emit_range(mcrt_ctx* ctx, const mcrt_photon_emit_params* params, int precision, uint64_t work_first, uint64_t work_count,
-                           const float** caustic_dev, uint64_t* n_caustic, const float** global_dev, uint64_t* n_global, mcrt_stats* stats)
+// Work items [work_first, work_first + work_count) of the emission plan; light l's emissions take the reference's
+// emission indices pass * n_l + j, j < n_l (pass 0: the reference's own pass).
+static int emitRange(mcrt_ctx* ctx, const mcrt_photon_emit_params* params, int precision, uint32_t pass, uint64_t work_first,
+                     uint64_t work_count, const float** caustic_dev, uint64_t* n_caustic, const float** global_dev, uint64_t* n_global,
+                     mcrt_stats* stats)
 {
-    if (!ctx) return MCRT_ERR_INVALID;
     std::vector<unsigned long long> offsets; std::vector<V4<double>> flux64; std::vector<V4<float>> flux32;
     int rc = emissionPlan(ctx, params, offsets, flux64, flux32);
     if (rc) return rc;
     const uint64_t total = offsets.back();
     if (work_first > total || work_count > total - work_first) { ctx->error = "mcrt_photon_emit_range: range outside the emission index space"; return MCRT_ERR_INVALID; }
+    for (size_t l = 0; l + 1 < offsets.size(); l++)
+        if (((unsigned long long)pass + 1ull) * (offsets[l + 1] - offsets[l]) > 0x100000000ull)
+        { ctx->error = "mcrt_photon_emit_pass: the pass's emission indices do not fit 32 bits"; return MCRT_ERR_INVALID; }
     if (precision != MCRT_PRECISION_F64 && precision != MCRT_PRECISION_F32) { ctx->error = "unknown precision"; return MCRT_ERR_INVALID; }
 
     freeEmission(ctx);
@@ -1386,11 +1395,13 @@ int mcrt_photon_emit_range(mcrt_ctx* ctx, const mcrt_photon_emit_params* params,
     if (work_count)
     {
         ctx->emit_work_first = work_first;
+        ctx->emit_pass = pass;
         if (precision == MCRT_PRECISION_F64)
             rc = runWavefront<double>(ctx, nullptr, 0, 1, 0, 1, work_count, params->global_seed, MCRT_INTERNAL_EMIT, nullptr, nullptr, nullptr, 1, 1.0, nullptr, stats);
         else
             rc = runWavefront<float>(ctx, nullptr, 0, 1, 0, 1, work_count, params->global_seed, MCRT_INTERNAL_EMIT, nullptr, nullptr, nullptr, 1, 1.0, nullptr, stats);
         ctx->emit_work_first = 0;
+        ctx->emit_pass = 0;
         if (rc) { freeEmission(ctx); return rc; }
         const Counters& c = ctx->h_counters[0];
         ctx->emit_stored[0] = c.n_photons[0]; ctx->emit_stored[1] = c.n_photons[1];
@@ -1401,6 +1412,13 @@ int mcrt_photon_emit_range(mcrt_ctx* ctx, const mcrt_photon_emit_params* params,
     if (n_caustic) *n_caustic = ctx->emit_stored[0];
     if (n_global) *n_global = ctx->emit_stored[1];
     return MCRT_OK;
+}
+
+int mcrt_photon_emit_range(mcrt_ctx* ctx, const mcrt_photon_emit_params* params, int precision, uint64_t work_first, uint64_t work_count,
+                           const float** caustic_dev, uint64_t* n_caustic, const float** global_dev, uint64_t* n_global, mcrt_stats* stats)
+{
+    if (!ctx) return MCRT_ERR_INVALID;
+    return emitRange(ctx, params, precision, 0, work_first, work_count, caustic_dev, n_caustic, global_dev, n_global, stats);
 }
 
 int mcrt_photon_build_dev(mcrt_ctx* ctx, const mcrt_photon_emit_params* params, const float* caustic_dev, uint64_t n_caustic,
@@ -1444,13 +1462,19 @@ int mcrt_photon_build_dev(mcrt_ctx* ctx, const mcrt_photon_emit_params* params, 
 int mcrt_photon_emit(mcrt_ctx* ctx, const mcrt_photon_emit_params* params, int precision, uint64_t* n_caustic,
                      uint64_t* n_global, mcrt_stats* stats)
 {
+    return mcrt_photon_emit_pass(ctx, params, precision, 0, n_caustic, n_global, stats);
+}
+
+int mcrt_photon_emit_pass(mcrt_ctx* ctx, const mcrt_photon_emit_params* params, int precision, uint32_t pass, uint64_t* n_caustic,
+                          uint64_t* n_global, mcrt_stats* stats)
+{
     if (!ctx) return MCRT_ERR_INVALID;
     uint64_t total = 0;
     int rc = mcrt_photon_emit_total(ctx, params, &total);
     if (rc) return rc;
     const float* raw[2] = { nullptr, nullptr };
     uint64_t n[2] = { 0, 0 };
-    if ((rc = mcrt_photon_emit_range(ctx, params, precision, 0, total, &raw[0], &n[0], &raw[1], &n[1], stats))) return rc;
+    if ((rc = emitRange(ctx, params, precision, pass, 0, total, &raw[0], &n[0], &raw[1], &n[1], stats))) return rc;
     if (n_caustic) *n_caustic = n[0];
     if (n_global) *n_global = n[1];
     double build_ms = 0.0;
@@ -2243,6 +2267,56 @@ int mcrt_knn_search(mcrt_ctx* ctx, int which, const double* points_xyz, size_t n
     cudaEventElapsedTime(&ms, ctx->ev_start, ctx->ev_stop);
     if (stats) { std::memset(stats, 0, sizeof(*stats)); stats->knn_queries = n; stats->gpu_ms_total = ms; stats->gpu_ms_knn = ms; }
     if (flag) { ctx->error = "k-NN frontier overflow"; return MCRT_ERR_UNSUPPORTED; }
+    return MCRT_OK;
+}
+
+int mcrt_photon_gather_radius(mcrt_ctx* ctx, double r_caustic, double r_global)
+{
+    if (!ctx) return MCRT_ERR_INVALID;
+    if (r_caustic == 0.0 && r_global == 0.0) { ctx->gather_r2[0] = ctx->gather_r2[1] = 0.0; return MCRT_OK; }
+    const double r[2] = { r_caustic, r_global };
+    for (int w = 0; w < 2; w++)
+        if (!(r[w] > 0.0) || !std::isfinite(r[w] * r[w]))
+        { ctx->error = "mcrt_photon_gather_radius: radii must be (0, 0) or two positive finite numbers"; return MCRT_ERR_INVALID; }
+    ctx->gather_r2[0] = r_caustic * r_caustic; ctx->gather_r2[1] = r_global * r_global;
+    return MCRT_OK;
+}
+
+int mcrt_photon_gather_search(mcrt_ctx* ctx, int which, const double* points_xyz, size_t n, double radius, uint32_t* out_count,
+                              double* out_flux_sum, double* out_cone_sum, mcrt_stats* stats)
+{
+    if (!ctx) return MCRT_ERR_INVALID;
+    if ((which != 0 && which != 1) || !(radius > 0.0) || !std::isfinite(radius * radius))
+    { ctx->error = "mcrt_photon_gather_search: invalid arguments"; return MCRT_ERR_INVALID; }
+    if (n == 0) return MCRT_OK;
+    if (!points_xyz || !out_count || !out_flux_sum || !out_cone_sum) { ctx->error = "mcrt_photon_gather_search: null buffer"; return MCRT_ERR_INVALID; }
+    if (!ctx->has_photons) { ctx->error = "no photon maps uploaded"; return MCRT_ERR_NO_PHOTONS; }
+    CK(cudaSetDevice(ctx->device));
+    double* d_pts = nullptr; uint32_t* d_cnt = nullptr; double* d_flux = nullptr; double* d_cone = nullptr; uint32_t* d_flag = nullptr;
+    auto cleanup = [&]() { cudaFree(d_pts); cudaFree(d_cnt); cudaFree(d_flux); cudaFree(d_cone); cudaFree(d_flag); };
+    if (cudaMalloc((void**)&d_pts, n * 24) != cudaSuccess || cudaMalloc((void**)&d_cnt, n * 4) != cudaSuccess ||
+        cudaMalloc((void**)&d_flux, n * 24) != cudaSuccess || cudaMalloc((void**)&d_cone, n * 24) != cudaSuccess ||
+        cudaMalloc((void**)&d_flag, 4) != cudaSuccess)
+    { cleanup(); ctx->error = "cudaMalloc failed"; return MCRT_ERR_CUDA; }
+    cudaStream_t s = ctx->stream;
+    cudaMemcpyAsync(d_pts, points_xyz, n * 24, cudaMemcpyHostToDevice, s);
+    cudaMemsetAsync(d_flag, 0, 4, s);
+    cudaEventRecord(ctx->ev_start, s);
+    launchGatherUser(ctx->photon_map[which], d_pts, n, radius * radius, d_cnt, d_flux, d_cone, d_flag, ctx->sm_count * ctx->blocks_per_sm, s);
+    cudaEventRecord(ctx->ev_stop, s);
+    uint32_t flag = 0;
+    cudaMemcpyAsync(out_count, d_cnt, n * 4, cudaMemcpyDeviceToHost, s);
+    cudaMemcpyAsync(out_flux_sum, d_flux, n * 24, cudaMemcpyDeviceToHost, s);
+    cudaMemcpyAsync(out_cone_sum, d_cone, n * 24, cudaMemcpyDeviceToHost, s);
+    cudaMemcpyAsync(&flag, d_flag, 4, cudaMemcpyDeviceToHost, s);
+    cudaError_t e = cudaStreamSynchronize(s);
+    if (e == cudaSuccess) e = cudaGetLastError();
+    cleanup();
+    if (e != cudaSuccess) { ctx->error = cudaGetErrorString(e); return MCRT_ERR_CUDA; }
+    float ms = 0.f;
+    cudaEventElapsedTime(&ms, ctx->ev_start, ctx->ev_stop);
+    if (stats) { std::memset(stats, 0, sizeof(*stats)); stats->knn_queries = n; stats->gpu_ms_total = ms; stats->gpu_ms_knn = ms; }
+    if (flag) { ctx->error = "gather stack overflow"; return MCRT_ERR_UNSUPPORTED; }
     return MCRT_OK;
 }
 

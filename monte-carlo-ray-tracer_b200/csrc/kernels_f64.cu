@@ -180,6 +180,53 @@ namespace mcrt
         }
     }
 
+    // Fixed-radius search on caller points (mcrt_photon_gather_search), the traversal of k_gather: per point the
+    // number of photons within r and the float64 sums of their float32 flux, plain and cone-weighted (1 - d/r).
+    __global__ void __launch_bounds__(32 * KNN_WARPS_PER_BLOCK) k_gather_user(DevicePhotonMap map, const double* points, size_t n,
+                                                                             double r2, uint32_t* out_count, double* out_flux,
+                                                                             double* out_cone, uint32_t* overflow_flag)
+    {
+        __shared__ uint32_t gather_stack[KNN_WARPS_PER_BLOCK][GATHER_STACK];
+        uint32_t* const stack = gather_stack[threadIdx.x >> 5];
+        const unsigned lane = threadIdx.x & 31u;
+        const size_t warps_total = (size_t)gridDim.x * KNN_WARPS_PER_BLOCK;
+        const double inv_r2 = 1.0 / r2;
+        uint32_t overflow = 0;
+        for (size_t q = (size_t)blockIdx.x * KNN_WARPS_PER_BLOCK + (threadIdx.x >> 5); q < n; q += warps_total)
+        {
+            uint32_t count = 0;
+            double f[3] = { 0.0, 0.0, 0.0 }, c[3] = { 0.0, 0.0, 0.0 };
+            gatherWarp(map, points[3 * q], points[3 * q + 1], points[3 * q + 2], r2, stack, &overflow,
+                       [&](unsigned long long, double d2, const float4& a, const float4&)
+                       {
+                           const double wp = fmax(0.0, 1.0 - sqrt(d2 * inv_r2));
+                           count++;
+                           f[0] += (double)a.x; f[1] += (double)a.y; f[2] += (double)a.z;
+                           c[0] += (double)a.x * wp; c[1] += (double)a.y * wp; c[2] += (double)a.z * wp;
+                       });
+            count = __reduce_add_sync(0xFFFFFFFFu, count);
+            for (int off = 16; off > 0; off >>= 1)
+                for (int j = 0; j < 3; j++)
+                {
+                    f[j] += __shfl_xor_sync(0xFFFFFFFFu, f[j], off);
+                    c[j] += __shfl_xor_sync(0xFFFFFFFFu, c[j], off);
+                }
+            if (lane == 0)
+            {
+                out_count[q] = count;
+                for (int j = 0; j < 3; j++) { out_flux[3 * q + j] = f[j]; out_cone[3 * q + j] = c[j]; }
+            }
+            __syncwarp();
+        }
+        if (overflow && lane == 0) atomicOr(overflow_flag, 1u);
+    }
+
+    void launchGatherUser(const DevicePhotonMap& map, const double* points, size_t n, double r2, uint32_t* out_count,
+                          double* out_flux, double* out_cone, uint32_t* overflow_flag, int grid, cudaStream_t s)
+    {
+        k_gather_user<<<grid, 32 * KNN_WARPS_PER_BLOCK, 0, s>>>(map, points, n, r2, out_count, out_flux, out_cone, overflow_flag);
+    }
+
     __global__ void k_sampler_stream(const uint32_t* pixel, const uint32_t* sample, size_t n, uint32_t n_shuffles,
                                      uint32_t global_seed, uint32_t* out)
     {

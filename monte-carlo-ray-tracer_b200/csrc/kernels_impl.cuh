@@ -56,6 +56,15 @@ namespace mcrt
     template <> void Launch<MCRT_REAL>::knn(const WaveParams<MCRT_REAL>& p, int grid, cudaStream_t s)
     {
         const dim3 g(grid * 2), b(32 * KNN_WARPS_PER_BLOCK);
+        if (p.pm.gather_r2[0] > 0.0)
+        {
+            // fixed-radius gather (mcrt_photon_gather_radius) in place of the k-NN estimate
+            const bool lite = (p.scene.material_flags_any & ~SHADE_FEATS_LITE) == 0;
+            if (!p.filmp.is_default_box) k_gather<MCRT_REAL, true, SHADE_FEATS_ALL><<<g, b, 0, s>>>(p);
+            else if (lite) k_gather<MCRT_REAL, false, SHADE_FEATS_LITE><<<g, b, 0, s>>>(p);
+            else k_gather<MCRT_REAL, false, SHADE_FEATS_ALL><<<g, b, 0, s>>>(p);
+            return;
+        }
         const size_t smem = knnSharedBytes(p.pm.k_nearest);
         // the photon maps hold at least k photons in every render that matters; if a map is smaller the
         // search clamps k itself and the register slots are simply not all used

@@ -42,6 +42,8 @@ namespace mcrt
     void launchFp64Peak(double* sink, int iterations, int grid, cudaStream_t s);
     void launchKnnUser(const DevicePhotonMap& map, uint32_t k, const double* points, size_t n, uint32_t* out_index,
                        double* out_d2, uint32_t* out_count, uint32_t* overflow_flag, int grid, cudaStream_t s);
+    void launchGatherUser(const DevicePhotonMap& map, const double* points, size_t n, double r2, uint32_t* out_count,
+                          double* out_flux, double* out_cone, uint32_t* overflow_flag, int grid, cudaStream_t s);
     void launchSamplerStream(const uint32_t* pixel, const uint32_t* sample, size_t n, uint32_t n_shuffles,
                              uint32_t global_seed, uint32_t* out, cudaStream_t s);
 }

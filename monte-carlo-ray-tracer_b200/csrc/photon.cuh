@@ -55,6 +55,7 @@ namespace mcrt
         DevicePhotonMap map[2];
         KnnQuery<R>* queries;
         uint32_t k_nearest, direct_visualization, query_capacity, _pad;
+        double gather_r2[2];     // fixed gather radius^2 per map (k_gather); 0: the k-NN estimate (k_knn)
     };
 
     MCRT_D double octantDistance2(const DeviceOctant& o, double px, double py, double pz)
@@ -404,6 +405,70 @@ namespace mcrt
         const uint32_t k_pad = (k + 31u) & ~31u;
         const size_t per_warp = (size_t)k_pad * 12 + (size_t)KNN_FRONTIER * 12 + (size_t)KNN_HIST_BINS * 4;
         return KNN_WARPS_PER_BLOCK * ((per_warp + 15) & ~(size_t)15);
+    }
+
+    // Fixed-radius search (progressive photon mapping, Knaus & Zwicker 2011): every photon whose float64
+    // distance2 to p is <= r2, the same inclusive test as knnSearchWarpT. One warp per query, depth first:
+    // the children of an inner octant within r (octantDistance2 <= r2) are tested by lanes 0..7 and pushed
+    // through a ballot onto the warp's stack in shared memory. A leaf - or an inner octant whose whole box
+    // lies within r (octantMaxDistance2 <= r2) - streams its contiguous photon range 32 photons = 1 KB per
+    // step, coalesced; every photon is still tested, so rounding at the box's corners cannot admit one
+    // beyond r. visit(idx, d2, a, b) runs on each lane that holds an accepted photon (a, b: its two float4).
+    // There is no result set, so the number of photons found is unbounded. A stack overflow drops octants
+    // and sets *overflow (the callers fail the call, as for the k-NN frontier); a depth-first walk holds at
+    // most 7 per level + 1, and the octree builder caps the depth at 64, so GATHER_STACK = 512 suffices.
+    constexpr int GATHER_STACK = 512;
+
+    template <class Visit>
+    MCRT_D void gatherWarp(const DevicePhotonMap& map, double px, double py, double pz, double r2, uint32_t* stack,
+                           uint32_t* overflow, Visit&& visit)
+    {
+        const unsigned lane = threadIdx.x & 31u;
+        if (map.n_octants == 0 || map.n_photons == 0) return;
+        if (!(octantDistance2(map.octants[0], px, py, pz) <= r2)) return;
+        uint32_t n_stack = 0, cur = 0;
+        while (true)
+        {
+            const DeviceOctant* node = &map.octants[cur];
+            if (node->leaf || octantMaxDistance2(*node, px, py, pz) <= r2)
+            {
+                const unsigned long long start = node->start, end = start + node->count;
+                for (unsigned long long base = start; base < end; base += 32)
+                {
+                    const unsigned long long idx = base + lane;
+                    if (idx < end)
+                    {
+                        const float4 a = __ldg(&map.photons[2 * idx]);
+                        const float4 b = __ldg(&map.photons[2 * idx + 1]);
+                        const double dx = px - (double)a.w, dy = py - (double)b.x, dz = pz - (double)b.y;
+                        const double d2 = dx * dx + dy * dy + dz * dz;
+                        if (d2 <= r2) visit(idx, d2, a, b);
+                    }
+                }
+            }
+            else
+            {
+                uint32_t child = OCTANT_NULL;
+                bool push = false;
+                if (lane < node->n_children)
+                {
+                    child = node->children[lane];
+                    push = octantDistance2(map.octants[child], px, py, pz) <= r2;
+                }
+                const unsigned ballot = __ballot_sync(0xFFFFFFFFu, push);
+                if (push)
+                {
+                    const uint32_t slot = n_stack + __popc(ballot & ((1u << lane) - 1u));
+                    if (slot < (uint32_t)GATHER_STACK) stack[slot] = child;
+                }
+                n_stack += __popc(ballot);
+                if (n_stack > (uint32_t)GATHER_STACK) { *overflow = 1; n_stack = GATHER_STACK; }
+            }
+            __syncwarp();
+            if (n_stack == 0) break;
+            cur = stack[--n_stack];
+            __syncwarp();   // the slot just read is the next push's
+        }
     }
 
     // Photon::dir(), photon.hpp:19-27: std::sin/std::cos of the *float* angles (float overloads),
