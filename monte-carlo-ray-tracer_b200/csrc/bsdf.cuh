@@ -108,6 +108,15 @@ namespace mcrt
         pdf = wi.z * Consts<R>::INV_PI;
         V3<R> lambert = m.reflectance * Consts<R>::INV_PI;
         if (!(flags & MAT_ROUGH)) return lambert;
+        if constexpr (sizeof(R) == 4)
+        {
+            // float32: a unit vector's z can round to a hair above 1 and its xy part to exactly 0 (normal incidence), where
+            // the float64 expressions below give sqrt(< 0) and 0 / 0; both limits of the term are 0
+            const R sin2 = (pow2(wi.x) + pow2(wi.y)) * (pow2(wo.x) + pow2(wo.y));
+            const R cos_delta_phi = sin2 > R(0) ? gclamp((wi.x * wo.x + wi.y * wo.y) / msqrt(sin2), R(0), R(1)) : R(0);
+            const R D = msqrt(gmax(R(0), (R(1) - pow2(wi.z)) * (R(1) - pow2(wo.z)))) / gmax(wi.z, wo.z);
+            return lambert * (m.A + m.B * cos_delta_phi * D);
+        }
         R cos_delta_phi = gclamp((wi.x * wo.x + wi.y * wo.y) /
                                  msqrt((pow2(wi.x) + pow2(wi.y)) * (pow2(wo.x) + pow2(wo.y))), R(0), R(1));
         R D = msqrt((R(1) - pow2(wi.z)) * (R(1) - pow2(wo.z))) / gmax(wi.z, wo.z);

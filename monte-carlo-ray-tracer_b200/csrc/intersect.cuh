@@ -96,6 +96,23 @@ namespace mcrt
     MCRT_D bool intersectSphere(const V4<R>& g0, const V4<R>& g1, const RayQ<R>& ray, R& t_out)
     {
         V3<R> so = ray.o - g0.xyz();
+        if constexpr (sizeof(R) == 4)
+        {
+            // float32: b^2 - 4c cancels for a sphere seen from many radii away, and the error of the hit point can then exceed
+            // the ray offset, so paths leaving the sphere hit it again. The discriminant from the squared distance between the
+            // centre and the ray does not cancel (Haines et al., Ray Tracing Gems ch. 7); d is unit length, as a = 1 assumes.
+            const R bh = dot(ray.d, so);
+            const V3<R> f = so - ray.d * bh;
+            const R r = g1.x, fl = msqrt(dot(f, f));
+            const R disc = (r - fl) * (r + fl);
+            if (disc < R(0)) return false;
+            const R q = -(bh + (bh < R(0) ? -msqrt(disc) : msqrt(disc)));
+            R t_min = (dot(so, so) - pow2(r)) / q, t_max = q;
+            if (t_min > t_max) { const R tmp = t_min; t_min = t_max; t_max = tmp; }
+            if (t_max < R(0)) return false;
+            t_out = t_min < R(0) ? t_max : t_min;
+            return true;
+        }
         R b = R(2) * dot(ray.d, so);
         R c = dot(so, so) - pow2(g1.x);
         R t_min, t_max;
