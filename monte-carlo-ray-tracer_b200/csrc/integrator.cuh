@@ -597,6 +597,9 @@ namespace mcrt
     template <class R> MCRT_D V3<R> skyColor(const V3<R>& dir)
     {
         R d = R(0) * dir.x + R(1) * dir.y + R(0) * dir.z;
+        // float32: a direction's y can round past +-1 (a refracted or reflected ray that is vertical to round-off), where
+        // asin is NaN and the NaN would poison the pixel; its limit is the pole's colour
+        if constexpr (sizeof(R) == 4) d = gclamp(d, R(-1), R(1));
         R fy = (R(1) + masin(d) / Consts<R>::PI) / R(2);
         return mix(V3<R>(R(1), R(0.5), R(0)), V3<R>(R(0), R(0.5), R(1)), fy);
     }
