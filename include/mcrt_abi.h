@@ -448,6 +448,34 @@ int mcrt_progressive_resolve_tiles_dev(mcrt_ctx* ctx, const double* a_rgb_dev, c
                                        uint32_t width, uint32_t rows, uint32_t tile, double* out_rgb_dev,
                                        double* tile_error_dev, double* tile_sums_dev, double* frame_error);
 
+/* Light groups. Radiance is linear in emittance, so the path tracer can deposit each contribution into the plane of the
+ * emitter it comes from, and one render yields every group's share of the frame. mcrt_set_light_groups assigns light l
+ * (the scene's l-th light_prim) to group group_of_light[l] < n_groups; plane n_groups holds the sky, so a render has
+ * n_groups + 1 planes. group_of_light NULL with n_lights = n_groups = 0 clears the table; a scene without lights sets
+ * its sky-only table with any non-NULL pointer and n_lights = n_groups = 0. mcrt_scene_upload clears the table too.
+ * MCRT_ERR_NO_SCENE before an upload. MCRT_ERR_INVALID: n_lights other than the scene's light count, an id >= n_groups,
+ * n_groups = 2^32 - 1. MCRT_ERR_UNSUPPORTED: an emissive primitive the scene does not list as a light (its
+ * contributions would have no group). The other entry points ignore the table. */
+int mcrt_set_light_groups(mcrt_ctx* ctx, const uint32_t* group_of_light, uint32_t n_lights, uint32_t n_groups);
+/* mcrt_render_accumulate_dev (active_tiles NULL) or mcrt_render_accumulate_tiles_dev (active_tiles HOST, same mask
+ * layout) into light-group planes: planes_dev[n_planes][n_rows*W][3], plane g the sums of group g's lights and plane
+ * n_groups the sky's. Every contribution lands in exactly one plane, so the planes add up to the sums of the one-plane
+ * entry points over the same samples; the box film's weight is the sample count. MCRT_ERR_INVALID: no group table,
+ * n_planes != n_groups + 1, a null planes_dev, and every argument the one-plane entry points refuse.
+ * MCRT_ERR_UNSUPPORTED: a reconstruction filter, the photon mapper (photons carry no light index). Nothing is
+ * written when a call is refused. */
+int mcrt_render_accumulate_groups_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_t y_first, uint32_t y_step, uint32_t n_rows,
+                                      uint32_t tile, const uint8_t* active_tiles, uint32_t sample_first, uint32_t sample_count,
+                                      uint32_t global_seed, int integrator_kind, int precision, double* planes_dev,
+                                      uint32_t n_planes, mcrt_stats* stats);
+/* Relighting: out_dev[i] = sum over g = 0, 1, ... n_planes - 1 of weights[g][i % 3] * planes_dev[g * n_values + i]
+ * (weights HOST [n_planes][3]; each product rounded, then added, in order of g, in float64). On unresolved sums the
+ * result is the sums of the scene with group g's emittance scaled by weights[g] (plane n_planes - 1: the sky), and
+ * feeds mcrt_progressive_resolve[_tiles]_dev and mcrt_denoise_dev as they are. out_dev must not overlap planes_dev.
+ * MCRT_ERR_INVALID: null pointers, n_planes 0, n_values not a multiple of 3. */
+int mcrt_light_groups_combine_dev(mcrt_ctx* ctx, const double* planes_dev, uint32_t n_planes, uint64_t n_values,
+                                  const double* weights, double* out_dev);
+
 /* Denoising a progressive frame (mcrt_denoise_dev) needs per-pixel guides: the first hits of the camera rays of samples
  * [sample_first, sample_first + sample_count) of every pixel of the whole width x height frame add
  * {albedo.rgb, shading normal.xyz, t, 1} per hit into features_dev [height*width][8] (device, float64); a miss adds

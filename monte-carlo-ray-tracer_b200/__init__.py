@@ -40,6 +40,7 @@ ABI_SYMBOLS = [
     "mcrt_render_accumulate_tiles_dev", "mcrt_progressive_resolve_tiles_dev",
     "mcrt_render_features_dev", "mcrt_denoise_dev", "mcrt_render_features_chain_dev",
     "mcrt_photon_emit_pass", "mcrt_photon_gather_radius", "mcrt_photon_gather_search",
+    "mcrt_set_light_groups", "mcrt_render_accumulate_groups_dev", "mcrt_light_groups_combine_dev",
 ]
 
 
@@ -237,6 +238,11 @@ def lib():
         L.mcrt_progressive_resolve_tiles_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                                          C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p,
                                                          C.POINTER(C.c_double)]
+        L.mcrt_set_light_groups.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32]
+        L.mcrt_render_accumulate_groups_dev.argtypes = [C.c_void_p, C.POINTER(CameraRec), C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
+                                                        C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int, C.c_int, C.c_void_p,
+                                                        C.c_uint32, C.POINTER(Stats)]
+        L.mcrt_light_groups_combine_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint64, C.c_void_p, C.c_void_p]
         L.mcrt_render_features_dev.argtypes = [C.c_void_p, C.POINTER(CameraRec), C.c_uint32, C.c_uint32, C.c_uint32, C.c_int,
                                                C.c_void_p, C.POINTER(Stats)]
         L.mcrt_render_features_chain_dev.argtypes = [C.c_void_p, C.POINTER(CameraRec), C.c_uint32, C.c_uint32, C.c_uint32, C.c_int,
@@ -656,6 +662,46 @@ class Integrator:
                                                              p(tile_error_ptr), p(tile_sums_ptr), C.byref(err)))
         return err.value
 
+    # -- light groups (see Progressive's light_groups)
+    def set_light_groups(self, ids, n_groups=None):
+        """mcrt_set_light_groups: light l (the scene's l-th light_prim) goes to group ids[l]; the renders of
+        render_accumulate_groups_dev then have n_groups + 1 planes, the last one the sky's. n_groups: max(ids) + 1 if None.
+        ids None clears the table."""
+        if ids is None:
+            self._check(lib().mcrt_set_light_groups(self.ctx, None, 0, 0))
+            return
+        ids = np.ascontiguousarray(ids, dtype=np.uint32).reshape(-1)
+        n_groups = (int(ids.max()) + 1 if ids.size else 0) if n_groups is None else int(n_groups)
+        table = ids if ids.size else np.zeros(1, np.uint32)   # a lightless scene's sky-only table: any non-null pointer
+        self._check(lib().mcrt_set_light_groups(self.ctx, table.ctypes.data_as(C.c_void_p), ids.size, n_groups))
+
+    def render_accumulate_groups_dev(self, camera, planes_ptr, n_planes, sample_first, sample_count, tile=0, active=None,
+                                     y_first=0, y_step=1, n_rows=None, precision=None):
+        """mcrt_render_accumulate_groups_dev: render_accumulate_dev (active None) or render_accumulate_tiles_dev into the
+        light-group planes planes_ptr [n_planes, n_rows, width, 3] (device)."""
+        self.set_film(camera)
+        n_rows = len(range(y_first, camera.height, y_step)) if n_rows is None else n_rows
+        mask = None
+        if active is not None:
+            mask = np.ascontiguousarray(active, dtype=np.uint8)
+            if mask.shape != tile_grid(n_rows, camera.width, tile):
+                raise McrtError(f"tile mask has shape {mask.shape}, expected {tile_grid(n_rows, camera.width, tile)}")
+        st = Stats()
+        self._check(lib().mcrt_render_accumulate_groups_dev(self.ctx, C.byref(camera.rec), y_first, y_step, n_rows, tile,
+                                                            mask.ctypes.data_as(C.c_void_p) if mask is not None else None,
+                                                            sample_first, sample_count, self.global_seed, self.kind,
+                                                            self.precision if precision is None else precision,
+                                                            C.c_void_p(planes_ptr), n_planes, C.byref(st)))
+        self.last_stats = st.as_dict()
+        return self.last_stats
+
+    def light_groups_combine_dev(self, planes_ptr, n_planes, n_values, weights, out_ptr):
+        """mcrt_light_groups_combine_dev: out = sum over g of weights[g] * plane g, added in order of g (device buffers of
+        n_values float64 per plane). weights: [n_planes, 3] or [n_planes] (one weight for all three channels)."""
+        w = light_group_weights(weights, n_planes)
+        self._check(lib().mcrt_light_groups_combine_dev(self.ctx, C.c_void_p(planes_ptr), n_planes, n_values,
+                                                        w.ctypes.data_as(C.c_void_p), C.c_void_p(out_ptr)))
+
     # -- denoising (see Progressive.denoise)
     def render_features_dev(self, camera, features_ptr, sample_first, sample_count, precision=None, specular_depth=0):
         """mcrt_render_features_dev: adds the first-hit guides {albedo.rgb, normal.xyz, t, hits} of samples
@@ -773,6 +819,9 @@ class PhotonMapper(Integrator):
             raise McrtError("PhotonMapper needs photon maps (scene pack exported with photon_map=True) or emit=...")
         self._maps = maps
         self.upload_photons()
+
+    def set_light_groups(self, ids, n_groups=None):
+        raise McrtError("the photon mapper has no light groups: photons carry no light index")
 
     def _emit_params(self, emissions, caustic_factor, max_photons_per_octree_leaf, k_nearest_photons, direct_visualization, scene_bounds):
         p = PhotonEmitParams()
@@ -1023,6 +1072,48 @@ def bvh4_host(scene, max_leaf=0xFFFFFFFF):
         lib().mcrt_bvh4_host_free(h)
 
 
+def light_groups_by_emittance(scene, rtol=1e-12):
+    """Groups the scene's lights by emittance: a light joins the first group whose first light's emittance equals its
+    own in every channel to within rtol (relative; the default only absorbs the last-bit differences a mesh light's
+    triangles get from their export), else it opens the next group. -> (ids uint32 [n_lights], the emittance of each
+    group's first light float64 [n_groups, 3])."""
+    a = scene.a
+    lp = np.asarray(a["light_prim"], np.int64)
+    em = np.ascontiguousarray(a["materials"]["emittance"][np.asarray(a["prim_material"], np.int64)[lp]], np.float64).reshape(-1, 3)
+    ids = np.zeros(len(lp), np.uint32)
+    groups = np.zeros((0, 3))
+    for l, row in enumerate(em):
+        same = np.nonzero((np.abs(groups - row) <= rtol * np.maximum(np.abs(groups), np.abs(row))).all(axis=1))[0]
+        if same.size:
+            ids[l] = same[0]
+        else:
+            ids[l] = len(groups)
+            groups = np.concatenate([groups, row[None]])
+    return ids, groups
+
+
+def light_group_weights(weights, n_planes):
+    """Weights of a light-group combination as float64 [n_planes, 3]: [n_planes, 3] as given, [n_planes] one weight for
+    the three channels of a plane."""
+    w = np.asarray(weights, np.float64)
+    if w.shape == (n_planes,):
+        w = np.repeat(w[:, None], 3, axis=1)
+    if w.shape != (n_planes, 3):
+        raise McrtError(f"light-group weights have shape {w.shape}, expected ({n_planes}, 3) or ({n_planes},)")
+    return np.ascontiguousarray(w)
+
+
+def light_groups_combine(planes, weights):
+    """numpy restatement of mcrt_light_groups_combine_dev: sum over g of weights[g] * planes[g], in order of g, each
+    product rounded before its addition. planes: [n_planes, ..., 3]."""
+    planes = np.asarray(planes, np.float64)
+    w = light_group_weights(weights, planes.shape[0])
+    out = planes[0] * w[0]
+    for g in range(1, planes.shape[0]):
+        out = out + planes[g] * w[g]
+    return out
+
+
 def tile_grid(rows, width, tile):
     """(tiles_y, tiles_x) of the tile x tile blocks of a rows x width grid; the last row and column of blocks may be
     smaller than tile x tile."""
@@ -1073,12 +1164,20 @@ class Progressive:
     comes back. Passes then render only the active tiles (mcrt_render_accumulate_tiles_dev), so every active tile has
     `counts` samples and a retired tile keeps the counts it had (`tile_counts`); the frame is resolved with those
     per-tile counts (mcrt_progressive_resolve_tiles_dev). While every tile is active, add, frame and error run the
-    uniform entry points. With a reconstruction filter, adaptive passes need the whole frame as the row set."""
+    uniform entry points. With a reconstruction filter, adaptive passes need the whole frame as the row set.
+
+    Light groups (light_groups = a group id per light, e.g. light_groups_by_emittance(scene)[0]; box film, path tracer):
+    A and B then hold one plane per group and one for the sky, [G+1, rows, width, 3], filled by
+    mcrt_render_accumulate_groups_dev. frame, error, render, render_adaptive and denoise work on the planes' sum, the
+    beauty frame, so they behave as without groups; group_frames() resolves each plane, and relight(weights) and
+    denoise(weights=...) work on any weighted sum (mcrt_light_groups_combine_dev), without rendering again."""
 
     _STATS = ("paths", "extension_rays", "shadow_rays")
 
-    def __init__(self, integrator, camera, y_first=0, y_step=1, n_rows=None, tile=16):
+    def __init__(self, integrator, camera, y_first=0, y_step=1, n_rows=None, tile=16, light_groups=None):
         import torch
+        if light_groups is not None and integrator.kind == INTEGRATOR_PHOTON:
+            raise McrtError("the photon mapper has no light groups: photons carry no light index")
         self.integrator, self.camera = integrator, camera
         self.y_first, self.y_step = int(y_first), int(y_step)
         self.n_rows = len(range(self.y_first, camera.height, self.y_step)) if n_rows is None else int(n_rows)
@@ -1086,8 +1185,16 @@ class Progressive:
         rec = camera.film_rec()
         self.filtered = rec is not None and not (rec.filter == FILM_FILTERS["box"] and rec.radius in (0.0, 0.5))
         self.rows = camera.height if self.filtered else self.n_rows   # rows of the sums and of the resolved frame
+        self.light_groups, self.n_planes = None, 1
+        if light_groups is not None:
+            if self.filtered:
+                raise McrtError("light groups take the box film only")
+            self.light_groups = np.ascontiguousarray(light_groups, dtype=np.uint32).reshape(-1)
+            self.n_planes = (int(self.light_groups.max()) + 1 if self.light_groups.size else 0) + 1
+            integrator.set_light_groups(self.light_groups, self.n_planes - 1)   # refuses a wrong table before anything is allocated
+        planes = (self.n_planes,) if self.light_groups is not None else ()
         dev = torch.device("cuda", integrator.device)
-        self.rgb = [torch.zeros((self.rows, camera.width, 3), dtype=torch.float64, device=dev) for _ in range(2)]
+        self.rgb = [torch.zeros(planes + (self.rows, camera.width, 3), dtype=torch.float64, device=dev) for _ in range(2)]
         self.wsum = [torch.zeros((self.rows, camera.width), dtype=torch.float64, device=dev) for _ in range(2)] if self.filtered else None
         torch.cuda.synchronize(dev)   # the library renders on its own stream
         self.counts = [0, 0]          # samples per pixel in A and B (of the active tiles)
@@ -1109,7 +1216,12 @@ class Progressive:
         """Renders samples [self.samples, self.samples + samples) of the active tiles into A (even pass) or B (odd pass)."""
         half = self.passes % 2
         wsum = self.wsum[half].data_ptr() if self.filtered else None
-        if self.active.all():
+        if self.light_groups is not None:
+            self.integrator.set_light_groups(self.light_groups, self.n_planes - 1)   # the integrator may serve other renders
+            st = self.integrator.render_accumulate_groups_dev(self.camera, self.rgb[half].data_ptr(), self.n_planes, self.samples,
+                                                              int(samples), self.tile, None if self.active.all() else self.active,
+                                                              self.y_first, self.y_step, self.n_rows)
+        elif self.active.all():
             st = self.integrator.render_accumulate_dev(self.camera, self.rgb[half].data_ptr(), wsum, self.samples,
                                                        int(samples), self.y_first, self.y_step, self.n_rows)
         else:
@@ -1126,29 +1238,63 @@ class Progressive:
     def _resolve(self, sums=False):
         """-> (frame, frame error, tile errors, tile sums {sum v, sum I^2} [tiles_y, tiles_x, 2] or None). sums: resolve
         through the per-tile entry point, which reports the tile sums, even while every tile is active."""
-        import torch
         if self._resolved is None or (sums and self._resolved[3] is None):
-            t = self.tile
-            out = torch.empty_like(self.rgb[0])
-            tiles = torch.empty(self.active.shape, dtype=torch.float64, device=out.device)
-            if self.active.all() and not sums:
-                ptrs = []
-                for h in (0, 1):
-                    has = self.counts[h] > 0
-                    ptrs += [self.rgb[h].data_ptr() if has else None,
-                             self.wsum[h].data_ptr() if has and self.filtered else None, self.counts[h]]
-                err = self.integrator.progressive_resolve_dev(*ptrs, self.camera.width, self.rows, t, out.data_ptr(), tiles.data_ptr())
-                self._resolved = (out.cpu().numpy(), err, tiles.cpu().numpy(), None)
-            else:
-                tile_sums = torch.empty(self.active.shape + (2,), dtype=torch.float64, device=out.device)
-                ptrs = []
-                for h in (0, 1):
-                    has = bool(self.tile_counts[..., h].any())
-                    ptrs += [self.rgb[h].data_ptr() if has else None, self.wsum[h].data_ptr() if has and self.filtered else None]
-                err = self.integrator.progressive_resolve_tiles_dev(*ptrs, self.tile_counts, self.camera.width, self.rows, t,
-                                                                    out.data_ptr(), tiles.data_ptr(), tile_sums.data_ptr())
-                self._resolved = (out.cpu().numpy(), err, tiles.cpu().numpy(), tile_sums.cpu().numpy())
+            self._resolved = self._resolve_halves(self._halves(), sums)
         return self._resolved
+
+    def _halves(self, weights=None):
+        """The sums of halves A and B, [rows, width, 3] each: with light groups the combination of their planes with
+        weights [G+1, 3] or [G+1] (None: every weight 1, the beauty frame's sums)."""
+        import torch
+        if self.light_groups is None:
+            if weights is not None:
+                raise McrtError("weights need a render with light groups")
+            return self.rgb
+        w = np.ones(self.n_planes) if weights is None else weights
+        out = []
+        for h in (0, 1):
+            o = torch.empty(self.rgb[h].shape[1:], dtype=torch.float64, device=self.rgb[h].device)
+            torch.cuda.synchronize(o.device)   # the library works on its own stream
+            self.integrator.light_groups_combine_dev(self.rgb[h].data_ptr(), self.n_planes, o.numel(), w, o.data_ptr())
+            out.append(o)
+        return out
+
+    def _resolve_halves(self, rgb, sums=False):
+        """_resolve of the half sums rgb [A, B] (the weight sums are self.wsum's)."""
+        import torch
+        t = self.tile
+        out = torch.empty_like(rgb[0])
+        tiles = torch.empty(self.active.shape, dtype=torch.float64, device=out.device)
+        if self.active.all() and not sums:
+            ptrs = []
+            for h in (0, 1):
+                has = self.counts[h] > 0
+                ptrs += [rgb[h].data_ptr() if has else None,
+                         self.wsum[h].data_ptr() if has and self.filtered else None, self.counts[h]]
+            err = self.integrator.progressive_resolve_dev(*ptrs, self.camera.width, self.rows, t, out.data_ptr(), tiles.data_ptr())
+            return out.cpu().numpy(), err, tiles.cpu().numpy(), None
+        tile_sums = torch.empty(self.active.shape + (2,), dtype=torch.float64, device=out.device)
+        ptrs = []
+        for h in (0, 1):
+            has = bool(self.tile_counts[..., h].any())
+            ptrs += [rgb[h].data_ptr() if has else None, self.wsum[h].data_ptr() if has and self.filtered else None]
+        err = self.integrator.progressive_resolve_tiles_dev(*ptrs, self.tile_counts, self.camera.width, self.rows, t,
+                                                            out.data_ptr(), tiles.data_ptr(), tile_sums.data_ptr())
+        return out.cpu().numpy(), err, tiles.cpu().numpy(), tile_sums.cpu().numpy()
+
+    # -- light groups
+    def group_frames(self):
+        """Each light-group plane resolved on its own, float64 [G+1, rows, width, 3]; the last plane is the sky's."""
+        if self.light_groups is None:
+            raise McrtError("group_frames needs a render with light groups")
+        return np.stack([self._resolve_halves([self.rgb[0][g], self.rgb[1][g]])[0] for g in range(self.n_planes)])
+
+    def relight(self, weights):
+        """The frame relit: the planes summed with weights [G+1, 3] or [G+1] (the last row weights the sky), resolved
+        like frame() -> (frame, frame relative error, per-tile relative errors). Weight w_g on group g equals a render
+        of the scene with group g's emittance scaled by w_g."""
+        frame, err, tiles, _ = self._resolve_halves(self._halves(weights))
+        return frame, err, tiles
 
     def frame(self):
         """The resolved frame, float64 [rows, width, 3]."""
@@ -1243,7 +1389,7 @@ class Progressive:
         return {"albedo": albedo, "normal": normal, "depth": depth, "coverage": hits / float(samples)}
 
     def denoise(self, iterations=None, sigma_color=None, sigma_normal=None, sigma_depth=None, sigma_albedo=None,
-                feature_samples=8, specular_depth=0):
+                feature_samples=8, specular_depth=0, weights=None):
         """The frame denoised by the cross-filtered a-trous filter of mcrt_denoise_dev, guided by features(feature_samples)
         -> (frame float64 [H, W, 3], residual error). The error is estimated like error()'s, from the difference of the
         two filtered halves: it measures the remaining noise, not the filter's bias. Arguments left None take the
@@ -1255,7 +1401,9 @@ class Progressive:
 
         Known limits: at specular_depth 0 the guides come from the first hit only, so glass and mirrors are guided by
         their own surface; rough and glossy lobes are never followed; the feature samples [0, F) also feed half A; the Owen-scrambled halves are not
-        independent, so the residual estimate can read about 10 % low."""
+        independent, so the residual estimate can read about 10 % low.
+
+        weights (light groups only): denoise the frame relit with these weights (relight) instead of the beauty frame."""
         import torch
         if (self.y_first, self.y_step, self.n_rows) != (0, 1, self.camera.height):
             raise McrtError("denoise needs the whole frame as the row set (y_first 0, y_step 1, n_rows = height)")
@@ -1266,10 +1414,11 @@ class Progressive:
         v = {k: DENOISE_DEFAULTS[k] if x is None else x for k, x in given.items()}
         params = DenoiseParams(int(v["iterations"]), 0, float(v["sigma_color"]), float(v["sigma_normal"]),
                                float(v["sigma_depth"]), float(v["sigma_albedo"]))
+        rgb = self._halves(weights)
         feats = self._feature_sums(feature_samples, specular_depth)
-        out = torch.empty_like(self.rgb[0])
+        out = torch.empty_like(rgb[0])
         w = (self.wsum[0].data_ptr(), self.wsum[1].data_ptr()) if self.filtered else (None, None)
-        err = self.integrator.denoise_dev(self.rgb[0].data_ptr(), w[0], self.rgb[1].data_ptr(), w[1], self.tile_counts, self.tile,
+        err = self.integrator.denoise_dev(rgb[0].data_ptr(), w[0], rgb[1].data_ptr(), w[1], self.tile_counts, self.tile,
                                           feats.data_ptr(), self.camera.width, self.camera.height, out.data_ptr(), params)
         return out.cpu().numpy(), err
 
@@ -1291,6 +1440,8 @@ class Progressive:
                  "scene_digest": np.array(h.hexdigest())}
         if ig.kind == INTEGRATOR_PHOTON:
             ident.update(self._photon_identity())
+        if self.light_groups is not None:
+            ident["light_groups"] = self.light_groups.copy()
         return ident
 
     def _photon_identity(self):
@@ -1315,13 +1466,14 @@ class Progressive:
             np.savez(f, **data)
 
     @classmethod
-    def load(cls, path, integrator, camera, tile=None):
+    def load(cls, path, integrator, camera, tile=None, light_groups=None):
         """Resumes a checkpoint written by save() with `integrator` and `camera` (and `tile`, the checkpoint's if None).
-        Raises McrtError, and resumes nothing, when the seed, precision, integrator kind, camera, film, tile, scene or
-        photon maps differ from the checkpoint's. A checkpoint without tile state resumes with every tile active."""
+        Raises McrtError, and resumes nothing, when the seed, precision, integrator kind, camera, film, tile, scene,
+        photon maps or light groups differ from the checkpoint's. A checkpoint without tile state resumes with every
+        tile active."""
         data = _read_checkpoint(path)
         y_first, y_step, n_rows = (int(v) for v in data["row_set"])
-        p = cls(integrator, camera, y_first, y_step, n_rows, int(data["tile"]) if tile is None else int(tile))
+        p = cls(integrator, camera, y_first, y_step, n_rows, int(data["tile"]) if tile is None else int(tile), light_groups)
         p._restore(path, data)
         return p
 
@@ -1329,6 +1481,8 @@ class Progressive:
         """Takes over the sums, counts and tile state of checkpoint `data` after checking its identity."""
         import torch
         ident = self._identity()
+        if ("light_groups" in data) != ("light_groups" in ident):
+            raise McrtError(f"checkpoint {path}: light groups differ from this render's; not resuming")
         for k, want in ident.items():
             if k not in data or not np.array_equal(data[k], want):
                 raise McrtError(f"checkpoint {path}: {k} differs from this render's; not resuming")
@@ -1394,9 +1548,11 @@ class ProgressivePhotonMapping(Progressive):
     the next add() emits again (the passes are deterministic)."""
 
     def __init__(self, photon_mapper, camera, emissions, caustic_factor, max_photons_per_octree_leaf=200, alpha=2 / 3,
-                 radius=None, k_nearest_photons=50, tile=16):
+                 radius=None, k_nearest_photons=50, tile=16, light_groups=None):
         if not isinstance(photon_mapper, PhotonMapper):
             raise McrtError("ProgressivePhotonMapping needs a PhotonMapper")
+        if light_groups is not None:
+            raise McrtError("the photon mapper has no light groups: photons carry no light index")
         ppm_radii(1.0, alpha, 1)   # validates alpha
         self.emissions, self.caustic_factor = int(emissions), float(caustic_factor)
         self.max_photons_per_octree_leaf, self.k_nearest_photons = int(max_photons_per_octree_leaf), int(k_nearest_photons)

@@ -96,6 +96,14 @@ struct mcrt_ctx
     uint32_t* d_pixel_list = nullptr;      // pixels of the active tiles of mcrt_render_accumulate_tiles_dev (grow-only)
     size_t pixel_list_values = 0;
     std::vector<uint32_t> h_pixel_list;
+    // light groups (mcrt_set_light_groups); mcrt_scene_upload clears them
+    bool has_light_groups = false;
+    bool emissive_unlit = false;            // the scene has an emissive primitive that is not one of its lights
+    uint32_t n_light_groups = 0;
+    uint32_t* d_group_of_light = nullptr;   // [n_lights] (grow-only)
+    size_t group_of_light_values = 0;
+    double* d_group_weights = nullptr;      // [n_planes][3] of mcrt_light_groups_combine_dev (grow-only)
+    size_t group_weight_values = 0;
     cudaEvent_t ev_start = nullptr, ev_stop = nullptr, ev_poll[2] = { nullptr, nullptr };
 
     // photon maps (PhotonMapper::caustic_map / global_map) + k-NN query queues
@@ -670,6 +678,7 @@ namespace
     {
         double* rgb;    // box film [n_pixels][3] in film_index order; filtered film [height*width][3]
         double* wsum;   // filtered film [height*width]; null with the box film
+        uint32_t n_planes = 0;   // box film only: rgb holds this many light-group planes (mcrt_render_accumulate_groups_dev)
     };
 
     // The wavefront loop shared by mcrt_render_rows(_dev) and mcrt_sample_rays. Camera work item w is sample
@@ -733,6 +742,12 @@ namespace
         double* const film_rgb = accum ? accum->rgb : ctx->d_film;
         double* const film_wsum = accum ? accum->wsum : ctx->d_film_wsum;
         p.film = film_rgb;
+        if (accum && accum->n_planes)
+        {
+            p.group_of_light = ctx->d_group_of_light;
+            p.plane_values = film_pixels * 3;
+            p.n_planes = accum->n_planes;
+        }
         p.filmp.is_default_box = filtered ? 0u : 1u;
         if (filtered)
         {
@@ -1110,6 +1125,8 @@ void mcrt_destroy(mcrt_ctx* ctx)
     if (ctx->d_resolve_scratch) cudaFree(ctx->d_resolve_scratch);
     if (ctx->d_denoise_scratch) cudaFree(ctx->d_denoise_scratch);
     if (ctx->d_pixel_list) cudaFree(ctx->d_pixel_list);
+    if (ctx->d_group_of_light) cudaFree(ctx->d_group_of_light);
+    if (ctx->d_group_weights) cudaFree(ctx->d_group_weights);
     if (ctx->d_counters) cudaFree(ctx->d_counters);
     if (ctx->d_sobol_bytes) cudaFree(ctx->d_sobol_bytes);
     if (ctx->h_counters) cudaFreeHost(ctx->h_counters);
@@ -1172,6 +1189,8 @@ int mcrt_scene_upload(mcrt_ctx* ctx, const mcrt_scene_desc* scene, uint64_t* h2d
 
     freeAll(ctx->scene_allocs);
     ctx->has_scene = false;
+    ctx->has_light_groups = false;
+    ctx->n_light_groups = 0;
 
     // scene scale for the fast mode's ray offsets
     double scale = 0.0;
@@ -1236,6 +1255,14 @@ int mcrt_scene_upload(mcrt_ctx* ctx, const mcrt_scene_desc* scene, uint64_t* h2d
     ctx->prim_interpolates.assign(s.n_prims, 0);
     for (uint32_t i = 0; i < s.n_prims; i++)
         if (s.prim_type[i] == MCRT_PRIM_TRIANGLE && s.tri_vn_index[s.prim_index[i]] >= 0) ctx->prim_interpolates[i] = 1;
+    {
+        // light groups need every emitter the paths can hit to be a light (buildArrays has checked the indices)
+        std::vector<uint8_t> lit(s.n_prims, 0);
+        for (uint32_t i = 0; i < s.n_lights; i++) lit[s.light_prim[i]] = 1;
+        ctx->emissive_unlit = false;
+        for (uint32_t i = 0; i < s.n_prims && !ctx->emissive_unlit; i++)
+            ctx->emissive_unlit = s.materials[s.prim_material[i]].emissive && !lit[i];
+    }
     ctx->has_scene = true;
     if (h2d_bytes) *h2d_bytes = bytes;
     return MCRT_OK;
@@ -1724,6 +1751,57 @@ int mcrt_render_accumulate_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_
                           precision, nullptr, stats, &sums);
 }
 
+namespace
+{
+    // The active-tile path of mcrt_render_accumulate_tiles_dev / _groups_dev (the caller has checked the sums)
+    int accumulateTiles(mcrt_ctx* ctx, const std::string& name, const mcrt_camera* camera, uint32_t y_first, uint32_t y_step,
+                        uint32_t n_rows, uint32_t tile, const uint8_t* active_tiles, uint32_t sample_first, uint32_t sample_count,
+                        uint32_t global_seed, int integrator_kind, int precision, const FilmSums& sums, mcrt_stats* stats)
+    {
+        if (tile == 0) { ctx->error = name + ": tile is 0"; return MCRT_ERR_INVALID; }
+        if (!active_tiles) { ctx->error = name + ": null tile mask"; return MCRT_ERR_INVALID; }
+        // the mask's size follows from the row set: check it before reading the mask
+        if (!camera || n_rows == 0 || y_step == 0 || camera->width == 0 ||
+            (uint64_t)y_first + (uint64_t)(n_rows - 1) * y_step >= camera->height)
+        {
+            ctx->error = name + ": invalid camera / row range";
+            return MCRT_ERR_INVALID;
+        }
+        if ((uint64_t)camera->width * n_rows > 0xFFFFFFFFull) { ctx->error = "row block too large"; return MCRT_ERR_INVALID; }
+        if (!ctx->film_default && (y_first != 0 || y_step != 1 || n_rows != camera->height))
+        {
+            // a filter splats across tiles: the resolve's tiles span the whole frame, so the row set must be the whole frame
+            ctx->error = name + ": with a reconstruction filter the row set must be the whole frame";
+            return MCRT_ERR_UNSUPPORTED;
+        }
+        // tile-major, row-major inside a tile: adjacent lanes of k_generate take adjacent pixels of one tile
+        const uint32_t width = camera->width;
+        const uint32_t tiles_x = (width + tile - 1) / tile, tiles_y = (n_rows + tile - 1) / tile;
+        std::vector<uint32_t>& list = ctx->h_pixel_list;
+        list.clear();
+        for (uint32_t ty = 0; ty < tiles_y; ty++)
+            for (uint32_t tx = 0; tx < tiles_x; tx++)
+            {
+                if (!active_tiles[(size_t)ty * tiles_x + tx]) continue;
+                const uint32_t y1 = std::min(n_rows, (ty + 1) * tile), x1 = std::min(width, (tx + 1) * tile);
+                for (uint32_t y = ty * tile; y < y1; y++)
+                    for (uint32_t x = tx * tile; x < x1; x++) list.push_back(y * width + x);
+            }
+        if (list.empty()) { ctx->error = name + ": no active tile"; return MCRT_ERR_INVALID; }
+        CK(cudaSetDevice(ctx->device));
+        if (ctx->pixel_list_values < list.size())
+        {
+            if (ctx->d_pixel_list) cudaFree(ctx->d_pixel_list);
+            ctx->d_pixel_list = nullptr; ctx->pixel_list_values = 0;
+            CK(cudaMalloc((void**)&ctx->d_pixel_list, list.size() * sizeof(uint32_t)));
+            ctx->pixel_list_values = list.size();
+        }
+        CK(cudaMemcpyAsync(ctx->d_pixel_list, list.data(), list.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+        return renderDispatch(ctx, camera, y_first, y_step, n_rows, sample_first, sample_count, global_seed, integrator_kind,
+                              precision, nullptr, stats, &sums, ctx->d_pixel_list, (uint32_t)list.size());
+    }
+}
+
 int mcrt_render_accumulate_tiles_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_t y_first, uint32_t y_step, uint32_t n_rows,
                                      uint32_t tile, const uint8_t* active_tiles, uint32_t sample_first, uint32_t sample_count,
                                      uint32_t global_seed, int integrator_kind, int precision, double* rgb_sum_dev,
@@ -1732,48 +1810,110 @@ int mcrt_render_accumulate_tiles_dev(mcrt_ctx* ctx, const mcrt_camera* camera, u
     if (!ctx) return MCRT_ERR_INVALID;
     int rc;
     if ((rc = checkAccumulateSums(ctx, "mcrt_render_accumulate_tiles_dev", sample_count, rgb_sum_dev, weight_sum_dev))) return rc;
-    if (tile == 0) { ctx->error = "mcrt_render_accumulate_tiles_dev: tile is 0"; return MCRT_ERR_INVALID; }
-    if (!active_tiles) { ctx->error = "mcrt_render_accumulate_tiles_dev: null tile mask"; return MCRT_ERR_INVALID; }
-    // the mask's size follows from the row set: check it before reading the mask
-    if (!camera || n_rows == 0 || y_step == 0 || camera->width == 0 ||
-        (uint64_t)y_first + (uint64_t)(n_rows - 1) * y_step >= camera->height)
+    const FilmSums sums = { rgb_sum_dev, weight_sum_dev };
+    return accumulateTiles(ctx, "mcrt_render_accumulate_tiles_dev", camera, y_first, y_step, n_rows, tile, active_tiles, sample_first,
+                           sample_count, global_seed, integrator_kind, precision, sums, stats);
+}
+
+int mcrt_set_light_groups(mcrt_ctx* ctx, const uint32_t* group_of_light, uint32_t n_lights, uint32_t n_groups)
+{
+    if (!ctx) return MCRT_ERR_INVALID;
+    if (!ctx->has_scene) { ctx->error = "mcrt_set_light_groups: no scene uploaded"; return MCRT_ERR_NO_SCENE; }
+    if (!group_of_light)
     {
-        ctx->error = "mcrt_render_accumulate_tiles_dev: invalid camera / row range";
+        if (n_lights || n_groups) { ctx->error = "mcrt_set_light_groups: a null table clears it; n_lights and n_groups must be 0"; return MCRT_ERR_INVALID; }
+        ctx->has_light_groups = false;
+        ctx->n_light_groups = 0;
+        return MCRT_OK;
+    }
+    if (n_lights != ctx->scene64.n_lights)
+    {
+        ctx->error = "mcrt_set_light_groups: n_lights " + std::to_string(n_lights) + ", the scene has " + std::to_string(ctx->scene64.n_lights);
         return MCRT_ERR_INVALID;
     }
-    if ((uint64_t)camera->width * n_rows > 0xFFFFFFFFull) { ctx->error = "row block too large"; return MCRT_ERR_INVALID; }
-    if (!ctx->film_default && (y_first != 0 || y_step != 1 || n_rows != camera->height))
+    if (n_groups == 0xFFFFFFFFu) { ctx->error = "mcrt_set_light_groups: n_groups + 1 planes must fit 32 bits"; return MCRT_ERR_INVALID; }
+    for (uint32_t l = 0; l < n_lights; l++)
+        if (group_of_light[l] >= n_groups)
+        {
+            ctx->error = "mcrt_set_light_groups: light " + std::to_string(l) + " has group " + std::to_string(group_of_light[l]) +
+                         ", n_groups is " + std::to_string(n_groups);
+            return MCRT_ERR_INVALID;
+        }
+    if (ctx->emissive_unlit)
     {
-        // a filter splats across tiles: the resolve's tiles span the whole frame, so the row set must be the whole frame
-        ctx->error = "mcrt_render_accumulate_tiles_dev: with a reconstruction filter the row set must be the whole frame";
+        ctx->error = "mcrt_set_light_groups: the scene has an emissive primitive that is not one of its lights";
         return MCRT_ERR_UNSUPPORTED;
     }
-    // tile-major, row-major inside a tile: adjacent lanes of k_generate take adjacent pixels of one tile
-    const uint32_t width = camera->width;
-    const uint32_t tiles_x = (width + tile - 1) / tile, tiles_y = (n_rows + tile - 1) / tile;
-    std::vector<uint32_t>& list = ctx->h_pixel_list;
-    list.clear();
-    for (uint32_t ty = 0; ty < tiles_y; ty++)
-        for (uint32_t tx = 0; tx < tiles_x; tx++)
-        {
-            if (!active_tiles[(size_t)ty * tiles_x + tx]) continue;
-            const uint32_t y1 = std::min(n_rows, (ty + 1) * tile), x1 = std::min(width, (tx + 1) * tile);
-            for (uint32_t y = ty * tile; y < y1; y++)
-                for (uint32_t x = tx * tile; x < x1; x++) list.push_back(y * width + x);
-        }
-    if (list.empty()) { ctx->error = "mcrt_render_accumulate_tiles_dev: no active tile"; return MCRT_ERR_INVALID; }
     CK(cudaSetDevice(ctx->device));
-    if (ctx->pixel_list_values < list.size())
+    ctx->has_light_groups = false;
+    if (ctx->group_of_light_values < n_lights)
     {
-        if (ctx->d_pixel_list) cudaFree(ctx->d_pixel_list);
-        ctx->d_pixel_list = nullptr; ctx->pixel_list_values = 0;
-        CK(cudaMalloc((void**)&ctx->d_pixel_list, list.size() * sizeof(uint32_t)));
-        ctx->pixel_list_values = list.size();
+        if (ctx->d_group_of_light) cudaFree(ctx->d_group_of_light);
+        ctx->d_group_of_light = nullptr; ctx->group_of_light_values = 0;
+        CK(cudaMalloc((void**)&ctx->d_group_of_light, n_lights * sizeof(uint32_t)));
+        ctx->group_of_light_values = n_lights;
     }
-    CK(cudaMemcpyAsync(ctx->d_pixel_list, list.data(), list.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
-    const FilmSums sums = { rgb_sum_dev, weight_sum_dev };
+    if (n_lights) CK(cudaMemcpyAsync(ctx->d_group_of_light, group_of_light, n_lights * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    ctx->n_light_groups = n_groups;
+    ctx->has_light_groups = true;
+    return MCRT_OK;
+}
+
+int mcrt_render_accumulate_groups_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_t y_first, uint32_t y_step, uint32_t n_rows,
+                                      uint32_t tile, const uint8_t* active_tiles, uint32_t sample_first, uint32_t sample_count,
+                                      uint32_t global_seed, int integrator_kind, int precision, double* planes_dev,
+                                      uint32_t n_planes, mcrt_stats* stats)
+{
+    if (!ctx) return MCRT_ERR_INVALID;
+    const std::string name = "mcrt_render_accumulate_groups_dev";
+    if (!ctx->film_default) { ctx->error = name + ": light-group planes take the box film only"; return MCRT_ERR_UNSUPPORTED; }
+    if (integrator_kind == MCRT_INTEGRATOR_PHOTON)
+    {
+        ctx->error = name + ": photons carry no light index, the photon mapper has no light groups";
+        return MCRT_ERR_UNSUPPORTED;
+    }
+    if (!ctx->has_light_groups) { ctx->error = name + ": no light-group table (mcrt_set_light_groups)"; return MCRT_ERR_INVALID; }
+    if (n_planes != ctx->n_light_groups + 1)
+    {
+        ctx->error = name + ": n_planes " + std::to_string(n_planes) + ", the table has " + std::to_string(ctx->n_light_groups) +
+                     " groups + the sky";
+        return MCRT_ERR_INVALID;
+    }
+    int rc;
+    if ((rc = checkAccumulateSums(ctx, name.c_str(), sample_count, planes_dev, nullptr))) return rc;
+    const FilmSums sums = { planes_dev, nullptr, n_planes };
+    if (active_tiles)
+        return accumulateTiles(ctx, name, camera, y_first, y_step, n_rows, tile, active_tiles, sample_first, sample_count, global_seed,
+                               integrator_kind, precision, sums, stats);
+    CK(cudaSetDevice(ctx->device));
     return renderDispatch(ctx, camera, y_first, y_step, n_rows, sample_first, sample_count, global_seed, integrator_kind,
-                          precision, nullptr, stats, &sums, ctx->d_pixel_list, (uint32_t)list.size());
+                          precision, nullptr, stats, &sums);
+}
+
+int mcrt_light_groups_combine_dev(mcrt_ctx* ctx, const double* planes_dev, uint32_t n_planes, uint64_t n_values,
+                                  const double* weights, double* out_dev)
+{
+    if (!ctx) return MCRT_ERR_INVALID;
+    if (!planes_dev || !weights || !out_dev || n_planes == 0 || n_values % 3 != 0)
+    {
+        ctx->error = "mcrt_light_groups_combine_dev: null pointer, no plane or n_values not a multiple of 3";
+        return MCRT_ERR_INVALID;
+    }
+    CK(cudaSetDevice(ctx->device));
+    const size_t values = 3 * (size_t)n_planes;
+    if (ctx->group_weight_values < values)
+    {
+        if (ctx->d_group_weights) cudaFree(ctx->d_group_weights);
+        ctx->d_group_weights = nullptr; ctx->group_weight_values = 0;
+        CK(cudaMalloc((void**)&ctx->d_group_weights, values * sizeof(double)));
+        ctx->group_weight_values = values;
+    }
+    CK(cudaMemcpyAsync(ctx->d_group_weights, weights, values * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+    if (n_values) launchLightGroupsCombine(planes_dev, n_planes, n_values, ctx->d_group_weights, out_dev, ctx->sm_count * ctx->blocks_per_sm, ctx->stream);
+    CK(cudaStreamSynchronize(ctx->stream));
+    CK(cudaGetLastError());
+    return MCRT_OK;
 }
 
 namespace

@@ -254,6 +254,11 @@ namespace mcrt
         const uint32_t* sobol_bytes; // byte-sliced Sobol matrices [6][4][256] (makeSobolByteTable)
         EmitParams<R> emit;         // photon emission pass (mcrt_photon_emit) only
         FilmParams filmp;           // reconstruction filter (default box: only `film` is used)
+        // light-group render (mcrt_render_accumulate_groups_dev): `film` holds n_planes planes of plane_values values each;
+        // a contribution of light l goes to plane group_of_light[l], the sky's to plane n_planes - 1. 0: one plane
+        const uint32_t* group_of_light;
+        size_t plane_values;
+        uint32_t n_planes;
     };
 
     // ------------------------------------------------------------------------------------------
@@ -349,14 +354,24 @@ namespace mcrt
         return (p.row_first + row * p.row_step) * p.camera.width + col;
     }
 
-    // Film::deposit of one radiance contribution of sample (pixel, sample)
-    // (FILM = false: the default box film, the kernels every benchmark and parity case runs)
-    template <bool FILM, class R>
-    MCRT_D void depositRadiance(const WaveParams<R>& p, uint32_t film_index, uint32_t pixel, uint32_t sample, const V3<R>& v)
+    // Film modes of the depositing kernels. FILM_MODE_BOX: the default box film, the kernels every benchmark and parity
+    // case runs; FILM_MODE_SPLAT: a reconstruction filter; FILM_MODE_GROUPS: the box film with one plane per light group
+    enum FilmMode : int { FILM_MODE_BOX = 0, FILM_MODE_SPLAT = 1, FILM_MODE_GROUPS = 2 };
+
+    // Film::deposit of one radiance contribution of sample (pixel, sample). light: index of the emitter it comes from,
+    // NO_PRIM for the sky (read by FILM_MODE_GROUPS only)
+    template <int FILM, class R>
+    MCRT_D void depositRadiance(const WaveParams<R>& p, uint32_t film_index, uint32_t pixel, uint32_t sample, const V3<R>& v,
+                                uint32_t light = NO_PRIM)
     {
-        if constexpr (!FILM)
+        if constexpr (FILM == FILM_MODE_BOX)
         {
             filmAddV(p.film, film_index, v);
+        }
+        else if constexpr (FILM == FILM_MODE_GROUPS)
+        {
+            const uint32_t plane = light == NO_PRIM ? p.n_planes - 1u : p.group_of_light[light];
+            filmAddV(p.film + plane * p.plane_values, film_index, v);
         }
         else
         {
@@ -609,7 +624,7 @@ namespace mcrt
     constexpr uint32_t SHADE_FEATS_ALL = 0xFFFFFFFFu;
     constexpr uint32_t SHADE_FEATS_LITE = ~(uint32_t)(MAT_ROUGH | MAT_ROUGH_SPECULAR | MAT_COMPLEX_IOR);
 
-    template <class R, int KIND, bool FILM, uint32_t FEATS>
+    template <class R, int KIND, int FILM, uint32_t FEATS>
     __global__ void __launch_bounds__(128, FEATS == 0xFFFFFFFFu ? MCRT_SHADE_MINBLOCKS : MCRT_SHADE_MINBLOCKS_LITE) k_shade(WaveParams<R> p, int cur)
     {
         __shared__ SobolByteTables sobol_tab;
@@ -713,14 +728,14 @@ namespace mcrt
                     {
                         if (ray.depth == 0 || ray.dirac_delta)
                         {
-                            depositRadiance<FILM>(p, film_index, meta.x, meta.y, m.emittance * throughput);
+                            depositRadiance<FILM>(p, film_index, meta.x, meta.y, m.emittance * throughput, ps.light);
                         }
                         else if (ls_light != NO_PRIM && sc.lights[ls_light].prim == hit.prim)
                         {
                             R cos_light_theta = dot(ia.out, ia.normal);
                             R light_pdf = pow2(ia.t) / (ps.area * cos_light_theta);
                             R mis_weight = powerHeuristic(ls_bsdf_pdf, light_pdf);
-                            depositRadiance<FILM>(p, film_index, meta.x, meta.y, (mis_weight * m.emittance / ls_select) * throughput);
+                            depositRadiance<FILM>(p, film_index, meta.x, meta.y, (mis_weight * m.emittance / ls_select) * throughput, ls_light);
                         }
                     }
 
@@ -926,7 +941,8 @@ namespace mcrt
         if (stack_overflows) atomicAdd(&c->ior_stack_overflows, (unsigned long long)stack_overflows);
     }
 
-    template <class R, bool FILM, int PRIMS, int FAST>
+    // FILM_MODE_GROUPS finds the sampled light's group through the light primitive's shading record (sm.x is L.prim)
+    template <class R, int FILM, int PRIMS, int FAST>
     __global__ void __launch_bounds__(256, FAST == 2 ? MCRT_TRACE_MINBLOCKS_DYN : (FAST == 1 ? MCRT_TRACE_MINBLOCKS_FAST : (PRIMS == PRIMS_ALL ? Mode<R>::trace_minblocks : Mode<R>::trace_minblocks_pruned))) k_shadow(WaveParams<R> p)
     {
         const uint32_t n = p.counters->n_shadow;
@@ -956,7 +972,8 @@ namespace mcrt
                         const V4<R> so = srec.o, sd = srec.d, sk = srec.k;
                         R light_pdf = pow2(h.t) / sd.w;
                         R mis_weight = powerHeuristic(light_pdf, so.w);
-                        depositRadiance<FILM>(p, sm.y, pixelOfFilmIndex(p, sm.y), sm.w, sk.xyz() * (mis_weight / (light_pdf * sk.w)));
+                        depositRadiance<FILM>(p, sm.y, pixelOfFilmIndex(p, sm.y), sm.w, sk.xyz() * (mis_weight / (light_pdf * sk.w)),
+                                              FILM == FILM_MODE_GROUPS ? p.scene.shade[sm.x].light : NO_PRIM);
                     }
                 }, cnt, overflow);
             flushStats(p.counters, cnt, rays, true, overflow);
@@ -978,7 +995,8 @@ namespace mcrt
                 const V4<R> sk = srec.k;
                 R light_pdf = pow2(h.t) / sd.w;
                 R mis_weight = powerHeuristic(light_pdf, so.w);
-                depositRadiance<FILM>(p, sm.y, pixelOfFilmIndex(p, sm.y), sm.w, sk.xyz() * (mis_weight / (light_pdf * sk.w)));
+                depositRadiance<FILM>(p, sm.y, pixelOfFilmIndex(p, sm.y), sm.w, sk.xyz() * (mis_weight / (light_pdf * sk.w)),
+                                      FILM == FILM_MODE_GROUPS ? p.scene.shade[sm.x].light : NO_PRIM);
             }
         }
         flushStats(p.counters, cnt, rays, true, overflow);

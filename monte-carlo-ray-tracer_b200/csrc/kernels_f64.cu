@@ -149,6 +149,26 @@ namespace mcrt
         else k_progressive_tile_error<false><<<tile_grid, 256, 0, s>>>(sums, n_tiles, both, tile_error, nullptr);
     }
 
+    // Relighting of light-group planes: out[i] = sum over g of weights[g][i % 3] * planes[g][i], g = 0, 1, ... in order,
+    // each product rounded before its addition (this unit has no FMA contraction), so numpy reproduces it bit for bit
+    static __global__ void __launch_bounds__(256) k_light_groups_combine(const double* planes, uint32_t n_planes, uint64_t n_values,
+                                                                         const double* weights, double* out)
+    {
+        for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n_values; i += (uint64_t)gridDim.x * blockDim.x)
+        {
+            const uint32_t c = (uint32_t)(i % 3u);
+            double acc = weights[c] * planes[i];
+            for (uint32_t g = 1; g < n_planes; g++) acc = acc + weights[3 * g + c] * planes[g * n_values + i];
+            out[i] = acc;
+        }
+    }
+
+    void launchLightGroupsCombine(const double* planes, uint32_t n_planes, uint64_t n_values, const double* weights, double* out,
+                                  int grid, cudaStream_t s)
+    {
+        k_light_groups_combine<<<grid, 256, 0, s>>>(planes, n_planes, n_values, weights, out);
+    }
+
     void launchFp64Peak(double* sink, int iterations, int grid, cudaStream_t s)
     {
         k_fp64_peak<<<grid, 256, 0, s>>>(sink, iterations);

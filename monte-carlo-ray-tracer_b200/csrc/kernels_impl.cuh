@@ -42,16 +42,21 @@ namespace mcrt
     {
         // scenes whose materials use no Oren-Nayar / GGX / conductor Fresnel run the instantiation without that code
         const bool lite = (p.scene.material_flags_any & ~SHADE_FEATS_LITE) == 0;
-        if (!p.filmp.is_default_box) k_shade<MCRT_REAL, 0, true, SHADE_FEATS_ALL><<<grid * 2, 128, 0, s>>>(p, cur);
-        else if (lite) k_shade<MCRT_REAL, 0, false, SHADE_FEATS_LITE><<<grid * 2, 128, 0, s>>>(p, cur);
-        else k_shade<MCRT_REAL, 0, false, SHADE_FEATS_ALL><<<grid * 2, 128, 0, s>>>(p, cur);
+        if (!p.filmp.is_default_box) k_shade<MCRT_REAL, 0, FILM_MODE_SPLAT, SHADE_FEATS_ALL><<<grid * 2, 128, 0, s>>>(p, cur);
+        else if (p.n_planes)
+        {
+            if (lite) k_shade<MCRT_REAL, 0, FILM_MODE_GROUPS, SHADE_FEATS_LITE><<<grid * 2, 128, 0, s>>>(p, cur);
+            else k_shade<MCRT_REAL, 0, FILM_MODE_GROUPS, SHADE_FEATS_ALL><<<grid * 2, 128, 0, s>>>(p, cur);
+        }
+        else if (lite) k_shade<MCRT_REAL, 0, FILM_MODE_BOX, SHADE_FEATS_LITE><<<grid * 2, 128, 0, s>>>(p, cur);
+        else k_shade<MCRT_REAL, 0, FILM_MODE_BOX, SHADE_FEATS_ALL><<<grid * 2, 128, 0, s>>>(p, cur);
     }
     template <> void Launch<MCRT_REAL>::shadePhoton(const WaveParams<MCRT_REAL>& p, int cur, int grid, cudaStream_t s)
     {
         const bool lite = (p.scene.material_flags_any & ~SHADE_FEATS_LITE) == 0;
-        if (!p.filmp.is_default_box) k_shade<MCRT_REAL, 1, true, SHADE_FEATS_ALL><<<grid * 2, 128, 0, s>>>(p, cur);
-        else if (lite) k_shade<MCRT_REAL, 1, false, SHADE_FEATS_LITE><<<grid * 2, 128, 0, s>>>(p, cur);
-        else k_shade<MCRT_REAL, 1, false, SHADE_FEATS_ALL><<<grid * 2, 128, 0, s>>>(p, cur);
+        if (!p.filmp.is_default_box) k_shade<MCRT_REAL, 1, FILM_MODE_SPLAT, SHADE_FEATS_ALL><<<grid * 2, 128, 0, s>>>(p, cur);
+        else if (lite) k_shade<MCRT_REAL, 1, FILM_MODE_BOX, SHADE_FEATS_LITE><<<grid * 2, 128, 0, s>>>(p, cur);
+        else k_shade<MCRT_REAL, 1, FILM_MODE_BOX, SHADE_FEATS_ALL><<<grid * 2, 128, 0, s>>>(p, cur);
     }
     template <> void Launch<MCRT_REAL>::knn(const WaveParams<MCRT_REAL>& p, int grid, cudaStream_t s)
     {
@@ -96,30 +101,43 @@ namespace mcrt
         #undef MCRT_KNN_LAUNCH
         #undef MCRT_KNN_LAUNCH1
     }
-    template <> void Launch<MCRT_REAL>::shadow(const WaveParams<MCRT_REAL>& p, int grid, cudaStream_t s)
+    // k_shadow of the box film (one plane or light-group planes) with the scene-specialised traversal
+    template <int FILM> static void launchShadowBox(const WaveParams<MCRT_REAL>& p, int grid, cudaStream_t s)
     {
         if constexpr (Mode<MCRT_REAL>::parity)
         {
-            if (p.scene.bvh4 && p.scene.dynamic_fetch && p.filmp.is_default_box)
+            if (p.scene.bvh4 && p.scene.dynamic_fetch)
             {
-                if (p.scene.prims_class == PRIMS_TRI) k_shadow<MCRT_REAL, false, PRIMS_TRI, 2><<<grid, 256, fastStackSharedBytes(256), s>>>(p);
-                else if (p.scene.prims_class == PRIMS_TRI_SPHERE) k_shadow<MCRT_REAL, false, PRIMS_TRI_SPHERE, 2><<<grid, 256, fastStackSharedBytes(256), s>>>(p);
-                else k_shadow<MCRT_REAL, false, PRIMS_ALL, 2><<<grid, 256, fastStackSharedBytes(256), s>>>(p);
+                if (p.scene.prims_class == PRIMS_TRI) k_shadow<MCRT_REAL, FILM, PRIMS_TRI, 2><<<grid, 256, fastStackSharedBytes(256), s>>>(p);
+                else if (p.scene.prims_class == PRIMS_TRI_SPHERE) k_shadow<MCRT_REAL, FILM, PRIMS_TRI_SPHERE, 2><<<grid, 256, fastStackSharedBytes(256), s>>>(p);
+                else k_shadow<MCRT_REAL, FILM, PRIMS_ALL, 2><<<grid, 256, fastStackSharedBytes(256), s>>>(p);
                 return;
             }
             if (p.scene.bvh4)
             {
-                if (!p.filmp.is_default_box) k_shadow<MCRT_REAL, true, PRIMS_ALL, 1><<<grid, 256, fastStackSharedBytes(256), s>>>(p);
-                else if (p.scene.prims_class == PRIMS_TRI) k_shadow<MCRT_REAL, false, PRIMS_TRI, 1><<<grid, 256, fastStackSharedBytes(256), s>>>(p);
-                else if (p.scene.prims_class == PRIMS_TRI_SPHERE) k_shadow<MCRT_REAL, false, PRIMS_TRI_SPHERE, 1><<<grid, 256, fastStackSharedBytes(256), s>>>(p);
-                else k_shadow<MCRT_REAL, false, PRIMS_ALL, 1><<<grid, 256, fastStackSharedBytes(256), s>>>(p);
+                if (p.scene.prims_class == PRIMS_TRI) k_shadow<MCRT_REAL, FILM, PRIMS_TRI, 1><<<grid, 256, fastStackSharedBytes(256), s>>>(p);
+                else if (p.scene.prims_class == PRIMS_TRI_SPHERE) k_shadow<MCRT_REAL, FILM, PRIMS_TRI_SPHERE, 1><<<grid, 256, fastStackSharedBytes(256), s>>>(p);
+                else k_shadow<MCRT_REAL, FILM, PRIMS_ALL, 1><<<grid, 256, fastStackSharedBytes(256), s>>>(p);
                 return;
             }
         }
-        if (!p.filmp.is_default_box) k_shadow<MCRT_REAL, true, PRIMS_ALL, 0><<<grid, 256, 0, s>>>(p);
-        else if (p.scene.prims_class == PRIMS_TRI) k_shadow<MCRT_REAL, false, PRIMS_TRI, 0><<<grid, 256, 0, s>>>(p);
-        else if (p.scene.prims_class == PRIMS_TRI_SPHERE) k_shadow<MCRT_REAL, false, PRIMS_TRI_SPHERE, 0><<<grid, 256, 0, s>>>(p);
-        else k_shadow<MCRT_REAL, false, PRIMS_ALL, 0><<<grid, 256, 0, s>>>(p);
+        if (p.scene.prims_class == PRIMS_TRI) k_shadow<MCRT_REAL, FILM, PRIMS_TRI, 0><<<grid, 256, 0, s>>>(p);
+        else if (p.scene.prims_class == PRIMS_TRI_SPHERE) k_shadow<MCRT_REAL, FILM, PRIMS_TRI_SPHERE, 0><<<grid, 256, 0, s>>>(p);
+        else k_shadow<MCRT_REAL, FILM, PRIMS_ALL, 0><<<grid, 256, 0, s>>>(p);
+    }
+    template <> void Launch<MCRT_REAL>::shadow(const WaveParams<MCRT_REAL>& p, int grid, cudaStream_t s)
+    {
+        if (!p.filmp.is_default_box)
+        {
+            // filtered film: the rare configuration, the generic traversal only
+            if constexpr (Mode<MCRT_REAL>::parity)
+            {
+                if (p.scene.bvh4) { k_shadow<MCRT_REAL, FILM_MODE_SPLAT, PRIMS_ALL, 1><<<grid, 256, fastStackSharedBytes(256), s>>>(p); return; }
+            }
+            k_shadow<MCRT_REAL, FILM_MODE_SPLAT, PRIMS_ALL, 0><<<grid, 256, 0, s>>>(p);
+        }
+        else if (p.n_planes) launchShadowBox<FILM_MODE_GROUPS>(p, grid, s);
+        else launchShadowBox<FILM_MODE_BOX>(p, grid, s);
     }
     template <> void Launch<MCRT_REAL>::shadeKey(const WaveParams<MCRT_REAL>& p, int grid, cudaStream_t s)
     {

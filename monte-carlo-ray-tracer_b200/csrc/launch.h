@@ -39,6 +39,9 @@ namespace mcrt
     void launchProgressiveResolve(const ProgressiveHalf& a, const ProgressiveHalf& b, bool weighted, uint32_t width, uint32_t rows,
                                   uint32_t tile, uint32_t tiles_x, double* out, double* sums, double* tile_error, uint32_t n_tiles,
                                   int grid, cudaStream_t s, const double* tile_counts = nullptr);
+    // out[i] = sum_g weights[g][i % 3] * planes[g * n_values + i], summed over g in order (mcrt_light_groups_combine_dev)
+    void launchLightGroupsCombine(const double* planes, uint32_t n_planes, uint64_t n_values, const double* weights, double* out,
+                                  int grid, cudaStream_t s);
     void launchFp64Peak(double* sink, int iterations, int grid, cudaStream_t s);
     void launchKnnUser(const DevicePhotonMap& map, uint32_t k, const double* points, size_t n, uint32_t* out_index,
                        double* out_d2, uint32_t* out_count, uint32_t* overflow_flag, int grid, cudaStream_t s);
