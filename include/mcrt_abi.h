@@ -472,9 +472,40 @@ int mcrt_render_accumulate_groups_dev(mcrt_ctx* ctx, const mcrt_camera* camera, 
  * (weights HOST [n_planes][3]; each product rounded, then added, in order of g, in float64). On unresolved sums the
  * result is the sums of the scene with group g's emittance scaled by weights[g] (plane n_planes - 1: the sky), and
  * feeds mcrt_progressive_resolve[_tiles]_dev and mcrt_denoise_dev as they are. out_dev must not overlap planes_dev.
- * MCRT_ERR_INVALID: null pointers, n_planes 0, n_values not a multiple of 3. */
+ * MCRT_ERR_INVALID: null pointers, n_planes 0, n_values not a multiple of 3. The function is a plain weighted sum of
+ * planes, so it recombines the light-path AOV planes of mcrt_render_accumulate_aovs_dev the same way. */
 int mcrt_light_groups_combine_dev(mcrt_ctx* ctx, const double* planes_dev, uint32_t n_planes, uint64_t n_values,
                                   const double* weights, double* out_dev);
+
+/* Light-path AOVs: the path tracer's contributions split by the kind of scattering they come through. The reference's
+ * material model picks exactly one interaction type (reflection, refraction or diffuse) per vertex, and next-event
+ * estimation and BSDF sampling at that vertex both use it, so "the lobe of the first scattering vertex" (the camera ray's
+ * hit) is one value per path. A contribution is direct when its light path has exactly one scattering vertex: light
+ * sampled from the first vertex, or the sky or an emitter reached by the ray leaving it; every later contribution is
+ * indirect.
+ *   plane 0 MCRT_AOV_BACKGROUND                the sky seen by the camera ray (it hits nothing)
+ *   plane 1 MCRT_AOV_EMISSION                  an emitter seen by the camera ray
+ *   plane 2 / 3 MCRT_AOV_DIFFUSE_DIRECT / _INDIRECT            the first vertex scattered diffusely
+ *   plane 4 / 5 MCRT_AOV_REFLECTION_DIRECT / _INDIRECT         ... reflected: mirrors, conductors, GGX, the Fresnel
+ *                                                              reflection of dielectric and coated materials
+ *   plane 6 / 7 MCRT_AOV_TRANSMISSION_DIRECT / _INDIRECT       ... refracted
+ * Every contribution lands in exactly one plane, so the planes add up to the beauty sums. */
+enum {
+    MCRT_AOV_BACKGROUND = 0, MCRT_AOV_EMISSION = 1, MCRT_AOV_DIFFUSE_DIRECT = 2, MCRT_AOV_DIFFUSE_INDIRECT = 3,
+    MCRT_AOV_REFLECTION_DIRECT = 4, MCRT_AOV_REFLECTION_INDIRECT = 5, MCRT_AOV_TRANSMISSION_DIRECT = 6,
+    MCRT_AOV_TRANSMISSION_INDIRECT = 7, MCRT_AOV_COUNT = 8
+};
+/* mcrt_render_accumulate_dev (active_tiles NULL) or mcrt_render_accumulate_tiles_dev (active_tiles HOST, same mask
+ * layout) into the AOV planes planes_dev[MCRT_AOV_COUNT][n_rows*W][3] (path tracer, box film; the box film's weight is
+ * the sample count). The planes add up to the sums of the one-plane entry points over the same samples, and
+ * mcrt_light_groups_combine_dev, mcrt_progressive_resolve[_tiles]_dev and mcrt_denoise_dev take them or their weighted
+ * sums. MCRT_ERR_INVALID: n_planes != MCRT_AOV_COUNT, a null planes_dev, and every argument the one-plane entry points
+ * refuse. MCRT_ERR_UNSUPPORTED: a reconstruction filter, the photon mapper. Nothing is written when a call is refused.
+ * The light-group table plays no part here, and the other entry points write no AOVs. */
+int mcrt_render_accumulate_aovs_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_t y_first, uint32_t y_step, uint32_t n_rows,
+                                    uint32_t tile, const uint8_t* active_tiles, uint32_t sample_first, uint32_t sample_count,
+                                    uint32_t global_seed, int integrator_kind, int precision, double* planes_dev,
+                                    uint32_t n_planes, mcrt_stats* stats);
 
 /* Denoising a progressive frame (mcrt_denoise_dev) needs per-pixel guides: the first hits of the camera rays of samples
  * [sample_first, sample_first + sample_count) of every pixel of the whole width x height frame add

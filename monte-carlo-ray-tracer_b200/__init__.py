@@ -41,7 +41,13 @@ ABI_SYMBOLS = [
     "mcrt_render_features_dev", "mcrt_denoise_dev", "mcrt_render_features_chain_dev",
     "mcrt_photon_emit_pass", "mcrt_photon_gather_radius", "mcrt_photon_gather_search",
     "mcrt_set_light_groups", "mcrt_render_accumulate_groups_dev", "mcrt_light_groups_combine_dev",
+    "mcrt_render_accumulate_aovs_dev",
 ]
+
+# The light-path AOV planes of mcrt_render_accumulate_aovs_dev, in plane order (MCRT_AOV_* of include/mcrt_abi.h):
+# the camera ray's own sky and emitter, then direct / indirect light by the lobe of the first scattering vertex
+AOV_NAMES = ("background", "emission", "diffuse_direct", "diffuse_indirect", "reflection_direct", "reflection_indirect",
+             "transmission_direct", "transmission_indirect")
 
 
 class McrtError(RuntimeError):
@@ -242,6 +248,7 @@ def lib():
         L.mcrt_render_accumulate_groups_dev.argtypes = [C.c_void_p, C.POINTER(CameraRec), C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
                                                         C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int, C.c_int, C.c_void_p,
                                                         C.c_uint32, C.POINTER(Stats)]
+        L.mcrt_render_accumulate_aovs_dev.argtypes = L.mcrt_render_accumulate_groups_dev.argtypes
         L.mcrt_light_groups_combine_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint64, C.c_void_p, C.c_void_p]
         L.mcrt_render_features_dev.argtypes = [C.c_void_p, C.POINTER(CameraRec), C.c_uint32, C.c_uint32, C.c_uint32, C.c_int,
                                                C.c_void_p, C.POINTER(Stats)]
@@ -679,6 +686,18 @@ class Integrator:
                                      y_first=0, y_step=1, n_rows=None, precision=None):
         """mcrt_render_accumulate_groups_dev: render_accumulate_dev (active None) or render_accumulate_tiles_dev into the
         light-group planes planes_ptr [n_planes, n_rows, width, 3] (device)."""
+        return self._render_accumulate_planes(lib().mcrt_render_accumulate_groups_dev, camera, planes_ptr, n_planes, sample_first,
+                                              sample_count, tile, active, y_first, y_step, n_rows, precision)
+
+    def render_accumulate_aovs_dev(self, camera, planes_ptr, sample_first, sample_count, tile=0, active=None,
+                                   y_first=0, y_step=1, n_rows=None, precision=None):
+        """mcrt_render_accumulate_aovs_dev: render_accumulate_dev (active None) or render_accumulate_tiles_dev into the
+        light-path AOV planes planes_ptr [8, n_rows, width, 3] (device), in the order of AOV_NAMES."""
+        return self._render_accumulate_planes(lib().mcrt_render_accumulate_aovs_dev, camera, planes_ptr, len(AOV_NAMES), sample_first,
+                                              sample_count, tile, active, y_first, y_step, n_rows, precision)
+
+    def _render_accumulate_planes(self, fn, camera, planes_ptr, n_planes, sample_first, sample_count, tile, active, y_first,
+                                  y_step, n_rows, precision):
         self.set_film(camera)
         n_rows = len(range(y_first, camera.height, y_step)) if n_rows is None else n_rows
         mask = None
@@ -687,17 +706,17 @@ class Integrator:
             if mask.shape != tile_grid(n_rows, camera.width, tile):
                 raise McrtError(f"tile mask has shape {mask.shape}, expected {tile_grid(n_rows, camera.width, tile)}")
         st = Stats()
-        self._check(lib().mcrt_render_accumulate_groups_dev(self.ctx, C.byref(camera.rec), y_first, y_step, n_rows, tile,
-                                                            mask.ctypes.data_as(C.c_void_p) if mask is not None else None,
-                                                            sample_first, sample_count, self.global_seed, self.kind,
-                                                            self.precision if precision is None else precision,
-                                                            C.c_void_p(planes_ptr), n_planes, C.byref(st)))
+        self._check(fn(self.ctx, C.byref(camera.rec), y_first, y_step, n_rows, tile,
+                       mask.ctypes.data_as(C.c_void_p) if mask is not None else None, sample_first, sample_count,
+                       self.global_seed, self.kind, self.precision if precision is None else precision,
+                       C.c_void_p(planes_ptr), n_planes, C.byref(st)))
         self.last_stats = st.as_dict()
         return self.last_stats
 
     def light_groups_combine_dev(self, planes_ptr, n_planes, n_values, weights, out_ptr):
         """mcrt_light_groups_combine_dev: out = sum over g of weights[g] * plane g, added in order of g (device buffers of
-        n_values float64 per plane). weights: [n_planes, 3] or [n_planes] (one weight for all three channels)."""
+        n_values float64 per plane). weights: [n_planes, 3] or [n_planes] (one weight for all three channels). The
+        planes may be light-group or AOV planes: the kernel is a plain weighted sum."""
         w = light_group_weights(weights, n_planes)
         self._check(lib().mcrt_light_groups_combine_dev(self.ctx, C.c_void_p(planes_ptr), n_planes, n_values,
                                                         w.ctypes.data_as(C.c_void_p), C.c_void_p(out_ptr)))
@@ -822,6 +841,9 @@ class PhotonMapper(Integrator):
 
     def set_light_groups(self, ids, n_groups=None):
         raise McrtError("the photon mapper has no light groups: photons carry no light index")
+
+    def render_accumulate_aovs_dev(self, *args, **kwargs):
+        raise McrtError("the photon mapper has no light-path AOVs")
 
     def _emit_params(self, emissions, caustic_factor, max_photons_per_octree_leaf, k_nearest_photons, direct_visualization, scene_bounds):
         p = PhotonEmitParams()
@@ -1170,14 +1192,23 @@ class Progressive:
     A and B then hold one plane per group and one for the sky, [G+1, rows, width, 3], filled by
     mcrt_render_accumulate_groups_dev. frame, error, render, render_adaptive and denoise work on the planes' sum, the
     beauty frame, so they behave as without groups; group_frames() resolves each plane, and relight(weights) and
-    denoise(weights=...) work on any weighted sum (mcrt_light_groups_combine_dev), without rendering again."""
+    denoise(weights=...) work on any weighted sum (mcrt_light_groups_combine_dev), without rendering again.
+
+    Light-path AOVs (aovs=True; box film, path tracer, not together with light groups): A and B hold the 8 planes of
+    AOV_NAMES, [8, rows, width, 3], filled by mcrt_render_accumulate_aovs_dev. frame, error, render, render_adaptive
+    and denoise work on the planes' sum, as with light groups; aov_frames() resolves each plane with its own noise
+    estimate, and relight(weights) and denoise(weights=...) recomposite the frame from weighted planes."""
 
     _STATS = ("paths", "extension_rays", "shadow_rays")
 
-    def __init__(self, integrator, camera, y_first=0, y_step=1, n_rows=None, tile=16, light_groups=None):
+    def __init__(self, integrator, camera, y_first=0, y_step=1, n_rows=None, tile=16, light_groups=None, aovs=False):
         import torch
         if light_groups is not None and integrator.kind == INTEGRATOR_PHOTON:
             raise McrtError("the photon mapper has no light groups: photons carry no light index")
+        if aovs and integrator.kind == INTEGRATOR_PHOTON:
+            raise McrtError("the photon mapper has no light-path AOVs")
+        if aovs and light_groups is not None:
+            raise McrtError("light groups and light-path AOVs in one render are not supported")
         self.integrator, self.camera = integrator, camera
         self.y_first, self.y_step = int(y_first), int(y_step)
         self.n_rows = len(range(self.y_first, camera.height, self.y_step)) if n_rows is None else int(n_rows)
@@ -1192,7 +1223,12 @@ class Progressive:
             self.light_groups = np.ascontiguousarray(light_groups, dtype=np.uint32).reshape(-1)
             self.n_planes = (int(self.light_groups.max()) + 1 if self.light_groups.size else 0) + 1
             integrator.set_light_groups(self.light_groups, self.n_planes - 1)   # refuses a wrong table before anything is allocated
-        planes = (self.n_planes,) if self.light_groups is not None else ()
+        self.aovs = bool(aovs)
+        if self.aovs:
+            if self.filtered:
+                raise McrtError("light-path AOVs take the box film only")
+            self.n_planes = len(AOV_NAMES)
+        planes = (self.n_planes,) if self._planar else ()
         dev = torch.device("cuda", integrator.device)
         self.rgb = [torch.zeros(planes + (self.rows, camera.width, 3), dtype=torch.float64, device=dev) for _ in range(2)]
         self.wsum = [torch.zeros((self.rows, camera.width), dtype=torch.float64, device=dev) for _ in range(2)] if self.filtered else None
@@ -1212,6 +1248,11 @@ class Progressive:
     def samples(self):
         return self.counts[0] + self.counts[1]
 
+    @property
+    def _planar(self):
+        """A and B hold planes (light groups or AOVs) whose sum is the beauty frame's sums."""
+        return self.light_groups is not None or self.aovs
+
     def add(self, samples):
         """Renders samples [self.samples, self.samples + samples) of the active tiles into A (even pass) or B (odd pass)."""
         half = self.passes % 2
@@ -1221,6 +1262,10 @@ class Progressive:
             st = self.integrator.render_accumulate_groups_dev(self.camera, self.rgb[half].data_ptr(), self.n_planes, self.samples,
                                                               int(samples), self.tile, None if self.active.all() else self.active,
                                                               self.y_first, self.y_step, self.n_rows)
+        elif self.aovs:
+            st = self.integrator.render_accumulate_aovs_dev(self.camera, self.rgb[half].data_ptr(), self.samples, int(samples), self.tile,
+                                                            None if self.active.all() else self.active, self.y_first, self.y_step,
+                                                            self.n_rows)
         elif self.active.all():
             st = self.integrator.render_accumulate_dev(self.camera, self.rgb[half].data_ptr(), wsum, self.samples,
                                                        int(samples), self.y_first, self.y_step, self.n_rows)
@@ -1243,12 +1288,12 @@ class Progressive:
         return self._resolved
 
     def _halves(self, weights=None):
-        """The sums of halves A and B, [rows, width, 3] each: with light groups the combination of their planes with
-        weights [G+1, 3] or [G+1] (None: every weight 1, the beauty frame's sums)."""
+        """The sums of halves A and B, [rows, width, 3] each: with light groups or AOVs the combination of their planes
+        with weights [n_planes, 3] or [n_planes] (None: every weight 1, the beauty frame's sums)."""
         import torch
-        if self.light_groups is None:
+        if not self._planar:
             if weights is not None:
-                raise McrtError("weights need a render with light groups")
+                raise McrtError("weights need a render with light groups or AOVs")
             return self.rgb
         w = np.ones(self.n_planes) if weights is None else weights
         out = []
@@ -1289,10 +1334,20 @@ class Progressive:
             raise McrtError("group_frames needs a render with light groups")
         return np.stack([self._resolve_halves([self.rgb[0][g], self.rgb[1][g]])[0] for g in range(self.n_planes)])
 
+    # -- light-path AOVs
+    def aov_frames(self):
+        """Each AOV plane resolved on its own (in the order of AOV_NAMES) -> (frames float64 [8, rows, width, 3], each
+        plane's relative error float64 [8], estimated from the difference of its two halves like error()'s)."""
+        if not self.aovs:
+            raise McrtError("aov_frames needs a render with aovs=True")
+        res = [self._resolve_halves([self.rgb[0][k], self.rgb[1][k]]) for k in range(self.n_planes)]
+        return np.stack([r[0] for r in res]), np.array([r[1] for r in res])
+
     def relight(self, weights):
-        """The frame relit: the planes summed with weights [G+1, 3] or [G+1] (the last row weights the sky), resolved
-        like frame() -> (frame, frame relative error, per-tile relative errors). Weight w_g on group g equals a render
-        of the scene with group g's emittance scaled by w_g."""
+        """The frame recomposited: the planes summed with weights [n_planes, 3] or [n_planes], resolved like frame()
+        -> (frame, frame relative error, per-tile relative errors). Light groups: the last row weights the sky, and
+        weight w_g on group g equals a render of the scene with group g's emittance scaled by w_g. AOVs: the rows weight
+        the planes of AOV_NAMES, e.g. 0 on the reflection planes removes what the first vertex reflected."""
         frame, err, tiles, _ = self._resolve_halves(self._halves(weights))
         return frame, err, tiles
 
@@ -1403,7 +1458,8 @@ class Progressive:
         their own surface; rough and glossy lobes are never followed; the feature samples [0, F) also feed half A; the Owen-scrambled halves are not
         independent, so the residual estimate can read about 10 % low.
 
-        weights (light groups only): denoise the frame relit with these weights (relight) instead of the beauty frame."""
+        weights (light groups or AOVs only): denoise the frame relit or recomposited with these weights (relight) instead of
+        the beauty frame."""
         import torch
         if (self.y_first, self.y_step, self.n_rows) != (0, 1, self.camera.height):
             raise McrtError("denoise needs the whole frame as the row set (y_first 0, y_step 1, n_rows = height)")
@@ -1442,6 +1498,8 @@ class Progressive:
             ident.update(self._photon_identity())
         if self.light_groups is not None:
             ident["light_groups"] = self.light_groups.copy()
+        if self.aovs:
+            ident["aovs"] = np.int64(len(AOV_NAMES))
         return ident
 
     def _photon_identity(self):
@@ -1466,14 +1524,14 @@ class Progressive:
             np.savez(f, **data)
 
     @classmethod
-    def load(cls, path, integrator, camera, tile=None, light_groups=None):
+    def load(cls, path, integrator, camera, tile=None, light_groups=None, aovs=False):
         """Resumes a checkpoint written by save() with `integrator` and `camera` (and `tile`, the checkpoint's if None).
         Raises McrtError, and resumes nothing, when the seed, precision, integrator kind, camera, film, tile, scene,
-        photon maps or light groups differ from the checkpoint's. A checkpoint without tile state resumes with every
-        tile active."""
+        photon maps, light groups or AOVs differ from the checkpoint's. A checkpoint without tile state resumes with
+        every tile active."""
         data = _read_checkpoint(path)
         y_first, y_step, n_rows = (int(v) for v in data["row_set"])
-        p = cls(integrator, camera, y_first, y_step, n_rows, int(data["tile"]) if tile is None else int(tile), light_groups)
+        p = cls(integrator, camera, y_first, y_step, n_rows, int(data["tile"]) if tile is None else int(tile), light_groups, aovs)
         p._restore(path, data)
         return p
 
@@ -1483,6 +1541,8 @@ class Progressive:
         ident = self._identity()
         if ("light_groups" in data) != ("light_groups" in ident):
             raise McrtError(f"checkpoint {path}: light groups differ from this render's; not resuming")
+        if ("aovs" in data) != ("aovs" in ident):
+            raise McrtError(f"checkpoint {path}: light-path AOVs differ from this render's; not resuming")
         for k, want in ident.items():
             if k not in data or not np.array_equal(data[k], want):
                 raise McrtError(f"checkpoint {path}: {k} differs from this render's; not resuming")
@@ -1548,11 +1608,13 @@ class ProgressivePhotonMapping(Progressive):
     the next add() emits again (the passes are deterministic)."""
 
     def __init__(self, photon_mapper, camera, emissions, caustic_factor, max_photons_per_octree_leaf=200, alpha=2 / 3,
-                 radius=None, k_nearest_photons=50, tile=16, light_groups=None):
+                 radius=None, k_nearest_photons=50, tile=16, light_groups=None, aovs=False):
         if not isinstance(photon_mapper, PhotonMapper):
             raise McrtError("ProgressivePhotonMapping needs a PhotonMapper")
         if light_groups is not None:
             raise McrtError("the photon mapper has no light groups: photons carry no light index")
+        if aovs:
+            raise McrtError("the photon mapper has no light-path AOVs")
         ppm_radii(1.0, alpha, 1)   # validates alpha
         self.emissions, self.caustic_factor = int(emissions), float(caustic_factor)
         self.max_photons_per_octree_leaf, self.k_nearest_photons = int(max_photons_per_octree_leaf), int(k_nearest_photons)

@@ -679,6 +679,7 @@ namespace
         double* rgb;    // box film [n_pixels][3] in film_index order; filtered film [height*width][3]
         double* wsum;   // filtered film [height*width]; null with the box film
         uint32_t n_planes = 0;   // box film only: rgb holds this many light-group planes (mcrt_render_accumulate_groups_dev)
+        bool aovs = false;       // ... or the MCRT_AOV_COUNT light-path planes (mcrt_render_accumulate_aovs_dev)
     };
 
     // The wavefront loop shared by mcrt_render_rows(_dev) and mcrt_sample_rays. Camera work item w is sample
@@ -747,6 +748,7 @@ namespace
             p.group_of_light = ctx->d_group_of_light;
             p.plane_values = film_pixels * 3;
             p.n_planes = accum->n_planes;
+            p.aovs = accum->aovs ? 1u : 0u;
         }
         p.filmp.is_default_box = filtered ? 0u : 1u;
         if (filtered)
@@ -1753,7 +1755,7 @@ int mcrt_render_accumulate_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_
 
 namespace
 {
-    // The active-tile path of mcrt_render_accumulate_tiles_dev / _groups_dev (the caller has checked the sums)
+    // The active-tile path of mcrt_render_accumulate_tiles_dev / _groups_dev / _aovs_dev (the caller has checked the sums)
     int accumulateTiles(mcrt_ctx* ctx, const std::string& name, const mcrt_camera* camera, uint32_t y_first, uint32_t y_step,
                         uint32_t n_rows, uint32_t tile, const uint8_t* active_tiles, uint32_t sample_first, uint32_t sample_count,
                         uint32_t global_seed, int integrator_kind, int precision, const FilmSums& sums, mcrt_stats* stats)
@@ -1883,6 +1885,35 @@ int mcrt_render_accumulate_groups_dev(mcrt_ctx* ctx, const mcrt_camera* camera, 
     int rc;
     if ((rc = checkAccumulateSums(ctx, name.c_str(), sample_count, planes_dev, nullptr))) return rc;
     const FilmSums sums = { planes_dev, nullptr, n_planes };
+    if (active_tiles)
+        return accumulateTiles(ctx, name, camera, y_first, y_step, n_rows, tile, active_tiles, sample_first, sample_count, global_seed,
+                               integrator_kind, precision, sums, stats);
+    CK(cudaSetDevice(ctx->device));
+    return renderDispatch(ctx, camera, y_first, y_step, n_rows, sample_first, sample_count, global_seed, integrator_kind,
+                          precision, nullptr, stats, &sums);
+}
+
+int mcrt_render_accumulate_aovs_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_t y_first, uint32_t y_step, uint32_t n_rows,
+                                    uint32_t tile, const uint8_t* active_tiles, uint32_t sample_first, uint32_t sample_count,
+                                    uint32_t global_seed, int integrator_kind, int precision, double* planes_dev,
+                                    uint32_t n_planes, mcrt_stats* stats)
+{
+    if (!ctx) return MCRT_ERR_INVALID;
+    const std::string name = "mcrt_render_accumulate_aovs_dev";
+    if (!ctx->film_default) { ctx->error = name + ": AOV planes take the box film only"; return MCRT_ERR_UNSUPPORTED; }
+    if (integrator_kind == MCRT_INTEGRATOR_PHOTON)
+    {
+        ctx->error = name + ": the photon mapper has no light-path AOVs (its estimates are not split by first lobe)";
+        return MCRT_ERR_UNSUPPORTED;
+    }
+    if (n_planes != MCRT_AOV_COUNT)
+    {
+        ctx->error = name + ": n_planes " + std::to_string(n_planes) + ", an AOV render has " + std::to_string(MCRT_AOV_COUNT);
+        return MCRT_ERR_INVALID;
+    }
+    int rc;
+    if ((rc = checkAccumulateSums(ctx, name.c_str(), sample_count, planes_dev, nullptr))) return rc;
+    const FilmSums sums = { planes_dev, nullptr, n_planes, true };
     if (active_tiles)
         return accumulateTiles(ctx, name, camera, y_first, y_step, n_rows, tile, active_tiles, sample_first, sample_count, global_seed,
                                integrator_kind, precision, sums, stats);

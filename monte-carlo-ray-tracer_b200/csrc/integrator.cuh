@@ -24,6 +24,7 @@
 #include "bvh4.cuh"
 #include "photon.cuh"
 #include "film.cuh"
+#include "mcrt_abi.h"
 
 // launch-bound knobs (overridable at build time for tuning experiments)
 // (float traversal runs at 64 registers / 32 warps per SM; double traversal keeps 128 registers, since it
@@ -93,7 +94,7 @@ namespace mcrt
         V4<R>* iors_a;   // iors[1..4]  (touched only while the path is inside nested media)
         V4<R>* iors_b;   // iors[5..7]
         uint4* meta;     // pixel, sample, depth | diffuse_depth<<16, refraction_level
-        uint4* meta2;    // ls.light as light index, ior_count | dirac<<8, film_index, source prim (fast mode)
+        uint4* meta2;    // ls.light as light index, ior_count | dirac<<8 | first lobe<<9 (FILM_MODE_AOV), film_index, source prim (fast mode)
     };
 
     // One shadow ray. k_shadow reads the queue through the ray-coherence sort, i.e. at random positions,
@@ -104,7 +105,7 @@ namespace mcrt
     {
         V4<R> o;         // start.xyz, bsdf_pdf
         V4<R> d;         // direction.xyz, area * cos_light
-        uint4 meta;      // light prim, film_index, source prim, sample
+        uint4 meta;      // light prim, film_index, source prim, sample (FILM_MODE_AOV: the AOV plane)
         V4<R> k;         // bsdf_absIdotN * Le * throughput, select_probability
     };
     static_assert(sizeof(ShadowRecord<double>) == 128 && sizeof(ShadowRecord<float>) == 64, "one shadow record per line");
@@ -255,10 +256,12 @@ namespace mcrt
         EmitParams<R> emit;         // photon emission pass (mcrt_photon_emit) only
         FilmParams filmp;           // reconstruction filter (default box: only `film` is used)
         // light-group render (mcrt_render_accumulate_groups_dev): `film` holds n_planes planes of plane_values values each;
-        // a contribution of light l goes to plane group_of_light[l], the sky's to plane n_planes - 1. 0: one plane
+        // a contribution of light l goes to plane group_of_light[l], the sky's to plane n_planes - 1. 0: one plane.
+        // AOV render (mcrt_render_accumulate_aovs_dev, aovs = 1): n_planes = MCRT_AOV_COUNT light-path planes instead
         const uint32_t* group_of_light;
         size_t plane_values;
         uint32_t n_planes;
+        uint32_t aovs;
     };
 
     // ------------------------------------------------------------------------------------------
@@ -355,14 +358,26 @@ namespace mcrt
     }
 
     // Film modes of the depositing kernels. FILM_MODE_BOX: the default box film, the kernels every benchmark and parity
-    // case runs; FILM_MODE_SPLAT: a reconstruction filter; FILM_MODE_GROUPS: the box film with one plane per light group
-    enum FilmMode : int { FILM_MODE_BOX = 0, FILM_MODE_SPLAT = 1, FILM_MODE_GROUPS = 2 };
+    // case runs; FILM_MODE_SPLAT: a reconstruction filter; FILM_MODE_GROUPS: the box film with one plane per light group;
+    // FILM_MODE_AOV: the box film with one plane per light-path class (MCRT_AOV_*)
+    enum FilmMode : int { FILM_MODE_BOX = 0, FILM_MODE_SPLAT = 1, FILM_MODE_GROUPS = 2, FILM_MODE_AOV = 3 };
+
+    // AOV plane of a contribution. lobe: interaction type + 1 of the path's first scattering vertex, 0 for the camera
+    // ray's own miss (the sky: background) or emitter hit (emission); indirect: the light path has more than one
+    // scattering vertex
+    MCRT_D uint32_t aovPlane(uint32_t lobe, bool indirect, bool miss)
+    {
+        if (lobe == 0u) return miss ? MCRT_AOV_BACKGROUND : MCRT_AOV_EMISSION;
+        const uint32_t direct = lobe == IA_DIFFUSE + 1u ? MCRT_AOV_DIFFUSE_DIRECT
+                              : (lobe == IA_REFLECT + 1u ? MCRT_AOV_REFLECTION_DIRECT : MCRT_AOV_TRANSMISSION_DIRECT);
+        return direct + (indirect ? 1u : 0u);
+    }
 
     // Film::deposit of one radiance contribution of sample (pixel, sample). light: index of the emitter it comes from,
-    // NO_PRIM for the sky (read by FILM_MODE_GROUPS only)
+    // NO_PRIM for the sky (read by FILM_MODE_GROUPS only); plane: its AOV plane (read by FILM_MODE_AOV only)
     template <int FILM, class R>
     MCRT_D void depositRadiance(const WaveParams<R>& p, uint32_t film_index, uint32_t pixel, uint32_t sample, const V3<R>& v,
-                                uint32_t light = NO_PRIM)
+                                uint32_t light = NO_PRIM, uint32_t plane = 0u)
     {
         if constexpr (FILM == FILM_MODE_BOX)
         {
@@ -371,6 +386,10 @@ namespace mcrt
         else if constexpr (FILM == FILM_MODE_GROUPS)
         {
             const uint32_t plane = light == NO_PRIM ? p.n_planes - 1u : p.group_of_light[light];
+            filmAddV(p.film + plane * p.plane_values, film_index, v);
+        }
+        else if constexpr (FILM == FILM_MODE_AOV)
+        {
             filmAddV(p.film + plane * p.plane_values, film_index, v);
         }
         else
@@ -659,6 +678,8 @@ namespace mcrt
             V3<R> sh_o, sh_d, sh_k;
             R sh_bsdf_pdf = R(0), sh_area_cos = R(0), sh_select = R(0);
             uint32_t sh_light = NO_PRIM;
+            // FILM_MODE_AOV: interaction type + 1 of the path's first vertex (0 before it), the shadow ray's AOV plane
+            uint32_t lobe = 0, sh_plane = 0;
 
             if (alive)
             {
@@ -672,6 +693,7 @@ namespace mcrt
                 ls_light = meta2.x;
                 ior_count = meta2.y & 0xFFu;
                 ray.dirac_delta = (meta2.y >> 8) & 1u;
+                if constexpr (FILM == FILM_MODE_AOV) lobe = (meta2.y >> 9) & 3u;
                 ray.refraction = false;
                 const uint32_t film_index = meta2.z;
 
@@ -704,7 +726,9 @@ namespace mcrt
                 if (hit.prim == NO_PRIM)
                 {
                     // path-tracer.cpp:27-30; the photon mapper adds no sky (photon-mapper.cpp:292-295)
-                    if constexpr (KIND == 0) depositRadiance<FILM>(p, film_index, meta.x, meta.y, skyColor(ray.direction) * throughput);
+                    if constexpr (KIND == 0)
+                        depositRadiance<FILM>(p, film_index, meta.x, meta.y, skyColor(ray.direction) * throughput, NO_PRIM,
+                                              FILM == FILM_MODE_AOV ? aovPlane(lobe, ray.depth > 1u, true) : 0u);
                     alive = false;
                 }
                 else
@@ -728,16 +752,21 @@ namespace mcrt
                     {
                         if (ray.depth == 0 || ray.dirac_delta)
                         {
-                            depositRadiance<FILM>(p, film_index, meta.x, meta.y, m.emittance * throughput, ps.light);
+                            depositRadiance<FILM>(p, film_index, meta.x, meta.y, m.emittance * throughput, ps.light,
+                                                  FILM == FILM_MODE_AOV ? aovPlane(lobe, ray.depth > 1u, false) : 0u);
                         }
                         else if (ls_light != NO_PRIM && sc.lights[ls_light].prim == hit.prim)
                         {
                             R cos_light_theta = dot(ia.out, ia.normal);
                             R light_pdf = pow2(ia.t) / (ps.area * cos_light_theta);
                             R mis_weight = powerHeuristic(ls_bsdf_pdf, light_pdf);
-                            depositRadiance<FILM>(p, film_index, meta.x, meta.y, (mis_weight * m.emittance / ls_select) * throughput, ls_light);
+                            depositRadiance<FILM>(p, film_index, meta.x, meta.y, (mis_weight * m.emittance / ls_select) * throughput, ls_light,
+                                                  FILM == FILM_MODE_AOV ? aovPlane(lobe, ray.depth > 1u, false) : 0u);
                         }
                     }
+
+                    // the camera ray's hit is the first vertex: its lobe is the path's, for NEE here and everything after
+                    if constexpr (FILM == FILM_MODE_AOV) if (ray.depth == 0) lobe = ia.type + 1u;
 
                     // ---- PhotonMapper::sampleRay control flow, photon-mapper.cpp:299-332
                     bool do_direct = true, do_bsdf = true;
@@ -825,6 +854,7 @@ namespace mcrt
                                     sh_area_cos = L.area * cos_light_theta;
                                     sh_select = ls_select;
                                     sh_light = L.prim;
+                                    if constexpr (FILM == FILM_MODE_AOV) sh_plane = aovPlane(lobe, ray.depth > 0u, false);
                                 }
                             }
                         }
@@ -906,7 +936,7 @@ namespace mcrt
                 }
                 stStream(&out.meta[slot], make_uint4(meta.x, meta.y, (nray.depth & 0xFFFFu) | (nray.diffuse_depth << 16),
                                                      (uint32_t)nray.refraction_level));
-                stStream(&out.meta2[slot], make_uint4(ls_light, ior_count | (nray.dirac_delta ? 256u : 0u), meta2.z,
+                stStream(&out.meta2[slot], make_uint4(ls_light, ior_count | (nray.dirac_delta ? 256u : 0u) | (lobe << 9), meta2.z,
                                                       sc.shade[hit_prim].type == PRIM_TRIANGLE ? hit_prim : NO_PRIM));
                 if (sorting) { p.sort.path_key[cur ^ 1][slot] = pkey; p.sort.path_rank[cur ^ 1][slot] = prank; }
             }
@@ -915,7 +945,8 @@ namespace mcrt
                 ShadowRecord<R>& srec = p.shadow[sslot];
                 stStream(&srec.o, V4<R>(sh_o, sh_bsdf_pdf));
                 stStream(&srec.d, V4<R>(sh_d, sh_area_cos));
-                stStream(&srec.meta, make_uint4(sh_light, meta2.z, sc.shade[hit_prim].type == PRIM_TRIANGLE ? hit_prim : NO_PRIM, meta.y));
+                stStream(&srec.meta, make_uint4(sh_light, meta2.z, sc.shade[hit_prim].type == PRIM_TRIANGLE ? hit_prim : NO_PRIM,
+                                                FILM == FILM_MODE_AOV ? sh_plane : meta.y));
                 // float64: also write the padding after meta, so that no 32-byte sector of the record is left half
                 // written (without this store the C2 shade stage measured 930 instead of 744 ms per frame)
                 if constexpr (sizeof(R) == 8) stStream(reinterpret_cast<uint4*>(&srec) + 5, make_uint4(0u, 0u, 0u, 0u));
@@ -941,7 +972,8 @@ namespace mcrt
         if (stack_overflows) atomicAdd(&c->ior_stack_overflows, (unsigned long long)stack_overflows);
     }
 
-    // FILM_MODE_GROUPS finds the sampled light's group through the light primitive's shading record (sm.x is L.prim)
+    // FILM_MODE_GROUPS finds the sampled light's group through the light primitive's shading record (sm.x is L.prim);
+    // FILM_MODE_AOV reads the AOV plane k_shade stored in place of the sample index (sm.w)
     template <class R, int FILM, int PRIMS, int FAST>
     __global__ void __launch_bounds__(256, FAST == 2 ? MCRT_TRACE_MINBLOCKS_DYN : (FAST == 1 ? MCRT_TRACE_MINBLOCKS_FAST : (PRIMS == PRIMS_ALL ? Mode<R>::trace_minblocks : Mode<R>::trace_minblocks_pruned))) k_shadow(WaveParams<R> p)
     {
@@ -973,7 +1005,7 @@ namespace mcrt
                         R light_pdf = pow2(h.t) / sd.w;
                         R mis_weight = powerHeuristic(light_pdf, so.w);
                         depositRadiance<FILM>(p, sm.y, pixelOfFilmIndex(p, sm.y), sm.w, sk.xyz() * (mis_weight / (light_pdf * sk.w)),
-                                              FILM == FILM_MODE_GROUPS ? p.scene.shade[sm.x].light : NO_PRIM);
+                                              FILM == FILM_MODE_GROUPS ? p.scene.shade[sm.x].light : NO_PRIM, sm.w);
                     }
                 }, cnt, overflow);
             flushStats(p.counters, cnt, rays, true, overflow);
@@ -996,7 +1028,7 @@ namespace mcrt
                 R light_pdf = pow2(h.t) / sd.w;
                 R mis_weight = powerHeuristic(light_pdf, so.w);
                 depositRadiance<FILM>(p, sm.y, pixelOfFilmIndex(p, sm.y), sm.w, sk.xyz() * (mis_weight / (light_pdf * sk.w)),
-                                      FILM == FILM_MODE_GROUPS ? p.scene.shade[sm.x].light : NO_PRIM);
+                                      FILM == FILM_MODE_GROUPS ? p.scene.shade[sm.x].light : NO_PRIM, sm.w);
             }
         }
         flushStats(p.counters, cnt, rays, true, overflow);
