@@ -277,6 +277,12 @@ int mcrt_photon_gather_search(mcrt_ctx* ctx, int which, const double* points_xyz
  * valid until the next mcrt_photon_emit / mcrt_destroy. */
 int mcrt_photon_download(mcrt_ctx* ctx, int which, mcrt_photon_map_desc* out);
 
+/* The index of the light that emitted each photon of a built map (which: 0 caustic, 1 global), out[n] HOST, in the
+ * order mcrt_photon_download returns the photons; n must be the map's photon count. Maps emitted by mcrt_photon_emit /
+ * mcrt_photon_emit_pass carry these indices; maps of mcrt_photon_upload and mcrt_photon_build_dev do not
+ * (MCRT_ERR_UNSUPPORTED), and neither do maps emitted before the last mcrt_scene_upload. */
+int mcrt_photon_download_lights(mcrt_ctx* ctx, int which, uint32_t* out, uint64_t n);
+
 /* The octree construction step of mcrt_photon_emit alone, on caller photons: Octree<Photon>
  * insertion + LinearOctree::compact (octree.cpp:34-81, linear-octree.cpp:201-244) on the GPU.
  * photons: HOST, [n][8] floats {flux.xyz, pos.xyz, phi, theta} (copied to the device); the result
@@ -460,10 +466,12 @@ int mcrt_set_light_groups(mcrt_ctx* ctx, const uint32_t* group_of_light, uint32_
 /* mcrt_render_accumulate_dev (active_tiles NULL) or mcrt_render_accumulate_tiles_dev (active_tiles HOST, same mask
  * layout) into light-group planes: planes_dev[n_planes][n_rows*W][3], plane g the sums of group g's lights and plane
  * n_groups the sky's. Every contribution lands in exactly one plane, so the planes add up to the sums of the one-plane
- * entry points over the same samples; the box film's weight is the sample count. MCRT_ERR_INVALID: no group table,
- * n_planes != n_groups + 1, a null planes_dev, and every argument the one-plane entry points refuse.
- * MCRT_ERR_UNSUPPORTED: a reconstruction filter, the photon mapper (photons carry no light index). Nothing is
- * written when a call is refused. */
+ * entry points over the same samples; the box film's weight is the sample count. The photon mapper splits its photon
+ * estimates by the light each photon came from, so it needs maps that carry light indices (mcrt_photon_download_lights);
+ * the photon mapper adds no sky, so its sky plane stays zero. MCRT_ERR_INVALID: no group table, n_planes !=
+ * n_groups + 1, a null planes_dev, and every argument the one-plane entry points refuse. MCRT_ERR_UNSUPPORTED: a
+ * reconstruction filter, the photon mapper with maps that carry no light index (or with no maps). Nothing is written
+ * when a call is refused. */
 int mcrt_render_accumulate_groups_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_t y_first, uint32_t y_step, uint32_t n_rows,
                                       uint32_t tile, const uint8_t* active_tiles, uint32_t sample_first, uint32_t sample_count,
                                       uint32_t global_seed, int integrator_kind, int precision, double* planes_dev,

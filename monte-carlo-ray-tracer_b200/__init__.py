@@ -41,7 +41,7 @@ ABI_SYMBOLS = [
     "mcrt_render_features_dev", "mcrt_denoise_dev", "mcrt_render_features_chain_dev",
     "mcrt_photon_emit_pass", "mcrt_photon_gather_radius", "mcrt_photon_gather_search",
     "mcrt_set_light_groups", "mcrt_render_accumulate_groups_dev", "mcrt_light_groups_combine_dev",
-    "mcrt_render_accumulate_aovs_dev",
+    "mcrt_render_accumulate_aovs_dev", "mcrt_photon_download_lights",
 ]
 
 # The light-path AOV planes of mcrt_render_accumulate_aovs_dev, in plane order (MCRT_AOV_* of include/mcrt_abi.h):
@@ -211,6 +211,7 @@ def lib():
         L.mcrt_photon_gather_search.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.c_double, C.c_void_p, C.c_void_p,
                                                 C.c_void_p, C.POINTER(Stats)]
         L.mcrt_photon_download.argtypes = [C.c_void_p, C.c_int, C.POINTER(PhotonMapDesc)]
+        L.mcrt_photon_download_lights.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_uint64]
         L.mcrt_octree_build.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p, C.POINTER(C.c_void_p),
                                         C.POINTER(PhotonMapDesc), C.POINTER(C.c_double)]
         L.mcrt_octree_free.argtypes = [C.c_void_p]
@@ -822,7 +823,11 @@ class PathTracer(Integrator):
 
 class PhotonMapper(Integrator):
     """Renders with the caustic/global photon maps the CPU photon pass produced (first pass stays on
-    the CPU, SURVEY.md §8f); maps come from the scene pack or from explicit arrays."""
+    the CPU, SURVEY.md §8f); maps come from the scene pack or from explicit arrays.
+
+    Light groups (set_light_groups, render_accumulate_groups_dev, Progressive(light_groups=...)) need maps that record
+    which light emitted each photon: the maps of emit() / emit_pass() do (has_photon_lights, photon_lights); the maps of
+    the scene pack, of photon_maps= and of emit_sharded do not."""
     kind = INTEGRATOR_PHOTON
 
     def __init__(self, scene, device=0, precision=PRECISION_F64, global_seed=0x12345678, photon_maps=None, emit=None):
@@ -839,8 +844,26 @@ class PhotonMapper(Integrator):
         self._maps = maps
         self.upload_photons()
 
+    @property
+    def has_photon_lights(self):
+        """True when the current maps record the light that emitted each photon (maps of emit / emit_pass)."""
+        return getattr(self, "_photon_lights", False)
+
+    def photon_lights(self, which):
+        """The index of the light that emitted each photon of map `which` (0 caustic, 1 global), uint32 [n_photons], in
+        the order of the photons of _maps[which] (mcrt_photon_download_lights)."""
+        if not self.has_photon_lights:
+            raise McrtError("the photon maps carry no light index: only the maps of emit() / emit_pass() do")
+        out = np.zeros(self.n_photons[which], np.uint32)
+        self._check(lib().mcrt_photon_download_lights(self.ctx, int(which), _ptr(out), out.size))
+        return out
+
     def set_light_groups(self, ids, n_groups=None):
-        raise McrtError("the photon mapper has no light groups: photons carry no light index")
+        """Integrator.set_light_groups, for maps that carry light indices (has_photon_lights)."""
+        if not self.has_photon_lights:
+            raise McrtError("the photon mapper has no light groups with these maps: their photons carry no light index "
+                            "(only the maps of emit() / emit_pass() do)")
+        return super().set_light_groups(ids, n_groups)
 
     def render_accumulate_aovs_dev(self, *args, **kwargs):
         raise McrtError("the photon mapper has no light-path AOVs")
@@ -884,6 +907,7 @@ class PhotonMapper(Integrator):
         self.k_nearest = int(k_nearest_photons)
         self._host_maps = None
         self._emitted = (int(k_nearest_photons), int(bool(direct_visualization)))
+        self._photon_lights = False   # the gathered arrays carry no light index
         self.n_photons = (gathered[0].numel() // 8, gathered[1].numel() // 8)
         return self.n_photons
 
@@ -909,6 +933,7 @@ class PhotonMapper(Integrator):
         # the maps stay in HBM (octrees are built there too); host copies only when somebody asks
         self._host_maps = None
         self._emitted = (int(k_nearest_photons), int(bool(direct_visualization)))
+        self._photon_lights = True
         self.n_photons = (nc.value, ng.value)
         return nc.value, ng.value
 
@@ -927,6 +952,7 @@ class PhotonMapper(Integrator):
     def _maps(self, value):
         self._host_maps = value
         self._emitted = None
+        self._photon_lights = False
 
     @staticmethod
     def _map_desc(m):
@@ -1188,8 +1214,8 @@ class Progressive:
     per-tile counts (mcrt_progressive_resolve_tiles_dev). While every tile is active, add, frame and error run the
     uniform entry points. With a reconstruction filter, adaptive passes need the whole frame as the row set.
 
-    Light groups (light_groups = a group id per light, e.g. light_groups_by_emittance(scene)[0]; box film, path tracer):
-    A and B then hold one plane per group and one for the sky, [G+1, rows, width, 3], filled by
+    Light groups (light_groups = a group id per light, e.g. light_groups_by_emittance(scene)[0]; box film; the path tracer,
+    or the photon mapper with maps that record each photon's light, PhotonMapper.has_photon_lights): A and B then hold one plane per group and one for the sky, [G+1, rows, width, 3], filled by
     mcrt_render_accumulate_groups_dev. frame, error, render, render_adaptive and denoise work on the planes' sum, the
     beauty frame, so they behave as without groups; group_frames() resolves each plane, and relight(weights) and
     denoise(weights=...) work on any weighted sum (mcrt_light_groups_combine_dev), without rendering again.
@@ -1203,8 +1229,9 @@ class Progressive:
 
     def __init__(self, integrator, camera, y_first=0, y_step=1, n_rows=None, tile=16, light_groups=None, aovs=False):
         import torch
-        if light_groups is not None and integrator.kind == INTEGRATOR_PHOTON:
-            raise McrtError("the photon mapper has no light groups: photons carry no light index")
+        if light_groups is not None and integrator.kind == INTEGRATOR_PHOTON and not integrator.has_photon_lights:
+            raise McrtError("the photon mapper has no light groups with these maps: their photons carry no light index "
+                            "(only the maps of emit() / emit_pass() do)")
         if aovs and integrator.kind == INTEGRATOR_PHOTON:
             raise McrtError("the photon mapper has no light-path AOVs")
         if aovs and light_groups is not None:
@@ -1503,12 +1530,17 @@ class Progressive:
         return ident
 
     def _photon_identity(self):
-        """The photon maps' part of _identity: a digest of the uploaded maps."""
+        """The photon maps' part of _identity: a digest of the uploaded maps, with light groups of each photon's light."""
         import hashlib
-        caustic, glob, k, dv = self.integrator._maps
+        ig = self.integrator
+        caustic, glob, k, dv = ig._maps
         ph = hashlib.sha256(np.array([k, dv], np.int64).tobytes())
-        for m in (caustic, glob):
-            rows = np.ascontiguousarray(np.asarray(m["photons"], np.float32).reshape(-1, 8)).view(np.dtype((np.void, 32))).ravel()
+        for which, m in enumerate((caustic, glob)):
+            rows = np.ascontiguousarray(np.asarray(m["photons"], np.float32).reshape(-1, 8))
+            if self.light_groups is not None:
+                # which light emitted a photon decides its plane: each row is the photon and its light index
+                rows = np.concatenate([rows.view(np.uint32), ig.photon_lights(which)[:, None]], axis=1)
+            rows = np.ascontiguousarray(rows).view(np.dtype((np.void, rows.shape[1] * 4))).ravel()
             ph.update(np.int64(len(rows)).tobytes() + np.sort(rows).tobytes())   # a set: order inside a leaf may differ
         return {"photon_digest": np.array(ph.hexdigest())}
 
@@ -1600,6 +1632,9 @@ class ProgressivePhotonMapping(Progressive):
     golden photon-mapping scene, a quarter of it reached the fixed k-NN map's error within 64 passes and the full
     radius did not (DESIGN.md section 6).
 
+    light_groups: as Progressive's. Every pass emits its own map, and emitted maps record each photon's light, so the
+    passes split their estimates by group; the pass-0 map is emitted before the table is set.
+
     Each pass replaces the photon mapper's uploaded maps and leaves it in gather mode (gather_radius(0, 0) returns
     it to the k-NN estimate). The frame no longer equals a one-shot render; it equals the same sequence of passes.
     Every sample is weighted equally: with passes of equal size that is Knaus and Zwicker's plain average of the
@@ -1611,15 +1646,16 @@ class ProgressivePhotonMapping(Progressive):
                  radius=None, k_nearest_photons=50, tile=16, light_groups=None, aovs=False):
         if not isinstance(photon_mapper, PhotonMapper):
             raise McrtError("ProgressivePhotonMapping needs a PhotonMapper")
-        if light_groups is not None:
-            raise McrtError("the photon mapper has no light groups: photons carry no light index")
         if aovs:
             raise McrtError("the photon mapper has no light-path AOVs")
         ppm_radii(1.0, alpha, 1)   # validates alpha
         self.emissions, self.caustic_factor = int(emissions), float(caustic_factor)
         self.max_photons_per_octree_leaf, self.k_nearest_photons = int(max_photons_per_octree_leaf), int(k_nearest_photons)
         self.alpha = float(alpha)
-        super().__init__(photon_mapper, camera, tile=tile)
+        if light_groups is not None and not photon_mapper.has_photon_lights:
+            # Progressive sets the table on maps that carry light indices: the pass-0 map
+            photon_mapper.emit_pass(0, self.emissions, self.caustic_factor, self.max_photons_per_octree_leaf, self.k_nearest_photons)
+        super().__init__(photon_mapper, camera, tile=tile, light_groups=light_groups)
         if radius is None:
             radius = self._initial_radii()
         r = (float(radius), float(radius)) if np.ndim(radius) == 0 else tuple(float(x) for x in radius)
@@ -1668,13 +1704,13 @@ class ProgressivePhotonMapping(Progressive):
 
     @classmethod
     def load(cls, path, photon_mapper, camera, emissions, caustic_factor, max_photons_per_octree_leaf=200, alpha=2 / 3,
-             radius=None, k_nearest_photons=50, tile=None):
+             radius=None, k_nearest_photons=50, tile=None, light_groups=None):
         """Resumes a checkpoint written by save(). Raises McrtError, and resumes nothing, when the seed, precision,
-        camera, film, tile, scene, emissions, caustic factor, leaf size, alpha or initial radii differ from the
-        checkpoint's (radius None derives them from the pass-0 maps again)."""
+        camera, film, tile, scene, emissions, caustic factor, leaf size, alpha, initial radii or light groups differ from
+        the checkpoint's (radius None derives them from the pass-0 maps again)."""
         data = _read_checkpoint(path)
         p = cls(photon_mapper, camera, emissions, caustic_factor, max_photons_per_octree_leaf, alpha, radius, k_nearest_photons,
-                int(data["tile"]) if tile is None else int(tile))
+                int(data["tile"]) if tile is None else int(tile), light_groups)
         p._restore(path, data)
         return p
 

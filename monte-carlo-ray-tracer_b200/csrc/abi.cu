@@ -121,6 +121,9 @@ struct mcrt_ctx
         std::vector<float> photons;
     } built_map[2];
     bool built_valid = false;
+    // the uploaded maps carry the emitting light of each photon (maps of mcrt_photon_emit / _emit_pass), even when a map
+    // holds no photon; maps of mcrt_photon_upload and mcrt_photon_build_dev do not
+    bool photon_lights = false;
     // maps built on the device by mcrt_photon_emit / mcrt_octree_build; host copies are made on demand
     PhotonOctreeDevice built_dev[2];
     bool built_host_current[2] = { false, false };
@@ -129,6 +132,7 @@ struct mcrt_ctx
     const unsigned long long* d_emit_offsets = nullptr;
     const void* d_emit_flux = nullptr;
     float4* d_emit_photons[2] = { nullptr, nullptr };
+    uint32_t* d_emit_lights[2] = { nullptr, nullptr };   // the emitting light of each photon of d_emit_photons
     unsigned long long emit_capacity[2] = { 0, 0 };
     std::vector<void*> emit_allocs;          // emission buffers (kept until the next emission / mcrt_destroy)
     unsigned long long emit_stored[2] = { 0, 0 };
@@ -800,6 +804,7 @@ namespace
             p.emit.emit_offsets = ctx->d_emit_offsets;
             p.emit.photon_flux = static_cast<const V4<R>*>(ctx->d_emit_flux);
             p.emit.photons[0] = ctx->d_emit_photons[0]; p.emit.photons[1] = ctx->d_emit_photons[1];
+            p.emit.lights[0] = ctx->d_emit_lights[0]; p.emit.lights[1] = ctx->d_emit_lights[1];
             p.emit.capacity[0] = ctx->emit_capacity[0]; p.emit.capacity[1] = ctx->emit_capacity[1];
             p.emit.non_caustic_reject = (R)ctx->emit_non_caustic_reject;
             p.emit.pass = ctx->emit_pass;
@@ -812,6 +817,7 @@ namespace
             p.pm.direct_visualization = ctx->direct_visualization;
             p.pm.query_capacity = knn_capacity;
             p.pm.gather_r2[0] = ctx->gather_r2[0]; p.pm.gather_r2[1] = ctx->gather_r2[1];
+            if (ctx->photon_lights) { p.pm.lights[0] = ctx->built_dev[0].lights; p.pm.lights[1] = ctx->built_dev[1].lights; }
         }
 
         Counters init;
@@ -1193,6 +1199,7 @@ int mcrt_scene_upload(mcrt_ctx* ctx, const mcrt_scene_desc* scene, uint64_t* h2d
     ctx->has_scene = false;
     ctx->has_light_groups = false;
     ctx->n_light_groups = 0;
+    ctx->photon_lights = false;   // the maps' light indices name the lights of the previous scene
 
     // scene scale for the fast mode's ray offsets
     double scale = 0.0;
@@ -1282,6 +1289,7 @@ int mcrt_photon_upload(mcrt_ctx* ctx, const mcrt_photon_map_desc* caustic_map, c
     for (int w = 0; w < 2; w++) { ctx->built_dev[w] = PhotonOctreeDevice(); ctx->built_host_current[w] = false; ctx->photon_map[w] = DevicePhotonMap(); }
     freeAll(ctx->photon_allocs);
     ctx->has_photons = false;
+    ctx->photon_lights = false;
     uint64_t bytes = 0;
     const mcrt_photon_map_desc* maps[2] = { caustic_map, global_map };
     for (int w = 0; w < 2; w++)
@@ -1372,6 +1380,7 @@ static void freeEmission(mcrt_ctx* ctx)
 {
     freeAll(ctx->emit_allocs);
     ctx->d_emit_offsets = nullptr; ctx->d_emit_flux = nullptr; ctx->d_emit_photons[0] = ctx->d_emit_photons[1] = nullptr;
+    ctx->d_emit_lights[0] = ctx->d_emit_lights[1] = nullptr;
     ctx->emit_stored[0] = ctx->emit_stored[1] = 0;
 }
 
@@ -1416,6 +1425,7 @@ static int emitRange(mcrt_ctx* ctx, const mcrt_photon_emit_params* params, int p
     {
         ctx->emit_capacity[w] = 4ull * work_count + 1024;
         if ((rc = devAlloc(ctx, ctx->emit_allocs, &ctx->d_emit_photons[w], (size_t)ctx->emit_capacity[w] * 2))) { freeEmission(ctx); return rc; }
+        if ((rc = devAlloc(ctx, ctx->emit_allocs, &ctx->d_emit_lights[w], (size_t)ctx->emit_capacity[w]))) { freeEmission(ctx); return rc; }
     }
     ctx->d_emit_offsets = d_off; ctx->d_emit_flux = d_flux;
     ctx->emit_non_caustic_reject = 1.0 / params->caustic_factor;
@@ -1450,10 +1460,11 @@ int mcrt_photon_emit_range(mcrt_ctx* ctx, const mcrt_photon_emit_params* params,
     return emitRange(ctx, params, precision, 0, work_first, work_count, caustic_dev, n_caustic, global_dev, n_global, stats);
 }
 
-int mcrt_photon_build_dev(mcrt_ctx* ctx, const mcrt_photon_emit_params* params, const float* caustic_dev, uint64_t n_caustic,
-                          const float* global_dev, uint64_t n_global, double* build_ms)
+// mcrt_photon_build_dev; lights_dev: null (the maps carry no light index), or the emitting light of each photon of the
+// two arrays (mcrt_photon_emit_pass), reordered with the photons
+static int buildPhotonMaps(mcrt_ctx* ctx, const mcrt_photon_emit_params* params, const float* caustic_dev, uint64_t n_caustic,
+                           const float* global_dev, uint64_t n_global, const uint32_t* const lights_dev[2], double* build_ms)
 {
-    if (!ctx) return MCRT_ERR_INVALID;
     if (!params || params->max_photons_per_octree_leaf == 0 || params->k_nearest_photons == 0 || params->k_nearest_photons > 1024 ||
         (n_caustic && !caustic_dev) || (n_global && !global_dev))
     { ctx->error = "mcrt_photon_build_dev: invalid arguments"; return MCRT_ERR_INVALID; }
@@ -1465,13 +1476,15 @@ int mcrt_photon_build_dev(mcrt_ctx* ctx, const mcrt_photon_emit_params* params, 
     for (int w = 0; w < 2; w++) { ctx->built_dev[w] = PhotonOctreeDevice(); ctx->built_host_current[w] = false; ctx->photon_map[w] = DevicePhotonMap(); }
     freeAll(ctx->photon_allocs);
     ctx->has_photons = false;
+    ctx->photon_lights = false;
     ctx->photon_build_ms = 0.0;
     const float4* src[2] = { reinterpret_cast<const float4*>(caustic_dev), reinterpret_cast<const float4*>(global_dev) };
     const uint64_t n[2] = { n_caustic, n_global };
     for (int w = 0; w < 2; w++)
     {
         const int rc = buildPhotonOctreeOnDevice(src[w], (uint32_t)n[w], params->scene_bounds, params->max_photons_per_octree_leaf,
-                                                 ctx->sm_count, ctx->stream, ctx->photon_allocs, ctx->built_dev[w], ctx->error);
+                                                 ctx->sm_count, ctx->stream, ctx->photon_allocs, ctx->built_dev[w], ctx->error,
+                                                 lights_dev ? lights_dev[w] : nullptr);
         if (rc) return rc;
         ctx->photon_map[w].octants = ctx->built_dev[w].octants;
         ctx->photon_map[w].photons = ctx->built_dev[w].photons;
@@ -1483,9 +1496,17 @@ int mcrt_photon_build_dev(mcrt_ctx* ctx, const mcrt_photon_emit_params* params, 
     ctx->direct_visualization = params->direct_visualization;
     ctx->has_photons = true;
     ctx->built_valid = true;
+    ctx->photon_lights = lights_dev != nullptr;
     if (build_ms) *build_ms = ctx->photon_build_ms;
     freeEmission(ctx);   // the raw emission buffers have been consumed (or superseded by the gathered arrays of a sharded pass)
     return MCRT_OK;
+}
+
+int mcrt_photon_build_dev(mcrt_ctx* ctx, const mcrt_photon_emit_params* params, const float* caustic_dev, uint64_t n_caustic,
+                          const float* global_dev, uint64_t n_global, double* build_ms)
+{
+    if (!ctx) return MCRT_ERR_INVALID;
+    return buildPhotonMaps(ctx, params, caustic_dev, n_caustic, global_dev, n_global, nullptr, build_ms);
 }
 
 int mcrt_photon_emit(mcrt_ctx* ctx, const mcrt_photon_emit_params* params, int precision, uint64_t* n_caustic,
@@ -1507,7 +1528,8 @@ int mcrt_photon_emit_pass(mcrt_ctx* ctx, const mcrt_photon_emit_params* params, 
     if (n_caustic) *n_caustic = n[0];
     if (n_global) *n_global = n[1];
     double build_ms = 0.0;
-    rc = mcrt_photon_build_dev(ctx, params, raw[0], n[0], raw[1], n[1], &build_ms);
+    const uint32_t* const lights[2] = { ctx->d_emit_lights[0], ctx->d_emit_lights[1] };
+    rc = buildPhotonMaps(ctx, params, raw[0], n[0], raw[1], n[1], lights, &build_ms);
     freeEmission(ctx);
     if (rc) return rc;
     if (stats) stats->gpu_ms_knn = build_ms;   // emission pass: this field reports the octree build
@@ -1596,6 +1618,27 @@ int mcrt_photon_download(mcrt_ctx* ctx, int which, mcrt_photon_map_desc* out)
         ctx->built_host_current[which] = true;
     }
     describeHostMap(ctx->built_map[which], out);
+    return MCRT_OK;
+}
+
+int mcrt_photon_download_lights(mcrt_ctx* ctx, int which, uint32_t* out, uint64_t n)
+{
+    if (!ctx) return MCRT_ERR_INVALID;
+    if (which != 0 && which != 1) { ctx->error = "mcrt_photon_download_lights: invalid arguments"; return MCRT_ERR_INVALID; }
+    if (!ctx->built_valid) { ctx->error = "no maps built by mcrt_photon_emit"; return MCRT_ERR_NO_PHOTONS; }
+    if (!ctx->photon_lights)
+    {
+        ctx->error = "mcrt_photon_download_lights: the maps carry no light index (only maps emitted by mcrt_photon_emit / _emit_pass do)";
+        return MCRT_ERR_UNSUPPORTED;
+    }
+    const PhotonOctreeDevice& d = ctx->built_dev[which];
+    if (n != d.n_photons || (n && !out))
+    {
+        ctx->error = "mcrt_photon_download_lights: n " + std::to_string(n) + ", the map has " + std::to_string(d.n_photons) + " photons";
+        return MCRT_ERR_INVALID;
+    }
+    CK(cudaSetDevice(ctx->device));
+    if (n) CK(cudaMemcpy(out, d.lights, (size_t)n * sizeof(uint32_t), cudaMemcpyDeviceToHost));
     return MCRT_OK;
 }
 
@@ -1870,9 +1913,9 @@ int mcrt_render_accumulate_groups_dev(mcrt_ctx* ctx, const mcrt_camera* camera, 
     if (!ctx) return MCRT_ERR_INVALID;
     const std::string name = "mcrt_render_accumulate_groups_dev";
     if (!ctx->film_default) { ctx->error = name + ": light-group planes take the box film only"; return MCRT_ERR_UNSUPPORTED; }
-    if (integrator_kind == MCRT_INTEGRATOR_PHOTON)
+    if (integrator_kind == MCRT_INTEGRATOR_PHOTON && !(ctx->has_photons && ctx->photon_lights))
     {
-        ctx->error = name + ": photons carry no light index, the photon mapper has no light groups";
+        ctx->error = name + ": the photon maps carry no light index (only maps emitted by mcrt_photon_emit / _emit_pass do)";
         return MCRT_ERR_UNSUPPORTED;
     }
     if (!ctx->has_light_groups) { ctx->error = name + ": no light-group table (mcrt_set_light_groups)"; return MCRT_ERR_INVALID; }

@@ -657,6 +657,11 @@ namespace
         }
     }
 
+    __global__ void k_gather_lights(const uint32_t* idx, const uint32_t* in, uint32_t* out, uint32_t n)
+    {
+        for (uint32_t p = blockIdx.x * blockDim.x + threadIdx.x; p < n; p += gridDim.x * blockDim.x) out[p] = in[idx[p]];
+    }
+
     // a leaf octant's box is the box of its own photons; for a single-leaf tree nobody has binned them
     __global__ void k_root_leaf_box(BNode* nodes, const float4* points, uint32_t n)
     {
@@ -871,7 +876,8 @@ int buildBvhOnDevice(const double* prim_bounds_host, uint32_t n, const double sc
 // guard against coincident photons; the reference would recurse forever), boxes = tight boxes of the
 // contained photons.
 int buildPhotonOctreeOnDevice(const float4* d_photons, uint32_t n, const double cell[6], uint32_t max_node_data, int sm_count,
-                              cudaStream_t s, std::vector<void*>& keep, PhotonOctreeDevice& out, std::string& error)
+                              cudaStream_t s, std::vector<void*>& keep, PhotonOctreeDevice& out, std::string& error,
+                              const uint32_t* d_lights)
 {
     out = PhotonOctreeDevice();
     if (n == 0) return MCRT_OK;
@@ -904,14 +910,22 @@ int buildPhotonOctreeOnDevice(const float4* d_photons, uint32_t n, const double 
         error = "photon octree: out of device memory"; return MCRT_ERR_CUDA;
     }
     keep.push_back(d_oct); keep.push_back(d_next); keep.push_back(d_sorted);
+    uint32_t* d_sorted_lights = nullptr;
+    if (d_lights)
+    {
+        if (cudaMalloc((void**)&d_sorted_lights, (size_t)n * sizeof(uint32_t)) != cudaSuccess)
+        { error = "photon octree: out of device memory"; return MCRT_ERR_CUDA; }
+        keep.push_back(d_sorted_lights);
+    }
     k_emit_octants<<<(core.n_nodes + 127) / 128, 128, 0, s>>>(core.d_nodes, core.n_nodes, d_oct, d_next);
     k_gather_points<<<sm_count * 8, 256, 0, s>>>(core.d_idx, d_photons, d_sorted, n);
+    if (d_lights) k_gather_lights<<<sm_count * 8, 256, 0, s>>>(core.d_idx, d_lights, d_sorted_lights, n);
     BK(cudaEventRecord(ev1, s));
     BK(cudaStreamSynchronize(s));
     BK(cudaGetLastError());
     float ms = 0.f;
     BK(cudaEventElapsedTime(&ms, ev0, ev1));
-    out.octants = d_oct; out.next_sibling = d_next; out.photons = d_sorted;
+    out.octants = d_oct; out.next_sibling = d_next; out.photons = d_sorted; out.lights = d_sorted_lights;
     out.n_octants = core.n_nodes; out.n_photons = n; out.gpu_ms = ms; out.rounds = core.rounds;
     return MCRT_OK;
 }

@@ -221,6 +221,7 @@ namespace mcrt
         const unsigned long long* emit_offsets;  // [n_lights + 1] prefix sums of num_light_emissions
         const V4<R>* photon_flux;                // [n_lights] light_flux / num_light_emissions
         float4* photons[2];                      // output: 2 float4 per photon {flux.xyz,pos.x | pos.yz,phi,theta}
+        uint32_t* lights[2];                     // output: the index of the light that emitted each photon
         unsigned long long capacity[2];
         R non_caustic_reject;                    // 1 / caustic_factor
         uint32_t pass;                           // emissions of light l take the indices pass * n_l + j (mcrt_photon_emit_pass)
@@ -1150,9 +1151,73 @@ namespace mcrt
         ia.inside = qr.meta.z & 1u;
     }
 
+    // One photon's term of the radiance estimate (photon-mapper.cpp:343-391): flux f / pdf, in the caustic map (which 0)
+    // weighted by the cone filter 1 - d/r (:383-386). false: the BSDF has no value in the photon's direction.
+    template <class R>
+    MCRT_D bool photonTerm(Interaction<R>& ia, uint32_t which, const float4& a, const float4& b, R d2, R inv_r2, V3<R>& term)
+    {
+        V3<R> bsdf_absIdotN; R bsdf_pdf;
+        if (!ia.bsdfWorld(bsdf_absIdotN, photonDir<R>(b.z, b.w), bsdf_pdf)) return false;
+        const V3<R> flux((R)a.x, (R)a.y, (R)a.z);
+        if (which == 0)
+        {
+            const R wp = gmax(R(0), R(1) - msqrt(d2 * inv_r2));
+            term = (flux * bsdf_absIdotN * wp) / bsdf_pdf;
+        }
+        else
+        {
+            term = flux * bsdf_absIdotN / bsdf_pdf;
+        }
+        return true;
+    }
+
+    // Light-group split of a photon estimate (FILM_MODE_GROUPS of k_knn / k_gather). Each lane keeps one run: the sum of
+    // its photons' terms since its photons' light group last changed (plane: that group; NO_PRIM: no run). Every term of
+    // a query shares the estimate's scale and the path weight, so the planes' deposits add up to the one-plane deposit up
+    // to rounding, and no term is negative. depositGroupRuns adds up the runs of each plane present over the warp, and
+    // the plane's lowest lane deposits scale(sum) * weight; with one group that is one deposit, as the one-plane kernel.
+    template <class R, class Scale>
+    MCRT_D void depositGroupRuns(const WaveParams<R>& p, uint32_t film_index, uint32_t plane, const V3<R>& sum, const V3<R>& weight,
+                                 Scale&& scale)
+    {
+        const unsigned lane = threadIdx.x & 31u;
+        unsigned pending = __ballot_sync(0xFFFFFFFFu, plane != NO_PRIM);
+        while (pending)
+        {
+            const int leader = __ffs(pending) - 1;
+            const uint32_t g = __shfl_sync(0xFFFFFFFFu, plane, leader);
+            const bool mine = plane == g;
+            V3<R> v = mine ? sum : V3<R>(R(0));
+            for (int off = 16; off > 0; off >>= 1)
+            {
+                v.x += __shfl_xor_sync(0xFFFFFFFFu, v.x, off);
+                v.y += __shfl_xor_sync(0xFFFFFFFFu, v.y, off);
+                v.z += __shfl_xor_sync(0xFFFFFFFFu, v.z, off);
+            }
+            if ((int)lane == leader) filmAddV(p.film + g * p.plane_values, film_index, scale(v) * weight);
+            pending &= ~__ballot_sync(0xFFFFFFFFu, mine);
+        }
+    }
+
+    // One step of the split, on the whole warp: each lane adds its photon's term of group g (NO_PRIM: no photon) to its
+    // run; the lanes whose photon belongs to another group than their run hand the run to the warp first.
+    template <class R, class Scale>
+    MCRT_D void groupRunStep(const WaveParams<R>& p, uint32_t film_index, const V3<R>& weight, Scale&& scale, uint32_t g,
+                             const V3<R>& term, uint32_t& run, V3<R>& run_sum)
+    {
+        const bool flush = g != NO_PRIM && run != NO_PRIM && g != run;
+        if (__any_sync(0xFFFFFFFFu, flush))
+        {
+            depositGroupRuns(p, film_index, flush ? run : NO_PRIM, run_sum, weight, scale);
+            if (flush) { run = NO_PRIM; run_sum = V3<R>(R(0)); }
+        }
+        if (g != NO_PRIM) { run = g; run_sum += term; }
+    }
+
     // ------------------------------------------------------------------------------------------
     // k_knn: one warp per photon-map query emitted by k_shade<R,1>; search + radiance estimate.
-    template <class R, int SLOTS, bool FILM, uint32_t FEATS>
+    // FILM_MODE_GROUPS splits the estimate by the light group of each photon (depositGroupRuns).
+    template <class R, int SLOTS, int FILM, uint32_t FEATS>
     __global__ void __launch_bounds__(32 * KNN_WARPS_PER_BLOCK, MCRT_KNN_MINBLOCKS) k_knn(WaveParams<R> p)
     {
         extern __shared__ __align__(16) unsigned char knn_smem[];
@@ -1177,6 +1242,32 @@ namespace mcrt
 
             const R top_d2 = (R)res_max;
             const R inv_max_r2 = R(1) / top_d2;
+            if constexpr (FILM == FILM_MODE_GROUPS)
+            {
+                const auto scale = [&](const V3<R>& v) { return which == 0 ? R(3) * v * inv_max_r2 * Consts<R>::INV_PI : v / (top_d2 * Consts<R>::PI); };
+                const V3<R> weight = qr.weight_t.xyz();
+                uint32_t run = NO_PRIM;
+                V3<R> run_sum(R(0));
+                // uniform steps of 32 results, so that every lane takes part in the hand-over of runs
+                for (uint32_t base = 0; base < found; base += 32)
+                {
+                    const uint32_t s = base + lane;
+                    uint32_t g = NO_PRIM;
+                    V3<R> term(R(0));
+                    if (s < found)
+                    {
+                        const uint32_t idx = sh.res_idx[s];
+                        g = p.group_of_light[__ldg(&p.pm.lights[which][idx])];
+                        const float4 a = __ldg(&map.photons[2 * (size_t)idx]);
+                        const float4 b = __ldg(&map.photons[2 * (size_t)idx + 1]);
+                        if (!photonTerm(ia, which, a, b, (R)sh.res_d2[s], inv_max_r2, term)) term = V3<R>(R(0));
+                    }
+                    groupRunStep(p, qr.meta.y, weight, scale, g, term, run, run_sum);
+                }
+                depositGroupRuns(p, qr.meta.y, run, run_sum, weight, scale);
+                __syncwarp();
+                continue;
+            }
             V3<R> sum(R(0));
             for (uint32_t s = lane; s < found; s += 32)
             {
@@ -1251,7 +1342,8 @@ namespace mcrt
     // the k nearest photons: every photon within r (gatherWarp) enters the estimate with k_knn's formulas, r^2 in
     // place of the k-th distance2 - caustic 3/(pi r^2) sum flux f/pdf (1 - d/r), global 1/(pi r^2) sum flux f/pdf.
     // The BSDF is evaluated on the lane that finds the photon, while the batch streams.
-    template <class R, bool FILM, uint32_t FEATS>
+    // FILM_MODE_GROUPS splits the estimate by light group as k_knn does, one step per 32 photons streamed.
+    template <class R, int FILM, uint32_t FEATS>
     __global__ void __launch_bounds__(32 * KNN_WARPS_PER_BLOCK, MCRT_GATHER_MINBLOCKS) k_gather(WaveParams<R> p)
     {
         __shared__ uint32_t gather_stack[KNN_WARPS_PER_BLOCK][GATHER_STACK];
@@ -1268,6 +1360,28 @@ namespace mcrt
             Interaction<R> ia;
             queryInteraction<FEATS>(p, qr, ia);
             const R inv_r2 = R(1) / (R)r2;
+            if constexpr (FILM == FILM_MODE_GROUPS)
+            {
+                const auto scale = [&](const V3<R>& v) { return which == 0 ? R(3) * v * inv_r2 * Consts<R>::INV_PI : v / ((R)r2 * Consts<R>::PI); };
+                const V3<R> weight = qr.weight_t.xyz();
+                const uint32_t* const lights = p.pm.lights[which];
+                uint32_t g = NO_PRIM, run = NO_PRIM;   // g: the group of this lane's photon of the current step
+                V3<R> term(R(0)), run_sum(R(0));
+                gatherWarp(p.pm.map[which], (double)qr.pos_n1.x, (double)qr.pos_n1.y, (double)qr.pos_n1.z, r2, stack, &overflow,
+                           [&](unsigned long long idx, double d2, const float4& a, const float4& b)
+                           {
+                               g = p.group_of_light[__ldg(&lights[idx])];
+                               if (!photonTerm(ia, which, a, b, (R)d2, inv_r2, term)) term = V3<R>(R(0));
+                           },
+                           [&]
+                           {
+                               groupRunStep(p, qr.meta.y, weight, scale, g, term, run, run_sum);
+                               g = NO_PRIM;
+                           });
+                depositGroupRuns(p, qr.meta.y, run, run_sum, weight, scale);   // no photon: no run, no deposit
+                __syncwarp();
+                continue;
+            }
             V3<R> sum(R(0));
             bool found = false;
             gatherWarp(p.pm.map[which], (double)qr.pos_n1.x, (double)qr.pos_n1.y, (double)qr.pos_n1.z, r2, stack, &overflow,
@@ -1501,9 +1615,12 @@ namespace mcrt
                     {
                         const unsigned long long idx = base + __popc(mask & ((1u << lane) - 1u));
                         if (idx < p.emit.capacity[which])
+                        {
                             storePhoton(p.emit.photons[which], idx, V3<double>((double)ph_flux.x, (double)ph_flux.y, (double)ph_flux.z),
                                         V3<double>((double)ph_pos.x, (double)ph_pos.y, (double)ph_pos.z),
                                         V3<double>((double)ph_dir.x, (double)ph_dir.y, (double)ph_dir.z));
+                            p.emit.lights[which][idx] = meta.x;   // the light k_emit_generate emitted the path from
+                        }
                         else c->photon_overflow = 1u;
                     }
                 }

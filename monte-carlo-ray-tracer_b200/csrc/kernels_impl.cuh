@@ -60,6 +60,11 @@ namespace mcrt
     {
         const bool lite = (p.scene.material_flags_any & ~SHADE_FEATS_LITE) == 0;
         if (!p.filmp.is_default_box) k_shade<MCRT_REAL, 1, FILM_MODE_SPLAT, SHADE_FEATS_ALL><<<grid * 2, 128, 0, s>>>(p, cur);
+        else if (p.n_planes)
+        {
+            if (lite) k_shade<MCRT_REAL, 1, FILM_MODE_GROUPS, SHADE_FEATS_LITE><<<grid * 2, 128, 0, s>>>(p, cur);
+            else k_shade<MCRT_REAL, 1, FILM_MODE_GROUPS, SHADE_FEATS_ALL><<<grid * 2, 128, 0, s>>>(p, cur);
+        }
         else if (lite) k_shade<MCRT_REAL, 1, FILM_MODE_BOX, SHADE_FEATS_LITE><<<grid * 2, 128, 0, s>>>(p, cur);
         else k_shade<MCRT_REAL, 1, FILM_MODE_BOX, SHADE_FEATS_ALL><<<grid * 2, 128, 0, s>>>(p, cur);
     }
@@ -70,9 +75,14 @@ namespace mcrt
         {
             // fixed-radius gather (mcrt_photon_gather_radius) in place of the k-NN estimate
             const bool lite = (p.scene.material_flags_any & ~SHADE_FEATS_LITE) == 0;
-            if (!p.filmp.is_default_box) k_gather<MCRT_REAL, true, SHADE_FEATS_ALL><<<g, b, 0, s>>>(p);
-            else if (lite) k_gather<MCRT_REAL, false, SHADE_FEATS_LITE><<<g, b, 0, s>>>(p);
-            else k_gather<MCRT_REAL, false, SHADE_FEATS_ALL><<<g, b, 0, s>>>(p);
+            if (!p.filmp.is_default_box) k_gather<MCRT_REAL, FILM_MODE_SPLAT, SHADE_FEATS_ALL><<<g, b, 0, s>>>(p);
+            else if (p.n_planes)
+            {
+                if (lite) k_gather<MCRT_REAL, FILM_MODE_GROUPS, SHADE_FEATS_LITE><<<g, b, 0, s>>>(p);
+                else k_gather<MCRT_REAL, FILM_MODE_GROUPS, SHADE_FEATS_ALL><<<g, b, 0, s>>>(p);
+            }
+            else if (lite) k_gather<MCRT_REAL, FILM_MODE_BOX, SHADE_FEATS_LITE><<<g, b, 0, s>>>(p);
+            else k_gather<MCRT_REAL, FILM_MODE_BOX, SHADE_FEATS_ALL><<<g, b, 0, s>>>(p);
             return;
         }
         const size_t smem = knnSharedBytes(p.pm.k_nearest);
@@ -82,17 +92,20 @@ namespace mcrt
         {
             // filtered film: the rare configuration, one generic instantiation
             static bool attr_set = false;
-            if (!attr_set) { cudaFuncSetAttribute(k_knn<MCRT_REAL, 0, true, SHADE_FEATS_ALL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)knnSharedBytes(1024)); attr_set = true; }
-            k_knn<MCRT_REAL, 0, true, SHADE_FEATS_ALL><<<g, b, smem, s>>>(p);
+            if (!attr_set) { cudaFuncSetAttribute(k_knn<MCRT_REAL, 0, FILM_MODE_SPLAT, SHADE_FEATS_ALL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)knnSharedBytes(1024)); attr_set = true; }
+            k_knn<MCRT_REAL, 0, FILM_MODE_SPLAT, SHADE_FEATS_ALL><<<g, b, smem, s>>>(p);
             return;
         }
         const bool lite = (p.scene.material_flags_any & ~SHADE_FEATS_LITE) == 0;
+        const bool groups = p.n_planes != 0;   // light-group planes
         const int slots = knnSlotsFor(p.pm.k_nearest);
         // k > 672 needs more than the default 48 KB of dynamic shared memory (knnSharedBytes)
-        #define MCRT_KNN_LAUNCH1(SL, FE) \
+        #define MCRT_KNN_LAUNCH2(SL, FM, FE) \
             do { static bool attr_set = false; \
-                 if (!attr_set) { cudaFuncSetAttribute(k_knn<MCRT_REAL, SL, false, FE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)knnSharedBytes(1024)); attr_set = true; } \
-                 k_knn<MCRT_REAL, SL, false, FE><<<g, b, smem, s>>>(p); } while (0)
+                 if (!attr_set) { cudaFuncSetAttribute(k_knn<MCRT_REAL, SL, FM, FE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)knnSharedBytes(1024)); attr_set = true; } \
+                 k_knn<MCRT_REAL, SL, FM, FE><<<g, b, smem, s>>>(p); } while (0)
+        #define MCRT_KNN_LAUNCH1(SL, FE) \
+            do { if (groups) MCRT_KNN_LAUNCH2(SL, FILM_MODE_GROUPS, FE); else MCRT_KNN_LAUNCH2(SL, FILM_MODE_BOX, FE); } while (0)
         #define MCRT_KNN_LAUNCH(SL) \
             do { if (lite) MCRT_KNN_LAUNCH1(SL, SHADE_FEATS_LITE); else MCRT_KNN_LAUNCH1(SL, SHADE_FEATS_ALL); } while (0)
         switch (slots)
@@ -105,6 +118,7 @@ namespace mcrt
         }
         #undef MCRT_KNN_LAUNCH
         #undef MCRT_KNN_LAUNCH1
+        #undef MCRT_KNN_LAUNCH2
     }
     // k_shadow of the box film (one plane, light-group planes or AOV planes) with the scene-specialised traversal
     template <int FILM> static void launchShadowBox(const WaveParams<MCRT_REAL>& p, int grid, cudaStream_t s)

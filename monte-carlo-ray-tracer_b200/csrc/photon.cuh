@@ -56,6 +56,9 @@ namespace mcrt
         KnnQuery<R>* queries;
         uint32_t k_nearest, direct_visualization, query_capacity, _pad;
         double gather_r2[2];     // fixed gather radius^2 per map (k_gather); 0: the k-NN estimate (k_knn)
+        // per map, the index of the light that emitted each photon, in map order (maps emitted on the device; read by the
+        // light-group estimates only). Kept out of DevicePhotonMap so that the search kernels' parameters keep their layout.
+        const uint32_t* lights[2];
     };
 
     MCRT_D double octantDistance2(const DeviceOctant& o, double px, double py, double pz)
@@ -413,15 +416,16 @@ namespace mcrt
     // through a ballot onto the warp's stack in shared memory. A leaf - or an inner octant whose whole box
     // lies within r (octantMaxDistance2 <= r2) - streams its contiguous photon range 32 photons = 1 KB per
     // step, coalesced; every photon is still tested, so rounding at the box's corners cannot admit one
-    // beyond r. visit(idx, d2, a, b) runs on each lane that holds an accepted photon (a, b: its two float4).
+    // beyond r. visit(idx, d2, a, b) runs on each lane that holds an accepted photon (a, b: its two float4);
+    // batch_end() runs on the whole warp, converged, after each step of 32 photons.
     // There is no result set, so the number of photons found is unbounded. A stack overflow drops octants
     // and sets *overflow (the callers fail the call, as for the k-NN frontier); a depth-first walk holds at
     // most 7 per level + 1, and the octree builder caps the depth at 64, so GATHER_STACK = 512 suffices.
     constexpr int GATHER_STACK = 512;
 
-    template <class Visit>
+    template <class Visit, class BatchEnd>
     MCRT_D void gatherWarp(const DevicePhotonMap& map, double px, double py, double pz, double r2, uint32_t* stack,
-                           uint32_t* overflow, Visit&& visit)
+                           uint32_t* overflow, Visit&& visit, BatchEnd&& batch_end)
     {
         const unsigned lane = threadIdx.x & 31u;
         if (map.n_octants == 0 || map.n_photons == 0) return;
@@ -444,6 +448,7 @@ namespace mcrt
                         const double d2 = dx * dx + dy * dy + dz * dz;
                         if (d2 <= r2) visit(idx, d2, a, b);
                     }
+                    batch_end();
                 }
             }
             else
@@ -469,6 +474,13 @@ namespace mcrt
             cur = stack[--n_stack];
             __syncwarp();   // the slot just read is the next push's
         }
+    }
+
+    template <class Visit>
+    MCRT_D void gatherWarp(const DevicePhotonMap& map, double px, double py, double pz, double r2, uint32_t* stack,
+                           uint32_t* overflow, Visit&& visit)
+    {
+        gatherWarp(map, px, py, pz, r2, stack, overflow, visit, [] {});
     }
 
     // Photon::dir(), photon.hpp:19-27: std::sin/std::cos of the *float* angles (float overloads),
