@@ -515,6 +515,34 @@ int mcrt_render_accumulate_aovs_dev(mcrt_ctx* ctx, const mcrt_camera* camera, ui
                                     uint32_t global_seed, int integrator_kind, int precision, double* planes_dev,
                                     uint32_t n_planes, mcrt_stats* stats);
 
+/* Photon-mapper components: the photon mapper's contributions split by the estimator that made them. Its sampleRay
+ * (photon-mapper.cpp:299-332) deposits at exactly one of four kinds of site, so every deposit lands in one plane:
+ *   plane 0 MCRT_PM_EMISSION   an emitter seen from the camera, directly or through an unbroken chain of delta bounces
+ *   plane 1 MCRT_PM_DIRECT     Monte Carlo direct light: next-event estimation and the BSDF-sampled emitter hit it is
+ *                              combined with by MIS (an emitter hit after the first non-delta vertex)
+ *   plane 2 MCRT_PM_CAUSTIC    every caustic-map density estimate
+ *   plane 3 MCRT_PM_GLOBAL     every global-map density estimate
+ * No estimate is split inside itself: each query deposits its whole estimate into one plane, so the planes add up to
+ * the one-plane sums up to the order of the float64 film additions. The photon mapper adds no sky, so there is no
+ * background plane. With direct_visualization the first non-delta vertex queries both maps and the path ends there: the
+ * direct plane stays zero and no shadow ray is traced. */
+enum {
+    MCRT_PM_EMISSION = 0, MCRT_PM_DIRECT = 1, MCRT_PM_CAUSTIC = 2, MCRT_PM_GLOBAL = 3, MCRT_PM_COMPONENT_COUNT = 4
+};
+/* mcrt_render_accumulate_dev (active_tiles NULL) or mcrt_render_accumulate_tiles_dev (active_tiles HOST, same mask
+ * layout) into the component planes planes_dev[MCRT_PM_COMPONENT_COUNT][n_rows*W][3] (photon mapper, box film; the box
+ * film's weight is the sample count). Any photon maps serve: those of mcrt_photon_upload, mcrt_photon_emit[_pass] and
+ * mcrt_photon_build_dev. mcrt_light_groups_combine_dev, mcrt_progressive_resolve[_tiles]_dev and mcrt_denoise_dev take
+ * the planes or their weighted sums. MCRT_ERR_UNSUPPORTED: the path tracer (it has light-path AOVs instead), a
+ * reconstruction filter. MCRT_ERR_INVALID: an integrator kind outside MCRT_INTEGRATOR_*, n_planes !=
+ * MCRT_PM_COMPONENT_COUNT, a null planes_dev, and every argument the one-plane entry points refuse. MCRT_ERR_NO_PHOTONS: no photon maps, as the one-plane photon render. Nothing is
+ * written when a call is refused. The light-group table plays no part here. */
+int mcrt_render_accumulate_photon_components_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_t y_first, uint32_t y_step,
+                                                 uint32_t n_rows, uint32_t tile, const uint8_t* active_tiles,
+                                                 uint32_t sample_first, uint32_t sample_count, uint32_t global_seed,
+                                                 int integrator_kind, int precision, double* planes_dev, uint32_t n_planes,
+                                                 mcrt_stats* stats);
+
 /* Denoising a progressive frame (mcrt_denoise_dev) needs per-pixel guides: the first hits of the camera rays of samples
  * [sample_first, sample_first + sample_count) of every pixel of the whole width x height frame add
  * {albedo.rgb, shading normal.xyz, t, 1} per hit into features_dev [height*width][8] (device, float64); a miss adds

@@ -41,13 +41,17 @@ ABI_SYMBOLS = [
     "mcrt_render_features_dev", "mcrt_denoise_dev", "mcrt_render_features_chain_dev",
     "mcrt_photon_emit_pass", "mcrt_photon_gather_radius", "mcrt_photon_gather_search",
     "mcrt_set_light_groups", "mcrt_render_accumulate_groups_dev", "mcrt_light_groups_combine_dev",
-    "mcrt_render_accumulate_aovs_dev", "mcrt_photon_download_lights",
+    "mcrt_render_accumulate_aovs_dev", "mcrt_photon_download_lights", "mcrt_render_accumulate_photon_components_dev",
 ]
 
 # The light-path AOV planes of mcrt_render_accumulate_aovs_dev, in plane order (MCRT_AOV_* of include/mcrt_abi.h):
 # the camera ray's own sky and emitter, then direct / indirect light by the lobe of the first scattering vertex
 AOV_NAMES = ("background", "emission", "diffuse_direct", "diffuse_indirect", "reflection_direct", "reflection_indirect",
              "transmission_direct", "transmission_indirect")
+
+# The photon mapper's component planes of mcrt_render_accumulate_photon_components_dev, in plane order (MCRT_PM_* of
+# include/mcrt_abi.h): emitters seen from the camera, Monte Carlo direct light, the caustic-map and global-map estimates
+PHOTON_COMPONENT_NAMES = ("emission", "direct", "caustic", "global")
 
 
 class McrtError(RuntimeError):
@@ -250,6 +254,7 @@ def lib():
                                                         C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int, C.c_int, C.c_void_p,
                                                         C.c_uint32, C.POINTER(Stats)]
         L.mcrt_render_accumulate_aovs_dev.argtypes = L.mcrt_render_accumulate_groups_dev.argtypes
+        L.mcrt_render_accumulate_photon_components_dev.argtypes = L.mcrt_render_accumulate_groups_dev.argtypes
         L.mcrt_light_groups_combine_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint64, C.c_void_p, C.c_void_p]
         L.mcrt_render_features_dev.argtypes = [C.c_void_p, C.POINTER(CameraRec), C.c_uint32, C.c_uint32, C.c_uint32, C.c_int,
                                                C.c_void_p, C.POINTER(Stats)]
@@ -827,7 +832,10 @@ class PhotonMapper(Integrator):
 
     Light groups (set_light_groups, render_accumulate_groups_dev, Progressive(light_groups=...)) need maps that record
     which light emitted each photon: the maps of emit() / emit_pass() do (has_photon_lights, photon_lights); the maps of
-    the scene pack, of photon_maps= and of emit_sharded do not."""
+    the scene pack, of photon_maps= and of emit_sharded do not.
+
+    Components (render_accumulate_components_dev, Progressive(components=True)) split a frame by the estimator behind
+    each contribution (PHOTON_COMPONENT_NAMES) and work with every kind of map."""
     kind = INTEGRATOR_PHOTON
 
     def __init__(self, scene, device=0, precision=PRECISION_F64, global_seed=0x12345678, photon_maps=None, emit=None):
@@ -867,6 +875,15 @@ class PhotonMapper(Integrator):
 
     def render_accumulate_aovs_dev(self, *args, **kwargs):
         raise McrtError("the photon mapper has no light-path AOVs")
+
+    def render_accumulate_components_dev(self, camera, planes_ptr, sample_first, sample_count, tile=0, active=None,
+                                         y_first=0, y_step=1, n_rows=None, precision=None):
+        """mcrt_render_accumulate_photon_components_dev: render_accumulate_dev (active None) or render_accumulate_tiles_dev
+        into the component planes planes_ptr [4, n_rows, width, 3] (device), in the order of PHOTON_COMPONENT_NAMES.
+        Works with every kind of map (scene pack, photon_maps=, emit, emit_pass, emit_sharded)."""
+        return self._render_accumulate_planes(lib().mcrt_render_accumulate_photon_components_dev, camera, planes_ptr,
+                                              len(PHOTON_COMPONENT_NAMES), sample_first, sample_count, tile, active, y_first,
+                                              y_step, n_rows, precision)
 
     def _emit_params(self, emissions, caustic_factor, max_photons_per_octree_leaf, k_nearest_photons, direct_visualization, scene_bounds):
         p = PhotonEmitParams()
@@ -1223,12 +1240,24 @@ class Progressive:
     Light-path AOVs (aovs=True; box film, path tracer, not together with light groups): A and B hold the 8 planes of
     AOV_NAMES, [8, rows, width, 3], filled by mcrt_render_accumulate_aovs_dev. frame, error, render, render_adaptive
     and denoise work on the planes' sum, as with light groups; aov_frames() resolves each plane with its own noise
-    estimate, and relight(weights) and denoise(weights=...) recomposite the frame from weighted planes."""
+    estimate, and relight(weights) and denoise(weights=...) recomposite the frame from weighted planes.
+
+    Photon-mapper components (components=True; box film, a PhotonMapper with any maps, not together with light groups
+    or AOVs): A and B hold the 4 planes of PHOTON_COMPONENT_NAMES, [4, rows, width, 3], filled by
+    mcrt_render_accumulate_photon_components_dev - emitters seen from the camera, direct light, the caustic-map and the
+    global-map estimates. Everything works on the planes' sum as with AOVs; component_frames() resolves each plane with
+    its own noise estimate, which shows which estimator still dominates the error, and relight(weights) /
+    denoise(weights=...) recomposite the frame, e.g. relight([1, 1, 0, 1]) removes the caustics."""
 
     _STATS = ("paths", "extension_rays", "shadow_rays")
 
-    def __init__(self, integrator, camera, y_first=0, y_step=1, n_rows=None, tile=16, light_groups=None, aovs=False):
+    def __init__(self, integrator, camera, y_first=0, y_step=1, n_rows=None, tile=16, light_groups=None, aovs=False,
+                 components=False):
         import torch
+        if components and integrator.kind != INTEGRATOR_PHOTON:
+            raise McrtError("photon-mapper components need a PhotonMapper (the path tracer has light-path AOVs)")
+        if components and (light_groups is not None or aovs):
+            raise McrtError("photon-mapper components together with light groups or AOVs in one render are not supported")
         if light_groups is not None and integrator.kind == INTEGRATOR_PHOTON and not integrator.has_photon_lights:
             raise McrtError("the photon mapper has no light groups with these maps: their photons carry no light index "
                             "(only the maps of emit() / emit_pass() do)")
@@ -1255,6 +1284,11 @@ class Progressive:
             if self.filtered:
                 raise McrtError("light-path AOVs take the box film only")
             self.n_planes = len(AOV_NAMES)
+        self.components = bool(components)
+        if self.components:
+            if self.filtered:
+                raise McrtError("photon-mapper components take the box film only")
+            self.n_planes = len(PHOTON_COMPONENT_NAMES)
         planes = (self.n_planes,) if self._planar else ()
         dev = torch.device("cuda", integrator.device)
         self.rgb = [torch.zeros(planes + (self.rows, camera.width, 3), dtype=torch.float64, device=dev) for _ in range(2)]
@@ -1277,8 +1311,8 @@ class Progressive:
 
     @property
     def _planar(self):
-        """A and B hold planes (light groups or AOVs) whose sum is the beauty frame's sums."""
-        return self.light_groups is not None or self.aovs
+        """A and B hold planes (light groups, AOVs or photon-mapper components) whose sum is the beauty frame's sums."""
+        return self.light_groups is not None or self.aovs or self.components
 
     def add(self, samples):
         """Renders samples [self.samples, self.samples + samples) of the active tiles into A (even pass) or B (odd pass)."""
@@ -1293,6 +1327,10 @@ class Progressive:
             st = self.integrator.render_accumulate_aovs_dev(self.camera, self.rgb[half].data_ptr(), self.samples, int(samples), self.tile,
                                                             None if self.active.all() else self.active, self.y_first, self.y_step,
                                                             self.n_rows)
+        elif self.components:
+            st = self.integrator.render_accumulate_components_dev(self.camera, self.rgb[half].data_ptr(), self.samples, int(samples),
+                                                                  self.tile, None if self.active.all() else self.active, self.y_first,
+                                                                  self.y_step, self.n_rows)
         elif self.active.all():
             st = self.integrator.render_accumulate_dev(self.camera, self.rgb[half].data_ptr(), wsum, self.samples,
                                                        int(samples), self.y_first, self.y_step, self.n_rows)
@@ -1315,12 +1353,12 @@ class Progressive:
         return self._resolved
 
     def _halves(self, weights=None):
-        """The sums of halves A and B, [rows, width, 3] each: with light groups or AOVs the combination of their planes
-        with weights [n_planes, 3] or [n_planes] (None: every weight 1, the beauty frame's sums)."""
+        """The sums of halves A and B, [rows, width, 3] each: with planes (light groups, AOVs, components) the combination
+        of the planes with weights [n_planes, 3] or [n_planes] (None: every weight 1, the beauty frame's sums)."""
         import torch
         if not self._planar:
             if weights is not None:
-                raise McrtError("weights need a render with light groups or AOVs")
+                raise McrtError("weights need a render with light groups, AOVs or photon-mapper components")
             return self.rgb
         w = np.ones(self.n_planes) if weights is None else weights
         out = []
@@ -1367,6 +1405,19 @@ class Progressive:
         plane's relative error float64 [8], estimated from the difference of its two halves like error()'s)."""
         if not self.aovs:
             raise McrtError("aov_frames needs a render with aovs=True")
+        return self._plane_frames()
+
+    # -- photon-mapper components
+    def component_frames(self):
+        """Each component plane resolved on its own (in the order of PHOTON_COMPONENT_NAMES) -> (frames float64
+        [4, rows, width, 3], each plane's relative error float64 [4], estimated from the difference of its two halves
+        like error()'s)."""
+        if not self.components:
+            raise McrtError("component_frames needs a render with components=True")
+        return self._plane_frames()
+
+    def _plane_frames(self):
+        """Every plane of A and B resolved on its own -> (frames [n_planes, rows, width, 3], relative errors [n_planes])."""
         res = [self._resolve_halves([self.rgb[0][k], self.rgb[1][k]]) for k in range(self.n_planes)]
         return np.stack([r[0] for r in res]), np.array([r[1] for r in res])
 
@@ -1374,7 +1425,8 @@ class Progressive:
         """The frame recomposited: the planes summed with weights [n_planes, 3] or [n_planes], resolved like frame()
         -> (frame, frame relative error, per-tile relative errors). Light groups: the last row weights the sky, and
         weight w_g on group g equals a render of the scene with group g's emittance scaled by w_g. AOVs: the rows weight
-        the planes of AOV_NAMES, e.g. 0 on the reflection planes removes what the first vertex reflected."""
+        the planes of AOV_NAMES, e.g. 0 on the reflection planes removes what the first vertex reflected. Components: the
+        rows weight the planes of PHOTON_COMPONENT_NAMES, e.g. [1, 1, 0, 1] removes the caustics."""
         frame, err, tiles, _ = self._resolve_halves(self._halves(weights))
         return frame, err, tiles
 
@@ -1485,7 +1537,7 @@ class Progressive:
         their own surface; rough and glossy lobes are never followed; the feature samples [0, F) also feed half A; the Owen-scrambled halves are not
         independent, so the residual estimate can read about 10 % low.
 
-        weights (light groups or AOVs only): denoise the frame relit or recomposited with these weights (relight) instead of
+        weights (light groups, AOVs or components only): denoise the frame relit or recomposited with these weights (relight) instead of
         the beauty frame."""
         import torch
         if (self.y_first, self.y_step, self.n_rows) != (0, 1, self.camera.height):
@@ -1527,6 +1579,8 @@ class Progressive:
             ident["light_groups"] = self.light_groups.copy()
         if self.aovs:
             ident["aovs"] = np.int64(len(AOV_NAMES))
+        if self.components:
+            ident["photon_components"] = np.int64(len(PHOTON_COMPONENT_NAMES))
         return ident
 
     def _photon_identity(self):
@@ -1556,14 +1610,15 @@ class Progressive:
             np.savez(f, **data)
 
     @classmethod
-    def load(cls, path, integrator, camera, tile=None, light_groups=None, aovs=False):
+    def load(cls, path, integrator, camera, tile=None, light_groups=None, aovs=False, components=False):
         """Resumes a checkpoint written by save() with `integrator` and `camera` (and `tile`, the checkpoint's if None).
         Raises McrtError, and resumes nothing, when the seed, precision, integrator kind, camera, film, tile, scene,
-        photon maps, light groups or AOVs differ from the checkpoint's. A checkpoint without tile state resumes with
-        every tile active."""
+        photon maps, light groups, AOVs or components differ from the checkpoint's. A checkpoint without tile state
+        resumes with every tile active."""
         data = _read_checkpoint(path)
         y_first, y_step, n_rows = (int(v) for v in data["row_set"])
-        p = cls(integrator, camera, y_first, y_step, n_rows, int(data["tile"]) if tile is None else int(tile), light_groups, aovs)
+        p = cls(integrator, camera, y_first, y_step, n_rows, int(data["tile"]) if tile is None else int(tile), light_groups, aovs,
+                components)
         p._restore(path, data)
         return p
 
@@ -1575,6 +1630,8 @@ class Progressive:
             raise McrtError(f"checkpoint {path}: light groups differ from this render's; not resuming")
         if ("aovs" in data) != ("aovs" in ident):
             raise McrtError(f"checkpoint {path}: light-path AOVs differ from this render's; not resuming")
+        if ("photon_components" in data) != ("photon_components" in ident):
+            raise McrtError(f"checkpoint {path}: photon-mapper components differ from this render's; not resuming")
         for k, want in ident.items():
             if k not in data or not np.array_equal(data[k], want):
                 raise McrtError(f"checkpoint {path}: {k} differs from this render's; not resuming")
@@ -1635,6 +1692,9 @@ class ProgressivePhotonMapping(Progressive):
     light_groups: as Progressive's. Every pass emits its own map, and emitted maps record each photon's light, so the
     passes split their estimates by group; the pass-0 map is emitted before the table is set.
 
+    components: as Progressive's. component_frames() then shows whether the caustic or the global estimate, whose radii
+    shrink on their own schedules, still dominates the error.
+
     Each pass replaces the photon mapper's uploaded maps and leaves it in gather mode (gather_radius(0, 0) returns
     it to the k-NN estimate). The frame no longer equals a one-shot render; it equals the same sequence of passes.
     Every sample is weighted equally: with passes of equal size that is Knaus and Zwicker's plain average of the
@@ -1643,7 +1703,7 @@ class ProgressivePhotonMapping(Progressive):
     the next add() emits again (the passes are deterministic)."""
 
     def __init__(self, photon_mapper, camera, emissions, caustic_factor, max_photons_per_octree_leaf=200, alpha=2 / 3,
-                 radius=None, k_nearest_photons=50, tile=16, light_groups=None, aovs=False):
+                 radius=None, k_nearest_photons=50, tile=16, light_groups=None, aovs=False, components=False):
         if not isinstance(photon_mapper, PhotonMapper):
             raise McrtError("ProgressivePhotonMapping needs a PhotonMapper")
         if aovs:
@@ -1655,7 +1715,7 @@ class ProgressivePhotonMapping(Progressive):
         if light_groups is not None and not photon_mapper.has_photon_lights:
             # Progressive sets the table on maps that carry light indices: the pass-0 map
             photon_mapper.emit_pass(0, self.emissions, self.caustic_factor, self.max_photons_per_octree_leaf, self.k_nearest_photons)
-        super().__init__(photon_mapper, camera, tile=tile, light_groups=light_groups)
+        super().__init__(photon_mapper, camera, tile=tile, light_groups=light_groups, components=components)
         if radius is None:
             radius = self._initial_radii()
         r = (float(radius), float(radius)) if np.ndim(radius) == 0 else tuple(float(x) for x in radius)
@@ -1704,13 +1764,13 @@ class ProgressivePhotonMapping(Progressive):
 
     @classmethod
     def load(cls, path, photon_mapper, camera, emissions, caustic_factor, max_photons_per_octree_leaf=200, alpha=2 / 3,
-             radius=None, k_nearest_photons=50, tile=None, light_groups=None):
+             radius=None, k_nearest_photons=50, tile=None, light_groups=None, components=False):
         """Resumes a checkpoint written by save(). Raises McrtError, and resumes nothing, when the seed, precision,
-        camera, film, tile, scene, emissions, caustic factor, leaf size, alpha, initial radii or light groups differ from
-        the checkpoint's (radius None derives them from the pass-0 maps again)."""
+        camera, film, tile, scene, emissions, caustic factor, leaf size, alpha, initial radii, light groups or components
+        differ from the checkpoint's (radius None derives them from the pass-0 maps again)."""
         data = _read_checkpoint(path)
         p = cls(photon_mapper, camera, emissions, caustic_factor, max_photons_per_octree_leaf, alpha, radius, k_nearest_photons,
-                int(data["tile"]) if tile is None else int(tile), light_groups)
+                int(data["tile"]) if tile is None else int(tile), light_groups, components=components)
         p._restore(path, data)
         return p
 

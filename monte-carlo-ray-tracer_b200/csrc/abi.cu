@@ -683,7 +683,9 @@ namespace
         double* rgb;    // box film [n_pixels][3] in film_index order; filtered film [height*width][3]
         double* wsum;   // filtered film [height*width]; null with the box film
         uint32_t n_planes = 0;   // box film only: rgb holds this many light-group planes (mcrt_render_accumulate_groups_dev)
-        bool aovs = false;       // ... or the MCRT_AOV_COUNT light-path planes (mcrt_render_accumulate_aovs_dev)
+        bool aovs = false;       // ... or planes each deposit site names: the MCRT_AOV_COUNT light-path planes of the
+                                 // path tracer (mcrt_render_accumulate_aovs_dev), the MCRT_PM_COMPONENT_COUNT estimator planes
+                                 // of the photon mapper (mcrt_render_accumulate_photon_components_dev)
     };
 
     // The wavefront loop shared by mcrt_render_rows(_dev) and mcrt_sample_rays. Camera work item w is sample
@@ -1798,7 +1800,7 @@ int mcrt_render_accumulate_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_
 
 namespace
 {
-    // The active-tile path of mcrt_render_accumulate_tiles_dev / _groups_dev / _aovs_dev (the caller has checked the sums)
+    // The active-tile path of mcrt_render_accumulate_tiles_dev and of accumulatePlanes (the caller has checked the sums)
     int accumulateTiles(mcrt_ctx* ctx, const std::string& name, const mcrt_camera* camera, uint32_t y_first, uint32_t y_step,
                         uint32_t n_rows, uint32_t tile, const uint8_t* active_tiles, uint32_t sample_first, uint32_t sample_count,
                         uint32_t global_seed, int integrator_kind, int precision, const FilmSums& sums, mcrt_stats* stats)
@@ -1844,6 +1846,22 @@ namespace
         CK(cudaMemcpyAsync(ctx->d_pixel_list, list.data(), list.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
         return renderDispatch(ctx, camera, y_first, y_step, n_rows, sample_first, sample_count, global_seed, integrator_kind,
                               precision, nullptr, stats, &sums, ctx->d_pixel_list, (uint32_t)list.size());
+    }
+
+    // The tail of mcrt_render_accumulate_groups_dev / _aovs_dev / _photon_components_dev, whose planes the caller has
+    // checked: a uniform pass, or an active-tile pass when a mask is given
+    int accumulatePlanes(mcrt_ctx* ctx, const std::string& name, const mcrt_camera* camera, uint32_t y_first, uint32_t y_step,
+                         uint32_t n_rows, uint32_t tile, const uint8_t* active_tiles, uint32_t sample_first, uint32_t sample_count,
+                         uint32_t global_seed, int integrator_kind, int precision, const FilmSums& sums, mcrt_stats* stats)
+    {
+        int rc;
+        if ((rc = checkAccumulateSums(ctx, name.c_str(), sample_count, sums.rgb, nullptr))) return rc;
+        if (active_tiles)
+            return accumulateTiles(ctx, name, camera, y_first, y_step, n_rows, tile, active_tiles, sample_first, sample_count, global_seed,
+                                   integrator_kind, precision, sums, stats);
+        CK(cudaSetDevice(ctx->device));
+        return renderDispatch(ctx, camera, y_first, y_step, n_rows, sample_first, sample_count, global_seed, integrator_kind,
+                              precision, nullptr, stats, &sums);
     }
 }
 
@@ -1925,15 +1943,8 @@ int mcrt_render_accumulate_groups_dev(mcrt_ctx* ctx, const mcrt_camera* camera, 
                      " groups + the sky";
         return MCRT_ERR_INVALID;
     }
-    int rc;
-    if ((rc = checkAccumulateSums(ctx, name.c_str(), sample_count, planes_dev, nullptr))) return rc;
-    const FilmSums sums = { planes_dev, nullptr, n_planes };
-    if (active_tiles)
-        return accumulateTiles(ctx, name, camera, y_first, y_step, n_rows, tile, active_tiles, sample_first, sample_count, global_seed,
-                               integrator_kind, precision, sums, stats);
-    CK(cudaSetDevice(ctx->device));
-    return renderDispatch(ctx, camera, y_first, y_step, n_rows, sample_first, sample_count, global_seed, integrator_kind,
-                          precision, nullptr, stats, &sums);
+    return accumulatePlanes(ctx, name, camera, y_first, y_step, n_rows, tile, active_tiles, sample_first, sample_count, global_seed,
+                            integrator_kind, precision, FilmSums{ planes_dev, nullptr, n_planes }, stats);
 }
 
 int mcrt_render_accumulate_aovs_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_t y_first, uint32_t y_step, uint32_t n_rows,
@@ -1954,15 +1965,39 @@ int mcrt_render_accumulate_aovs_dev(mcrt_ctx* ctx, const mcrt_camera* camera, ui
         ctx->error = name + ": n_planes " + std::to_string(n_planes) + ", an AOV render has " + std::to_string(MCRT_AOV_COUNT);
         return MCRT_ERR_INVALID;
     }
-    int rc;
-    if ((rc = checkAccumulateSums(ctx, name.c_str(), sample_count, planes_dev, nullptr))) return rc;
-    const FilmSums sums = { planes_dev, nullptr, n_planes, true };
-    if (active_tiles)
-        return accumulateTiles(ctx, name, camera, y_first, y_step, n_rows, tile, active_tiles, sample_first, sample_count, global_seed,
-                               integrator_kind, precision, sums, stats);
-    CK(cudaSetDevice(ctx->device));
-    return renderDispatch(ctx, camera, y_first, y_step, n_rows, sample_first, sample_count, global_seed, integrator_kind,
-                          precision, nullptr, stats, &sums);
+    return accumulatePlanes(ctx, name, camera, y_first, y_step, n_rows, tile, active_tiles, sample_first, sample_count, global_seed,
+                            integrator_kind, precision, FilmSums{ planes_dev, nullptr, n_planes, true }, stats);
+}
+
+int mcrt_render_accumulate_photon_components_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_t y_first, uint32_t y_step,
+                                                 uint32_t n_rows, uint32_t tile, const uint8_t* active_tiles,
+                                                 uint32_t sample_first, uint32_t sample_count, uint32_t global_seed,
+                                                 int integrator_kind, int precision, double* planes_dev, uint32_t n_planes,
+                                                 mcrt_stats* stats)
+{
+    if (!ctx) return MCRT_ERR_INVALID;
+    const std::string name = "mcrt_render_accumulate_photon_components_dev";
+    // an allowlist: every kind but the photon mapper would run the path tracer's AOV kernels, whose planes go up to 7
+    if (integrator_kind == MCRT_INTEGRATOR_PATH)
+    {
+        ctx->error = name + ": the path tracer has no photon-mapper components (it has light-path AOVs)";
+        return MCRT_ERR_UNSUPPORTED;
+    }
+    if (integrator_kind != MCRT_INTEGRATOR_PHOTON)
+    {
+        ctx->error = name + ": unknown integrator kind " + std::to_string(integrator_kind);
+        return MCRT_ERR_INVALID;
+    }
+    if (!ctx->film_default) { ctx->error = name + ": component planes take the box film only"; return MCRT_ERR_UNSUPPORTED; }
+    if (n_planes != MCRT_PM_COMPONENT_COUNT)
+    {
+        ctx->error = name + ": n_planes " + std::to_string(n_planes) + ", a component render has " +
+                     std::to_string(MCRT_PM_COMPONENT_COUNT);
+        return MCRT_ERR_INVALID;
+    }
+    // the kernels' FILM_MODE_AOV instantiations: each deposit site names its plane, here the MCRT_PM_* estimator planes
+    return accumulatePlanes(ctx, name, camera, y_first, y_step, n_rows, tile, active_tiles, sample_first, sample_count, global_seed,
+                            integrator_kind, precision, FilmSums{ planes_dev, nullptr, n_planes, true }, stats);
 }
 
 int mcrt_light_groups_combine_dev(mcrt_ctx* ctx, const double* planes_dev, uint32_t n_planes, uint64_t n_values,

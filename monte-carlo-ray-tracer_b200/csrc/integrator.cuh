@@ -258,7 +258,8 @@ namespace mcrt
         FilmParams filmp;           // reconstruction filter (default box: only `film` is used)
         // light-group render (mcrt_render_accumulate_groups_dev): `film` holds n_planes planes of plane_values values each;
         // a contribution of light l goes to plane group_of_light[l], the sky's to plane n_planes - 1. 0: one plane.
-        // AOV render (mcrt_render_accumulate_aovs_dev, aovs = 1): n_planes = MCRT_AOV_COUNT light-path planes instead
+        // AOV render (mcrt_render_accumulate_aovs_dev, aovs = 1): n_planes = MCRT_AOV_COUNT light-path planes instead;
+        // photon-mapper components (mcrt_render_accumulate_photon_components_dev, aovs = 1): MCRT_PM_COMPONENT_COUNT
         const uint32_t* group_of_light;
         size_t plane_values;
         uint32_t n_planes;
@@ -360,7 +361,8 @@ namespace mcrt
 
     // Film modes of the depositing kernels. FILM_MODE_BOX: the default box film, the kernels every benchmark and parity
     // case runs; FILM_MODE_SPLAT: a reconstruction filter; FILM_MODE_GROUPS: the box film with one plane per light group;
-    // FILM_MODE_AOV: the box film with one plane per light-path class (MCRT_AOV_*)
+    // FILM_MODE_AOV: the box film with one plane per class of contribution, the plane each deposit site names - the
+    // light-path planes (MCRT_AOV_*) in the path tracer, the estimator planes (MCRT_PM_*) in the photon mapper
     enum FilmMode : int { FILM_MODE_BOX = 0, FILM_MODE_SPLAT = 1, FILM_MODE_GROUPS = 2, FILM_MODE_AOV = 3 };
 
     // AOV plane of a contribution. lobe: interaction type + 1 of the path's first scattering vertex, 0 for the camera
@@ -679,7 +681,8 @@ namespace mcrt
             V3<R> sh_o, sh_d, sh_k;
             R sh_bsdf_pdf = R(0), sh_area_cos = R(0), sh_select = R(0);
             uint32_t sh_light = NO_PRIM;
-            // FILM_MODE_AOV: interaction type + 1 of the path's first vertex (0 before it), the shadow ray's AOV plane
+            // FILM_MODE_AOV: interaction type + 1 of the path's first vertex (0 before it; path tracer only), the shadow
+            // ray's plane
             uint32_t lobe = 0, sh_plane = 0;
 
             if (alive)
@@ -694,7 +697,7 @@ namespace mcrt
                 ls_light = meta2.x;
                 ior_count = meta2.y & 0xFFu;
                 ray.dirac_delta = (meta2.y >> 8) & 1u;
-                if constexpr (FILM == FILM_MODE_AOV) lobe = (meta2.y >> 9) & 3u;
+                if constexpr (KIND == 0 && FILM == FILM_MODE_AOV) lobe = (meta2.y >> 9) & 3u;
                 ray.refraction = false;
                 const uint32_t film_index = meta2.z;
 
@@ -754,7 +757,8 @@ namespace mcrt
                         if (ray.depth == 0 || ray.dirac_delta)
                         {
                             depositRadiance<FILM>(p, film_index, meta.x, meta.y, m.emittance * throughput, ps.light,
-                                                  FILM == FILM_MODE_AOV ? aovPlane(lobe, ray.depth > 1u, false) : 0u);
+                                                  FILM != FILM_MODE_AOV ? 0u : (KIND == 0 ? aovPlane(lobe, ray.depth > 1u, false)
+                                                                                          : (uint32_t)MCRT_PM_EMISSION));
                         }
                         else if (ls_light != NO_PRIM && sc.lights[ls_light].prim == hit.prim)
                         {
@@ -762,12 +766,13 @@ namespace mcrt
                             R light_pdf = pow2(ia.t) / (ps.area * cos_light_theta);
                             R mis_weight = powerHeuristic(ls_bsdf_pdf, light_pdf);
                             depositRadiance<FILM>(p, film_index, meta.x, meta.y, (mis_weight * m.emittance / ls_select) * throughput, ls_light,
-                                                  FILM == FILM_MODE_AOV ? aovPlane(lobe, ray.depth > 1u, false) : 0u);
+                                                  FILM != FILM_MODE_AOV ? 0u : (KIND == 0 ? aovPlane(lobe, ray.depth > 1u, false)
+                                                                                          : (uint32_t)MCRT_PM_DIRECT));
                         }
                     }
 
                     // the camera ray's hit is the first vertex: its lobe is the path's, for NEE here and everything after
-                    if constexpr (FILM == FILM_MODE_AOV) if (ray.depth == 0) lobe = ia.type + 1u;
+                    if constexpr (KIND == 0 && FILM == FILM_MODE_AOV) if (ray.depth == 0) lobe = ia.type + 1u;
 
                     // ---- PhotonMapper::sampleRay control flow, photon-mapper.cpp:299-332
                     bool do_direct = true, do_bsdf = true;
@@ -855,7 +860,7 @@ namespace mcrt
                                     sh_area_cos = L.area * cos_light_theta;
                                     sh_select = ls_select;
                                     sh_light = L.prim;
-                                    if constexpr (FILM == FILM_MODE_AOV) sh_plane = aovPlane(lobe, ray.depth > 0u, false);
+                                    if constexpr (FILM == FILM_MODE_AOV) sh_plane = KIND == 0 ? aovPlane(lobe, ray.depth > 0u, false) : (uint32_t)MCRT_PM_DIRECT;
                                 }
                             }
                         }
@@ -1216,7 +1221,8 @@ namespace mcrt
 
     // ------------------------------------------------------------------------------------------
     // k_knn: one warp per photon-map query emitted by k_shade<R,1>; search + radiance estimate.
-    // FILM_MODE_GROUPS splits the estimate by the light group of each photon (depositGroupRuns).
+    // FILM_MODE_GROUPS splits the estimate by the light group of each photon (depositGroupRuns); FILM_MODE_AOV deposits
+    // the whole estimate into its map's component plane, MCRT_PM_CAUSTIC + which.
     template <class R, int SLOTS, int FILM, uint32_t FEATS>
     __global__ void __launch_bounds__(32 * KNN_WARPS_PER_BLOCK, MCRT_KNN_MINBLOCKS) k_knn(WaveParams<R> p)
     {
@@ -1300,7 +1306,8 @@ namespace mcrt
             {
                 V3<R> radiance = which == 0 ? R(3) * sum * inv_max_r2 * Consts<R>::INV_PI
                                             : sum / (top_d2 * Consts<R>::PI);
-                depositRadiance<FILM>(p, qr.meta.y, pixelOfFilmIndex(p, qr.meta.y), qr.meta.w, radiance * qr.weight_t.xyz());
+                depositRadiance<FILM>(p, qr.meta.y, pixelOfFilmIndex(p, qr.meta.y), qr.meta.w, radiance * qr.weight_t.xyz(), NO_PRIM,
+                                      MCRT_PM_CAUSTIC + which);
             }
             __syncwarp();
         }
@@ -1342,7 +1349,8 @@ namespace mcrt
     // the k nearest photons: every photon within r (gatherWarp) enters the estimate with k_knn's formulas, r^2 in
     // place of the k-th distance2 - caustic 3/(pi r^2) sum flux f/pdf (1 - d/r), global 1/(pi r^2) sum flux f/pdf.
     // The BSDF is evaluated on the lane that finds the photon, while the batch streams.
-    // FILM_MODE_GROUPS splits the estimate by light group as k_knn does, one step per 32 photons streamed.
+    // FILM_MODE_GROUPS splits the estimate by light group as k_knn does, one step per 32 photons streamed; FILM_MODE_AOV
+    // deposits into the map's component plane as k_knn does.
     template <class R, int FILM, uint32_t FEATS>
     __global__ void __launch_bounds__(32 * KNN_WARPS_PER_BLOCK, MCRT_GATHER_MINBLOCKS) k_gather(WaveParams<R> p)
     {
@@ -1413,7 +1421,8 @@ namespace mcrt
             if (lane == 0)
             {
                 V3<R> radiance = which == 0 ? R(3) * sum * inv_r2 * Consts<R>::INV_PI : sum / ((R)r2 * Consts<R>::PI);
-                depositRadiance<FILM>(p, qr.meta.y, pixelOfFilmIndex(p, qr.meta.y), qr.meta.w, radiance * qr.weight_t.xyz());
+                depositRadiance<FILM>(p, qr.meta.y, pixelOfFilmIndex(p, qr.meta.y), qr.meta.w, radiance * qr.weight_t.xyz(), NO_PRIM,
+                                      MCRT_PM_CAUSTIC + which);
             }
             __syncwarp();
         }

@@ -60,6 +60,12 @@ namespace mcrt
     {
         const bool lite = (p.scene.material_flags_any & ~SHADE_FEATS_LITE) == 0;
         if (!p.filmp.is_default_box) k_shade<MCRT_REAL, 1, FILM_MODE_SPLAT, SHADE_FEATS_ALL><<<grid * 2, 128, 0, s>>>(p, cur);
+        else if (p.n_planes && p.aovs)
+        {
+            // photon-mapper components: FILM_MODE_AOV deposits into the plane each site names (MCRT_PM_*)
+            if (lite) k_shade<MCRT_REAL, 1, FILM_MODE_AOV, SHADE_FEATS_LITE><<<grid * 2, 128, 0, s>>>(p, cur);
+            else k_shade<MCRT_REAL, 1, FILM_MODE_AOV, SHADE_FEATS_ALL><<<grid * 2, 128, 0, s>>>(p, cur);
+        }
         else if (p.n_planes)
         {
             if (lite) k_shade<MCRT_REAL, 1, FILM_MODE_GROUPS, SHADE_FEATS_LITE><<<grid * 2, 128, 0, s>>>(p, cur);
@@ -76,6 +82,11 @@ namespace mcrt
             // fixed-radius gather (mcrt_photon_gather_radius) in place of the k-NN estimate
             const bool lite = (p.scene.material_flags_any & ~SHADE_FEATS_LITE) == 0;
             if (!p.filmp.is_default_box) k_gather<MCRT_REAL, FILM_MODE_SPLAT, SHADE_FEATS_ALL><<<g, b, 0, s>>>(p);
+            else if (p.n_planes && p.aovs)
+            {
+                if (lite) k_gather<MCRT_REAL, FILM_MODE_AOV, SHADE_FEATS_LITE><<<g, b, 0, s>>>(p);
+                else k_gather<MCRT_REAL, FILM_MODE_AOV, SHADE_FEATS_ALL><<<g, b, 0, s>>>(p);
+            }
             else if (p.n_planes)
             {
                 if (lite) k_gather<MCRT_REAL, FILM_MODE_GROUPS, SHADE_FEATS_LITE><<<g, b, 0, s>>>(p);
@@ -97,7 +108,8 @@ namespace mcrt
             return;
         }
         const bool lite = (p.scene.material_flags_any & ~SHADE_FEATS_LITE) == 0;
-        const bool groups = p.n_planes != 0;   // light-group planes
+        // film mode of the box film: one plane, light-group planes, or the photon mapper's component planes (FILM_MODE_AOV)
+        const int film_mode = !p.n_planes ? FILM_MODE_BOX : (p.aovs ? FILM_MODE_AOV : FILM_MODE_GROUPS);
         const int slots = knnSlotsFor(p.pm.k_nearest);
         // k > 672 needs more than the default 48 KB of dynamic shared memory (knnSharedBytes)
         #define MCRT_KNN_LAUNCH2(SL, FM, FE) \
@@ -105,7 +117,9 @@ namespace mcrt
                  if (!attr_set) { cudaFuncSetAttribute(k_knn<MCRT_REAL, SL, FM, FE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)knnSharedBytes(1024)); attr_set = true; } \
                  k_knn<MCRT_REAL, SL, FM, FE><<<g, b, smem, s>>>(p); } while (0)
         #define MCRT_KNN_LAUNCH1(SL, FE) \
-            do { if (groups) MCRT_KNN_LAUNCH2(SL, FILM_MODE_GROUPS, FE); else MCRT_KNN_LAUNCH2(SL, FILM_MODE_BOX, FE); } while (0)
+            do { if (film_mode == FILM_MODE_GROUPS) MCRT_KNN_LAUNCH2(SL, FILM_MODE_GROUPS, FE); \
+                 else if (film_mode == FILM_MODE_AOV) MCRT_KNN_LAUNCH2(SL, FILM_MODE_AOV, FE); \
+                 else MCRT_KNN_LAUNCH2(SL, FILM_MODE_BOX, FE); } while (0)
         #define MCRT_KNN_LAUNCH(SL) \
             do { if (lite) MCRT_KNN_LAUNCH1(SL, SHADE_FEATS_LITE); else MCRT_KNN_LAUNCH1(SL, SHADE_FEATS_ALL); } while (0)
         switch (slots)
@@ -120,7 +134,8 @@ namespace mcrt
         #undef MCRT_KNN_LAUNCH1
         #undef MCRT_KNN_LAUNCH2
     }
-    // k_shadow of the box film (one plane, light-group planes or AOV planes) with the scene-specialised traversal
+    // k_shadow of the box film (one plane, light-group planes, or AOV / photon-mapper component planes) with the
+    // scene-specialised traversal
     template <int FILM> static void launchShadowBox(const WaveParams<MCRT_REAL>& p, int grid, cudaStream_t s)
     {
         if constexpr (Mode<MCRT_REAL>::parity)
