@@ -7,7 +7,10 @@
 // sampler streams bit-exact, Scene::intersect same primitive and t, per-sample radiance and images
 // to 1e-9. Each function cites the reference lines it restates (paths relative to /root/reference).
 //
-// Not restated here: the photon mapper (checked directly against golden outputs on the GPU).
+// The photon mapper (photon-mapper.cpp:24-391) is restated too: the emission pass photon by photon in emission order, the
+// octree by the restated builder below, and PhotonMapper::sampleRay with a brute-force k-NN search in place of the octree
+// search. Pinned by tests/test_photon_mapper_oracle_cpu.py to pm_hexagon_room_64: maps bit-exact, per-sample radiance and
+// image to 1e-12, ray counts and k-NN results exact; tests/test_gpu_photon_mapper.py holds the device to it.
 #include <algorithm>
 #include <cmath>
 #include <cstdint>
@@ -555,13 +558,14 @@ namespace
         return r;
     }
 
-    bool sampleBSDF(const Interaction& ia, const Sampler& smp, D3& f, double& pdf, Ray& nr) // interaction.cpp:56-72
+    // flux: the photon pass's adjoint BSDF (photon-mapper.cpp:259), which keeps the (n2/n1)^2 of rough transmission
+    bool sampleBSDF(const Interaction& ia, const Sampler& smp, D3& f, double& pdf, Ray& nr, bool flux = false) // interaction.cpp:56-72
     {
         nr = spawn(ia, smp);
         D3 wi = ia.cs.to(nr.direction);
         if ((nr.refraction && wi.z >= 0.0) || (!nr.refraction && wi.z <= 0.0)) return false;
         D3 wo = ia.cs.to(ia.out);
-        f = ia.bsdfLocal(wo, wi, pdf, false, nr.dirac_delta) * std::abs(wi.z);
+        f = ia.bsdfLocal(wo, wi, pdf, flux, nr.dirac_delta) * std::abs(wi.z);
         return pdf > 0.0;
     }
 
@@ -1373,10 +1377,12 @@ namespace
         std::vector<uint32_t> next;
         std::vector<uint8_t> leaf;
         std::vector<float> photons;
+        std::vector<uint64_t> tags;
     };
 
-    void octreeBuild(OctreeOut& out, std::vector<float>& data, std::vector<float>& scratch, uint64_t begin, uint64_t end,
-                     const double* bmin, const double* bmax, uint32_t max_node_data, bool last, int depth)
+    // tags: optional per-photon values (the path that stored the photon) moved along with the photons
+    void octreeBuild(OctreeOut& out, std::vector<float>& data, std::vector<float>& scratch, std::vector<uint64_t>* tags, uint64_t begin,
+                     uint64_t end, const double* bmin, const double* bmax, uint32_t max_node_data, bool last, int depth)
     {
         const uint64_t count = end - begin;
         const uint32_t idx = (uint32_t)out.leaf.size();
@@ -1412,13 +1418,16 @@ namespace
             starts[0] = begin;
             for (int o = 0; o < 8; o++) starts[o + 1] = starts[o] + counts[o];
             scratch.resize(8 * count);
+            std::vector<uint64_t> moved(tags ? count : 0);
             for (int o = 0; o < 8; o++) cursor[o] = starts[o] - begin;
             for (uint64_t i = begin; i < end; i++)
             {
                 const int o = octantOf(&data[8 * i]);
+                if (tags) moved[cursor[o]] = (*tags)[i];
                 std::memcpy(&scratch[8 * cursor[o]++], &data[8 * i], 32);
             }
             std::memcpy(&data[8 * begin], scratch.data(), 32 * count);
+            if (tags) std::copy(moved.begin(), moved.end(), tags->begin() + begin);
             int last_used = -1;
             for (int o = 0; o < 8; o++) if (counts[o]) last_used = o;
             for (int o = 0; o < 8; o++)
@@ -1431,7 +1440,7 @@ namespace
                     const double h = half[c] * 0.5;
                     cmin[c] = new_origin - h; cmax[c] = new_origin + h;
                 }
-                octreeBuild(out, data, scratch, starts[o], starts[o + 1], cmin, cmax, max_node_data, o == last_used, depth + 1);
+                octreeBuild(out, data, scratch, tags, starts[o], starts[o + 1], cmin, cmax, max_node_data, o == last_used, depth + 1);
             }
         }
         for (int c = 0; c < 3; c++) { out.bounds[6 * idx + c] = lo[c]; out.bounds[6 * idx + 3 + c] = hi[c]; }
@@ -1447,7 +1456,7 @@ void oracle_octree_build(const float* photons, uint64_t n, uint32_t max_node_dat
     auto* o = new OctreeOut();
     o->photons.assign(photons, photons + 8 * n);
     std::vector<float> scratch;
-    if (n) octreeBuild(*o, o->photons, scratch, 0, n, scene_bounds6, scene_bounds6 + 3, max_node_data, true, 0);
+    if (n) octreeBuild(*o, o->photons, scratch, nullptr, 0, n, scene_bounds6, scene_bounds6 + 3, max_node_data, true, 0);
     std::memset(out, 0, sizeof(*out));
     out->n_octants = (uint32_t)o->leaf.size();
     out->octant_bounds = o->bounds.data(); out->octant_start = o->start.data(); out->octant_count = o->count.data();
@@ -1457,6 +1466,385 @@ void oracle_octree_build(const float* photons, uint64_t n, uint32_t max_node_dat
 }
 
 void oracle_octree_free(void* handle) { delete static_cast<OctreeOut*>(handle); }
+
+// ---------------------------------------------------------------- photon mapper (photon-mapper.cpp, photon.hpp)
+namespace
+{
+    enum { PM_LIGHT = 0, PM_REJECT = 2 };                        // sampling.hpp:59-76
+    enum { PM_EMISSION, PM_DIRECT, PM_CAUSTIC, PM_GLOBAL };      // the four terms sampleRay adds up
+
+    struct PhotonList
+    {
+        std::vector<float> photons;      // [n][8] {flux.xyz, pos.xyz, phi, theta}
+        std::vector<uint64_t> emission;  // light << 32 | the light's emission index: the path that stored each photon
+    };
+
+    void storePhoton(PhotonList& list, D3 flux, D3 pos, D3 dir, uint64_t emission) // Photon::Photon, photon.hpp:7-12
+    {
+        const float theta = (float)std::atan2(std::sqrt(dir.x * dir.x + dir.y * dir.y), dir.z);
+        const float phi = (float)std::atan2(dir.y, dir.x);
+        const float v[8] = { (float)flux.x, (float)flux.y, (float)flux.z, (float)pos.x, (float)pos.y, (float)pos.z, phi, theta };
+        list.photons.insert(list.photons.end(), v, v + 8);
+        list.emission.push_back(emission);
+    }
+
+    D3 photonDir(float phi, float theta) // Photon::dir, photon.hpp:19-27: glibc's float sinf / cosf
+    {
+        const float sin_theta = std::sin(theta);
+        return D3((double)std::cos(phi) * sin_theta, (double)std::sin(phi) * sin_theta, (double)std::cos(theta));
+    }
+
+    void updateIORs(std::vector<double>& iors, const Ray& ray) // RefractionHistory::update, ray.cpp:80-93
+    {
+        if (ray.refraction_level > 0)
+        {
+            if (ray.refraction_level == (int)iors.size()) iors.push_back(ray.medium_ior);
+            else if (ray.refraction_level < (int)iors.size() - 1) iors.pop_back();
+        }
+    }
+
+    // PhotonMapper::emitPhoton, photon-mapper.cpp:225-277
+    void emitPhoton(const Scene& s, Ray ray, D3 flux, Sampler& smp, double non_caustic_reject, uint64_t emission, PhotonList& caustic,
+                    PhotonList& global)
+    {
+        std::vector<double> iors(1, ray.medium_ior);
+        while (true)
+        {
+            smp.shuffle();
+            Isect is = intersect(s, ray, nullptr);
+            if (is.prim == 0xFFFFFFFFu) return;
+            int ext = std::min(std::max(ray.refraction_level - 1, 0), (int)iors.size() - 1);
+            Interaction ia = makeInteraction(s, is, ray, iors[ext], smp);
+            if (!ia.material->dirac_delta) // :245-256: only where a non-delta interaction is possible
+            {
+                if (ray.dirac_delta) storePhoton(caustic, flux, ia.position, -ray.direction, emission);
+                else if (non_caustic_reject > smp.get(PM_REJECT)) storePhoton(global, flux / non_caustic_reject, ia.position, -ray.direction, emission);
+            }
+            D3 f; double pdf; Ray nr;
+            if (!sampleBSDF(ia, smp, f, pdf, nr, true)) return;
+            f = f / pdf;
+            double survive = std::min(compMax(f), 0.95); // :265-272: survival probability instead of flux scaling
+            if (survive == 0.0 || survive <= smp.get(ABSORB)) return;
+            flux = flux * (f / survive);
+            ray = nr;
+            updateIORs(iors, ray);
+        }
+    }
+
+    struct PhotonPass { OctreeOut maps[2]; uint64_t emissions = 0; };
+
+    // PhotonMapper::PhotonMapper's first pass, photon-mapper.cpp:24-110: emissions per light in proportion to its flux, emission
+    // j of light l drawn from the sampler at (l, j), every photon appended in emission order as a single thread does
+    void photonPass(const Scene& s, uint64_t emissions, double caustic_factor, uint32_t seed, PhotonList& caustic, PhotonList& global,
+                    uint64_t& total)
+    {
+        const size_t n_lights = s.light_prim.size();
+        const size_t photon_emissions = (size_t)((double)emissions * caustic_factor);
+        std::vector<D3> light_flux(n_lights);
+        double total_flux = 0.0;
+        for (size_t l = 0; l < n_lights; l++)
+        {
+            const uint32_t prim = s.light_prim[l];
+            light_flux[l] = D3(s.materials[s.prim_material[prim]].emittance) * s.prim_area[prim];
+            total_flux += 0.0 + light_flux[l].x + light_flux[l].y + light_flux[l].z; // glm::compAdd
+        }
+        const double non_caustic_reject = 1.0 / caustic_factor;
+        Sampler smp(seed);
+        total = 0;
+        for (size_t l = 0; l < n_lights; l++)
+        {
+            const uint32_t prim = s.light_prim[l];
+            const double share = (0.0 + light_flux[l].x + light_flux[l].y + light_flux[l].z) / total_flux;
+            const size_t n = (size_t)((double)photon_emissions * share);
+            const D3 photon_flux = light_flux[l] / (double)n;
+            total += n;
+            smp.initiate((uint32_t)l);
+            for (size_t j = 0; j < n; j++)
+            {
+                smp.setIndex((uint32_t)j);
+                const double u0 = smp.get(PM_LIGHT), u1 = smp.get(PM_LIGHT + 1), u2 = smp.get(PM_LIGHT + 2), u3 = smp.get(PM_LIGHT + 3);
+                const D3 pos = lightPoint(s, prim, u0, u1), normal = primNormal(s, prim, pos);
+                const double r = std::sqrt(u2), az = u3 * TWO_PI; // Sampling::cosWeightedHemi
+                const D3 dir = Frame(normal).from(D3(r * std::cos(az), r * std::sin(az), std::sqrt(1 - u2)));
+                emitPhoton(s, makeRay(pos + normal * EPS, dir, s.d.scene_ior), photon_flux, smp, non_caustic_reject, (uint64_t)l << 32 | j, caustic, global);
+            }
+        }
+    }
+
+    struct PhotonMaps
+    {
+        const Scene* s;
+        std::vector<float> photons[2];
+        uint32_t k;
+        bool direct_visualization;
+    };
+
+    struct PMCounts { uint64_t rays = 0, shadow_rays = 0, queries = 0, ties = 0; };
+
+    // LinearOctree::knnSearch as a brute-force float64 search over the whole map, then the estimates of photon-mapper.cpp:343-391.
+    // A photon at the k-th distance that is not taken while another at the same distance is counts a tie: the reference's choice
+    // between them depends on its octree walk, which this search does not restate.
+    // -> the min(k, n) nearest photons (distance2, index), farthest first, as the reference pops its max-heap of results
+    std::vector<std::pair<double, uint32_t>> knnBrute(const PhotonMaps& pm, int which, D3 p, PMCounts& cnt)
+    {
+        const std::vector<float>& ph = pm.photons[which];
+        const size_t n = ph.size() / 8;
+        cnt.queries++;
+        std::vector<std::pair<double, uint32_t>> d(n);
+        if (n == 0) return d;
+        for (size_t i = 0; i < n; i++)
+        {
+            const D3 v = p - D3(ph[8 * i + 3], ph[8 * i + 4], ph[8 * i + 5]); // glm::distance2
+            d[i] = { dot(v, v), (uint32_t)i };
+        }
+        const size_t k = std::min<size_t>(pm.k, n);
+        std::nth_element(d.begin(), d.begin() + (k - 1), d.end());
+        const double kth = d[k - 1].first;
+        for (size_t i = k; i < n; i++) if (d[i].first == kth) { cnt.ties++; break; }
+        d.resize(k);
+        std::sort(d.begin(), d.end(), [](const std::pair<double, uint32_t>& a, const std::pair<double, uint32_t>& b) { return a.first > b.first; });
+        return d;
+    }
+
+    D3 photonEstimate(const PhotonMaps& pm, int which, const Interaction& ia, PMCounts& cnt)
+    {
+        const std::vector<float>& ph = pm.photons[which];
+        const std::vector<std::pair<double, uint32_t>> d = knnBrute(pm, which, ia.position, cnt);
+        if (d.empty()) return D3();
+        const double max_distance2 = d[0].first, inv_max_distance2 = 1.0 / max_distance2;
+        D3 radiance;
+        for (const auto& r : d)
+        {
+            const float* p = &ph[8 * (size_t)r.second];
+            D3 f; double pdf;
+            if (!ia.bsdfWorld(f, photonDir(p[6], p[7]), pdf)) continue;
+            const D3 flux((double)p[0], (double)p[1], (double)p[2]);
+            if (which == 0) // cone filter, :383-386
+            {
+                const double wp = std::max(0.0, 1.0 - std::sqrt(r.first * inv_max_distance2));
+                radiance = radiance + (flux * f * wp) / pdf;
+            }
+            else radiance = radiance + flux * f / pdf;
+        }
+        if (which == 0) return 3.0 * radiance * inv_max_distance2 * INV_PI;
+        return radiance / (max_distance2 * PI);
+    }
+
+    // PhotonMapper::sampleRay, photon-mapper.cpp:279-341. comp: the radiance split into PM_EMISSION (emission seen directly or
+    // through delta vertices), PM_DIRECT (next-event estimation and its MIS partner), PM_CAUSTIC and PM_GLOBAL; the return value
+    // is the reference's running sum.
+    D3 pmSampleRay(const PhotonMaps& pm, Ray ray, Sampler& smp, D3 comp[4], PMCounts& cnt)
+    {
+        const Scene& s = *pm.s;
+        D3 radiance, throughput(1, 1, 1);
+        std::vector<double> iors(1, ray.medium_ior);
+        LightSample ls;
+        for (int c = 0; c < 4; c++) comp[c] = D3();
+        auto add = [&](int c, D3 v) { v = v * throughput; comp[c] = comp[c] + v; radiance = radiance + v; };
+        while (true)
+        {
+            smp.shuffle();
+            Isect is = intersect(s, ray, &cnt.rays);
+            if (is.prim == 0xFFFFFFFFu) return radiance; // no sky, :292-295
+            int ext = std::min(std::max(ray.refraction_level - 1, 0), (int)iors.size() - 1);
+            Interaction ia = makeInteraction(s, is, ray, iors[ext], smp);
+            add(ray.depth == 0 || ray.dirac_delta ? PM_EMISSION : PM_DIRECT, sampleEmissive(s, ia, ls));
+            if (ia.dirac_delta)
+            {
+                if (!ray.dirac_delta && ray.depth != 0) return radiance;
+            }
+            else
+            {
+                add(PM_CAUSTIC, photonEstimate(pm, 0, ia, cnt));
+                if (pm.direct_visualization || !(ray.dirac_delta || ray.depth == 0))
+                {
+                    add(PM_GLOBAL, photonEstimate(pm, 1, ia, cnt));
+                    return radiance;
+                }
+                uint64_t shadow = 0;
+                add(PM_DIRECT, sampleDirect(s, ia, ls, smp, &shadow));
+                cnt.shadow_rays += shadow; cnt.rays += shadow;
+            }
+            D3 f;
+            if (!sampleBSDF(ia, smp, f, ls.bsdf_pdf, ray)) return radiance;
+            throughput = throughput * (f / ls.bsdf_pdf);
+            double survive = compMax(throughput) * ray.refraction_scale; // Integrator::absorb, integrator.cpp:112-129
+            if (survive == 0.0) return radiance;
+            if (ray.diffuse_depth > 3 || ray.depth > 16)
+            {
+                survive = std::min(0.95, survive);
+                if (survive <= smp.get(ABSORB)) return radiance;
+                throughput = throughput / survive;
+            }
+            updateIORs(iors, ray);
+        }
+    }
+}
+
+// The photon pass: emissions * caustic_factor emissions over the scene's lights, the caustic and global photons built into
+// octrees (max_node_data photons per leaf, root box scene_bounds6) as oracle_octree_build does; emission[which] (n_photons of the
+// map): light << 32 | the light's emission index, the path that stored each photon, in map order. Memory owned by *handle
+// (oracle_photon_pass_free).
+void oracle_photon_pass(void* h, uint64_t emissions, double caustic_factor, uint32_t max_node_data, const double* scene_bounds6, uint32_t seed,
+                        void** handle, mcrt_photon_map_desc* caustic_out, mcrt_photon_map_desc* global_out, const uint64_t** emission,
+                        uint64_t* total_emissions)
+{
+    const Scene& s = *static_cast<Scene*>(h);
+    PhotonList lists[2];
+    auto* pass = new PhotonPass();
+    photonPass(s, emissions, caustic_factor, seed, lists[0], lists[1], pass->emissions);
+    mcrt_photon_map_desc* out[2] = { caustic_out, global_out };
+    for (int w = 0; w < 2; w++)
+    {
+        OctreeOut& o = pass->maps[w];
+        // the reference inserts its photons into the octree last first: every leaf of its maps holds them in reverse
+        // emission order (pm_hexagon_room_64's maps, bit for bit)
+        const uint64_t n = lists[w].emission.size();
+        o.photons.resize(8 * n); o.tags.resize(n);
+        for (uint64_t i = 0; i < n; i++)
+        {
+            std::memcpy(&o.photons[8 * i], &lists[w].photons[8 * (n - 1 - i)], 32);
+            o.tags[i] = lists[w].emission[n - 1 - i];
+        }
+        std::vector<float> scratch;
+        if (n) octreeBuild(o, o.photons, scratch, &o.tags, 0, n, scene_bounds6, scene_bounds6 + 3, max_node_data, true, 0);
+        std::memset(out[w], 0, sizeof(*out[w]));
+        out[w]->n_octants = (uint32_t)o.leaf.size();
+        out[w]->octant_bounds = o.bounds.data(); out[w]->octant_start = o.start.data(); out[w]->octant_count = o.count.data();
+        out[w]->octant_next_sibling = o.next.data(); out[w]->octant_leaf = o.leaf.data();
+        out[w]->n_photons = n; out[w]->photons = o.photons.data();
+        emission[w] = o.tags.data();
+    }
+    *total_emissions = pass->emissions;
+    *handle = pass;
+}
+
+void oracle_photon_pass_free(void* handle) { delete static_cast<PhotonPass*>(handle); }
+
+// PhotonMapper's second pass over given maps (only their photons are read): k nearest photons, direct_visualization
+void* oracle_pm_create(void* h, const mcrt_photon_map_desc* caustic, const mcrt_photon_map_desc* global, uint32_t k, uint32_t direct_visualization)
+{
+    auto* pm = new PhotonMaps();
+    pm->s = static_cast<Scene*>(h);
+    const mcrt_photon_map_desc* m[2] = { caustic, global };
+    for (int w = 0; w < 2; w++) copyv(pm->photons[w], m[w]->photons, 8 * (size_t)m[w]->n_photons);
+    pm->k = k;
+    pm->direct_visualization = direct_visualization != 0;
+    return pm;
+}
+
+void oracle_pm_destroy(void* pm) { delete static_cast<PhotonMaps*>(pm); }
+
+namespace
+{
+    void storeSample(const D3& r, const D3 comp[4], size_t i, double* rgb, double* comp_out)
+    {
+        rgb[3 * i] = r.x; rgb[3 * i + 1] = r.y; rgb[3 * i + 2] = r.z;
+        if (comp_out)
+            for (int c = 0; c < 4; c++) { double* o = comp_out + (4 * i + c) * 3; o[0] = comp[c].x; o[1] = comp[c].y; o[2] = comp[c].z; }
+    }
+    void storeCounts(const PMCounts& c, uint64_t* counts)
+    {
+        if (counts) { counts[0] = c.rays; counts[1] = c.shadow_rays; counts[2] = c.queries; counts[3] = c.ties; }
+    }
+}
+
+// per (ray, pixel, sample): rgb [n][3], comp [n][4][3] (may be null); counts: rays, shadow rays, k-NN queries, k-th distance ties
+void oracle_pm_sample_rays(void* pmh, const mcrt_ray* rays, const uint32_t* pixel, const uint32_t* sample, size_t n, uint32_t seed,
+                           double* rgb, double* comp, uint64_t* counts)
+{
+    const PhotonMaps& pm = *static_cast<PhotonMaps*>(pmh);
+    Sampler smp(seed);
+    PMCounts cnt;
+    for (size_t i = 0; i < n; i++)
+    {
+        smp.initiate(pixel[i]); smp.setIndex(sample[i]);
+        D3 c[4];
+        const D3 r = pmSampleRay(pm, makeRay(D3(rays[i].origin), D3(rays[i].direction), pm.s->d.scene_ior), smp, c, cnt);
+        storeSample(r, c, i, rgb, comp);
+    }
+    storeCounts(cnt, counts);
+}
+
+// the brute-force k-NN search on caller points: out_d2 / out_index [n][k] nearest first (unused slots: +inf / 0xFFFFFFFF),
+// out_count [n]; *ties: queries with a tie at the k-th distance
+void oracle_pm_knn(void* pmh, int which, const double* points, size_t n, double* out_d2, uint32_t* out_index, uint32_t* out_count, uint64_t* ties)
+{
+    const PhotonMaps& pm = *static_cast<PhotonMaps*>(pmh);
+    PMCounts cnt;
+    for (size_t i = 0; i < n; i++)
+    {
+        const std::vector<std::pair<double, uint32_t>> d = knnBrute(pm, which, D3(points + 3 * i), cnt);
+        out_count[i] = (uint32_t)d.size();
+        for (uint32_t j = 0; j < pm.k; j++)
+        {
+            const bool have = j < d.size();
+            out_d2[i * pm.k + j] = have ? d[d.size() - 1 - j].first : std::numeric_limits<double>::infinity();
+            out_index[i * pm.k + j] = have ? d[d.size() - 1 - j].second : 0xFFFFFFFFu;
+        }
+    }
+    *ties = cnt.ties;
+}
+
+// Camera::samplePixel for (pixel, sample) pairs, as oracle_sample_pixels; rays6 (may be null): the camera rays
+void oracle_pm_sample_pixels(void* pmh, const mcrt_camera* cam, const uint32_t* pixel, const uint32_t* sample, size_t n, uint32_t seed,
+                             double* rgb, double* comp, double* rays6, uint64_t* counts)
+{
+    const PhotonMaps& pm = *static_cast<PhotonMaps*>(pmh);
+    Sampler smp(seed);
+    PMCounts cnt;
+    for (size_t i = 0; i < n; i++)
+    {
+        smp.initiate(pixel[i]); smp.setIndex(sample[i]);
+        const Ray ray = cameraRay(*cam, pm.s->d.scene_ior, pixel[i], smp);
+        if (rays6)
+        {
+            const double v[6] = { ray.start.x, ray.start.y, ray.start.z, ray.direction.x, ray.direction.y, ray.direction.z };
+            std::memcpy(rays6 + 6 * i, v, sizeof(v));
+        }
+        D3 c[4];
+        const D3 r = pmSampleRay(pm, ray, smp, c, cnt);
+        storeSample(r, c, i, rgb, comp);
+    }
+    storeCounts(cnt, counts);
+}
+
+// rows [y0, y1) with the default box film, as oracle_render_rows; comp (may be null): [4][y1 - y0][width][3], each term's
+// mean over the pixel's samples (not clamped)
+void oracle_pm_render_rows(void* pmh, const mcrt_camera* cam, uint32_t y0, uint32_t y1, uint32_t sqrtspp, uint32_t seed, double* out,
+                           double* comp, uint64_t* counts)
+{
+    const PhotonMaps& pm = *static_cast<PhotonMaps*>(pmh);
+    Sampler smp(seed);
+    PMCounts cnt;
+    const uint32_t spp = sqrtspp * sqrtspp;
+    const size_t plane = (size_t)(y1 - y0) * cam->width * 3;
+    for (uint32_t y = y0; y < y1; y++)
+        for (uint32_t x = 0; x < cam->width; x++)
+        {
+            const uint32_t pixel = y * cam->width + x;
+            smp.initiate(pixel);
+            D3 sum, csum[4];
+            for (uint32_t i = 0; i < spp; i++)
+            {
+                smp.setIndex(i);
+                D3 c[4];
+                const D3 r = pmSampleRay(pm, cameraRay(*cam, pm.s->d.scene_ior, pixel, smp), smp, c, cnt);
+                sum = sum + r * 1.0; // Film::Splat::update, weight 1
+                for (int k = 0; k < 4; k++) csum[k] = csum[k] + c[k];
+            }
+            const size_t at = ((size_t)(y - y0) * cam->width + x) * 3;
+            const D3 v = sum / (double)spp;
+            out[at] = v.x < 0.0 ? 0.0 : v.x; out[at + 1] = v.y < 0.0 ? 0.0 : v.y; out[at + 2] = v.z < 0.0 ? 0.0 : v.z;
+            if (comp)
+                for (int k = 0; k < 4; k++)
+                {
+                    const D3 m = csum[k] / (double)spp;
+                    comp[k * plane + at] = m.x; comp[k * plane + at + 1] = m.y; comp[k * plane + at + 2] = m.z;
+                }
+        }
+    storeCounts(cnt, counts);
+}
 
 // Image::save without the file (image.cpp:37-88, histogram.cpp, pixel-operators.cpp, srgb.hpp:54-62)
 namespace

@@ -39,6 +39,19 @@ def lib():
         L.oracle_octree_free.argtypes = [C.c_void_p]
         L.oracle_image_tonemap.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_double)]
         L.oracle_render_film.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]
+        L.oracle_photon_pass.argtypes = [C.c_void_p, C.c_uint64, C.c_double, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(C.c_void_p),
+                                         C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)]
+        L.oracle_photon_pass_free.argtypes = [C.c_void_p]
+        L.oracle_pm_create.restype = C.c_void_p
+        L.oracle_pm_create.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32]
+        L.oracle_pm_destroy.argtypes = [C.c_void_p]
+        L.oracle_pm_sample_rays.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32, C.c_void_p, C.c_void_p,
+                                            C.c_void_p]
+        L.oracle_pm_sample_pixels.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32, C.c_void_p, C.c_void_p,
+                                              C.c_void_p, C.c_void_p]
+        L.oracle_pm_knn.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]
+        L.oracle_pm_render_rows.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p,
+                                            C.c_void_p]
         _lib = L
     return _lib
 
@@ -175,3 +188,92 @@ class PortScene:
         rays = C.c_uint64()
         lib().oracle_render_rows(self.h, C.addressof(camera.rec), y0, y1, sqrtspp, seed, _p(out), C.byref(rays))
         return out, rays.value
+
+    # ---------------------------------------------------------------------------------------- photon mapper
+    def photon_pass(self, emissions, caustic_factor, max_photons_per_octree_leaf, scene_bounds, seed):
+        """PhotonMapper::PhotonMapper's photon pass restated -> (caustic map, global map, (caustic lights, global lights),
+        total emissions, (caustic paths, global paths)). Maps are dicts as the product's _map_arrays returns; lights: the
+        emitting light of each photon; paths: light << 32 | the light's emission index, the path that stored each photon."""
+        bounds = np.ascontiguousarray(scene_bounds, dtype=np.float64).reshape(6)
+        h = C.c_void_p()
+        d = [self.pkg.PhotonMapDesc(), self.pkg.PhotonMapDesc()]
+        path_ptrs = (C.c_void_p * 2)()
+        total = C.c_uint64()
+        lib().oracle_photon_pass(self.h, int(emissions), float(caustic_factor), int(max_photons_per_octree_leaf), _p(bounds), int(seed),
+                                 C.byref(h), C.addressof(d[0]), C.addressof(d[1]), C.cast(path_ptrs, C.POINTER(C.c_void_p)), C.byref(total))
+        try:
+            maps = [self.pkg._map_arrays(m) for m in d]
+            paths = tuple(np.ctypeslib.as_array(C.cast(path_ptrs[w], C.POINTER(C.c_uint64)), shape=(int(d[w].n_photons),)).copy()
+                          if d[w].n_photons else np.zeros(0, np.uint64) for w in range(2))
+        finally:
+            lib().oracle_photon_pass_free(h)
+        return maps[0], maps[1], tuple((p >> np.uint64(32)).astype(np.uint32) for p in paths), total.value, paths
+
+    def photon_mapper(self, maps):
+        """PhotonMapper::sampleRay restated over `maps` = (caustic, global, k, direct_visualization), the tuple
+        PhotonMapper(photon_maps=...) takes."""
+        return PortPhotonMapper(self, maps)
+
+
+class PortPhotonMapper:
+    """The restatement's PhotonMapper::sampleRay over given maps. Every call returns (rgb, components, counts): components
+    [..., 4, 3] in the order of the product's PHOTON_COMPONENT_NAMES (emission, direct, caustic, global), counts a dict of
+    rays (every Scene::intersect call), shadow_rays, knn_queries and knn_ties (queries whose k-th distance is shared by a
+    photon left out: the reference's choice between them follows its octree walk, which the brute-force search does not
+    restate)."""
+
+    def __init__(self, ps, maps):
+        caustic, glob, k, dv = maps
+        self.ps = ps
+        self.k, self.direct_visualization = int(k), bool(dv)
+        self._keep = [np.ascontiguousarray(m["photons"], dtype=np.float32) for m in (caustic, glob)]
+        self._desc = []
+        for ph in self._keep:
+            d = ps.pkg.PhotonMapDesc()
+            d.n_photons = ph.size // 8
+            d.photons = ph.ctypes.data_as(C.c_void_p) if ph.size else None
+            self._desc.append(d)
+        self.h = lib().oracle_pm_create(ps.h, C.addressof(self._desc[0]), C.addressof(self._desc[1]), self.k, int(self.direct_visualization))
+
+    def close(self):
+        if self.h:
+            lib().oracle_pm_destroy(self.h); self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    @staticmethod
+    def _counts(c):
+        return dict(rays=int(c[0]), shadow_rays=int(c[1]), knn_queries=int(c[2]), knn_ties=int(c[3]))
+
+    def knn(self, which, points):
+        """brute-force k nearest photons of map `which` -> (index [n, k], distance2 [n, k] nearest first, count [n], ties)"""
+        points = np.ascontiguousarray(points, dtype=np.float64).reshape(-1, 3)
+        n = len(points)
+        d2 = np.zeros((n, self.k)); idx = np.zeros((n, self.k), np.uint32); cnt = np.zeros(n, np.uint32); ties = C.c_uint64()
+        lib().oracle_pm_knn(self.h, int(which), _p(points), n, _p(d2), _p(idx), _p(cnt), C.byref(ties))
+        return idx, d2, cnt, ties.value
+
+    def sample_rays(self, rays, pixel, sample, seed):
+        rays = np.ascontiguousarray(rays, dtype=np.float64).reshape(-1, 6)
+        pixel = np.ascontiguousarray(pixel, dtype=np.uint32); sample = np.ascontiguousarray(sample, dtype=np.uint32)
+        rgb = np.zeros((len(rays), 3)); comp = np.zeros((len(rays), 4, 3)); c = np.zeros(4, np.uint64)
+        lib().oracle_pm_sample_rays(self.h, _p(rays), _p(pixel), _p(sample), len(rays), seed, _p(rgb), _p(comp), _p(c))
+        return rgb, comp, self._counts(c)
+
+    def sample_pixels(self, camera, pixel, sample, seed):
+        """-> (rgb [n, 3], components [n, 4, 3], camera rays [n, 6], counts)"""
+        pixel = np.ascontiguousarray(pixel, dtype=np.uint32); sample = np.ascontiguousarray(sample, dtype=np.uint32)
+        n = len(pixel)
+        rgb = np.zeros((n, 3)); comp = np.zeros((n, 4, 3)); rays = np.zeros((n, 6)); c = np.zeros(4, np.uint64)
+        lib().oracle_pm_sample_pixels(self.h, C.addressof(camera.rec), _p(pixel), _p(sample), n, seed, _p(rgb), _p(comp), _p(rays), _p(c))
+        return rgb, comp, rays, self._counts(c)
+
+    def render_rows(self, camera, y0, y1, sqrtspp, seed):
+        """-> (frame [rows, width, 3], component frames [4, rows, width, 3] (per-pixel means), counts)"""
+        out = np.zeros((y1 - y0, camera.width, 3)); comp = np.zeros((4, y1 - y0, camera.width, 3)); c = np.zeros(4, np.uint64)
+        lib().oracle_pm_render_rows(self.h, C.addressof(camera.rec), y0, y1, sqrtspp, seed, _p(out), _p(comp), _p(c))
+        return out, comp, self._counts(c)
