@@ -890,7 +890,14 @@ class PhotonMapper(Integrator):
         p.emissions = int(emissions); p.caustic_factor = float(caustic_factor)
         p.max_photons_per_octree_leaf = int(max_photons_per_octree_leaf); p.k_nearest_photons = int(k_nearest_photons)
         p.direct_visualization = int(bool(direct_visualization)); p.global_seed = self.global_seed
-        b = scene_bounds if scene_bounds is not None else self.scene.a["node_bounds"][:6]
+        if scene_bounds is not None:
+            b = scene_bounds
+        elif self.scene.a["node_bounds"].size >= 6:
+            b = self.scene.a["node_bounds"][:6]   # the BVH root's box
+        elif "scene_bounds" in self.scene.extra:
+            b = self.scene.extra["scene_bounds"]  # a scene without a BVH: the pack's scene box
+        else:
+            raise McrtError("the scene has no BVH and no scene bounds: pass scene_bounds")
         for i in range(6):
             p.scene_bounds[i] = float(b[i])
         return p

@@ -14,7 +14,7 @@ def build(force=False):
     hdr = os.path.join(ROOT, "include", "mcrt_abi.h")
     os.makedirs(os.path.dirname(LIB), exist_ok=True)
     if force or not os.path.exists(LIB) or os.path.getmtime(LIB) < max(os.path.getmtime(src), os.path.getmtime(hdr)):
-        subprocess.check_call(["g++", "-std=c++17", "-O2", "-ffp-contract=off", "-fPIC", "-shared", "-I", os.path.join(ROOT, "include"),
+        subprocess.check_call(["g++", "-std=c++17", "-O2", "-ffp-contract=off", "-fPIC", "-shared", "-pthread", "-I", os.path.join(ROOT, "include"),
                                src, "-o", LIB])
     return LIB
 

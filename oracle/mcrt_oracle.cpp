@@ -15,8 +15,10 @@
 #include <cmath>
 #include <cstdint>
 #include <cstring>
+#include <functional>
 #include <limits>
 #include <memory>
+#include <thread>
 #include <vector>
 
 #include "mcrt_abi.h"
@@ -1534,9 +1536,12 @@ namespace
     struct PhotonPass { OctreeOut maps[2]; uint64_t emissions = 0; };
 
     // PhotonMapper::PhotonMapper's first pass, photon-mapper.cpp:24-110: emissions per light in proportion to its flux, emission
-    // j of light l drawn from the sampler at (l, j), every photon appended in emission order as a single thread does
-    void photonPass(const Scene& s, uint64_t emissions, double caustic_factor, uint32_t seed, PhotonList& caustic, PhotonList& global,
-                    uint64_t& total)
+    // j of light l drawn from the sampler at (l, j), every photon appended in emission order as a single thread does.
+    // Pass `pass` of progressive photon mapping (mcrt_photon_emit_pass) draws light l's emission j at (l, pass * n_l + j),
+    // computed in 64 bits and cast to the sampler's 32-bit index, with the flux of a one-pass map; pass 0 is the
+    // reference's pass. false, and nothing emitted, when a light's indices of the pass do not fit 32 bits.
+    bool photonPass(const Scene& s, uint64_t emissions, double caustic_factor, uint32_t pass, uint32_t seed, PhotonList& caustic,
+                    PhotonList& global, uint64_t& total)
     {
         const size_t n_lights = s.light_prim.size();
         const size_t photon_emissions = (size_t)((double)emissions * caustic_factor);
@@ -1548,27 +1553,36 @@ namespace
             light_flux[l] = D3(s.materials[s.prim_material[prim]].emittance) * s.prim_area[prim];
             total_flux += 0.0 + light_flux[l].x + light_flux[l].y + light_flux[l].z; // glm::compAdd
         }
+        std::vector<size_t> counts(n_lights);
+        for (size_t l = 0; l < n_lights; l++)
+        {
+            const double share = (0.0 + light_flux[l].x + light_flux[l].y + light_flux[l].z) / total_flux;
+            counts[l] = (size_t)((double)photon_emissions * share);
+            if (((uint64_t)pass + 1) * (uint64_t)counts[l] > 0x100000000ull) return false;
+        }
         const double non_caustic_reject = 1.0 / caustic_factor;
         Sampler smp(seed);
         total = 0;
         for (size_t l = 0; l < n_lights; l++)
         {
             const uint32_t prim = s.light_prim[l];
-            const double share = (0.0 + light_flux[l].x + light_flux[l].y + light_flux[l].z) / total_flux;
-            const size_t n = (size_t)((double)photon_emissions * share);
+            const size_t n = counts[l];
             const D3 photon_flux = light_flux[l] / (double)n;
             total += n;
             smp.initiate((uint32_t)l);
             for (size_t j = 0; j < n; j++)
             {
-                smp.setIndex((uint32_t)j);
+                const uint32_t index = (uint32_t)((uint64_t)pass * n + j);
+                smp.setIndex(index);
                 const double u0 = smp.get(PM_LIGHT), u1 = smp.get(PM_LIGHT + 1), u2 = smp.get(PM_LIGHT + 2), u3 = smp.get(PM_LIGHT + 3);
                 const D3 pos = lightPoint(s, prim, u0, u1), normal = primNormal(s, prim, pos);
                 const double r = std::sqrt(u2), az = u3 * TWO_PI; // Sampling::cosWeightedHemi
                 const D3 dir = Frame(normal).from(D3(r * std::cos(az), r * std::sin(az), std::sqrt(1 - u2)));
-                emitPhoton(s, makeRay(pos + normal * EPS, dir, s.d.scene_ior), photon_flux, smp, non_caustic_reject, (uint64_t)l << 32 | j, caustic, global);
+                emitPhoton(s, makeRay(pos + normal * EPS, dir, s.d.scene_ior), photon_flux, smp, non_caustic_reject, (uint64_t)l << 32 | index,
+                           caustic, global);
             }
         }
+        return true;
     }
 
     struct PhotonMaps
@@ -1577,9 +1591,12 @@ namespace
         std::vector<float> photons[2];
         uint32_t k;
         bool direct_visualization;
+        double gather_r2[2] = { 0.0, 0.0 };   // fixed gather radius^2 of the caustic / global map (k_gather); 0: k-NN
     };
 
-    struct PMCounts { uint64_t rays = 0, shadow_rays = 0, queries = 0, ties = 0; };
+    // queries: photon-map queries, ties: k-NN queries with a tie at the k-th distance, empty: queries that took no photon,
+    // photons: photons taken by all queries
+    struct PMCounts { uint64_t rays = 0, shadow_rays = 0, queries = 0, ties = 0, empty = 0, photons = 0; };
 
     // LinearOctree::knnSearch as a brute-force float64 search over the whole map, then the estimates of photon-mapper.cpp:343-391.
     // A photon at the k-th distance that is not taken while another at the same distance is counts a tie: the reference's choice
@@ -1606,12 +1623,37 @@ namespace
         return d;
     }
 
-    D3 photonEstimate(const PhotonMaps& pm, int which, const Interaction& ia, PMCounts& cnt)
+    // The fixed-radius search of progressive photon mapping (gatherWarp, k_gather_user) as a brute force: every photon whose
+    // float64 distance2 is <= r2, the same inclusive test. -> (distance2, index), farthest first, as knnBrute
+    std::vector<std::pair<double, uint32_t>> gatherBrute(const PhotonMaps& pm, int which, D3 p, double r2, PMCounts& cnt)
     {
         const std::vector<float>& ph = pm.photons[which];
-        const std::vector<std::pair<double, uint32_t>> d = knnBrute(pm, which, ia.position, cnt);
-        if (d.empty()) return D3();
-        const double max_distance2 = d[0].first, inv_max_distance2 = 1.0 / max_distance2;
+        const size_t n = ph.size() / 8;
+        cnt.queries++;
+        std::vector<std::pair<double, uint32_t>> d;
+        for (size_t i = 0; i < n; i++)
+        {
+            const D3 v = p - D3(ph[8 * i + 3], ph[8 * i + 4], ph[8 * i + 5]);
+            const double d2 = dot(v, v);
+            if (d2 <= r2) d.push_back({ d2, (uint32_t)i });
+        }
+        std::sort(d.begin(), d.end(), [](const std::pair<double, uint32_t>& a, const std::pair<double, uint32_t>& b) { return a.first > b.first; });
+        return d;
+    }
+
+    double coneWeight(double d2, double inv_r2) { return std::max(0.0, 1.0 - std::sqrt(d2 * inv_r2)); } // :383-386
+
+    // The estimates of photon-mapper.cpp:343-391 over the photons a query takes: with gather_r2 0 the k nearest (knnBrute),
+    // normalised by the k-th distance2; otherwise every photon within the fixed radius (gatherBrute), normalised by r^2, as
+    // k_gather does. Only the selection and the normaliser r2 differ between the two. A query that takes no photon adds nothing.
+    D3 photonEstimate(const PhotonMaps& pm, int which, const Interaction& ia, double gather_r2, PMCounts& cnt)
+    {
+        const std::vector<float>& ph = pm.photons[which];
+        const std::vector<std::pair<double, uint32_t>> d = gather_r2 > 0.0 ? gatherBrute(pm, which, ia.position, gather_r2, cnt)
+                                                                            : knnBrute(pm, which, ia.position, cnt);
+        cnt.photons += d.size();
+        if (d.empty()) { cnt.empty++; return D3(); }
+        const double r2 = gather_r2 > 0.0 ? gather_r2 : d[0].first, inv_r2 = 1.0 / r2;
         D3 radiance;
         for (const auto& r : d)
         {
@@ -1619,15 +1661,11 @@ namespace
             D3 f; double pdf;
             if (!ia.bsdfWorld(f, photonDir(p[6], p[7]), pdf)) continue;
             const D3 flux((double)p[0], (double)p[1], (double)p[2]);
-            if (which == 0) // cone filter, :383-386
-            {
-                const double wp = std::max(0.0, 1.0 - std::sqrt(r.first * inv_max_distance2));
-                radiance = radiance + (flux * f * wp) / pdf;
-            }
+            if (which == 0) radiance = radiance + (flux * f * coneWeight(r.first, inv_r2)) / pdf; // cone filter
             else radiance = radiance + flux * f / pdf;
         }
-        if (which == 0) return 3.0 * radiance * inv_max_distance2 * INV_PI;
-        return radiance / (max_distance2 * PI);
+        if (which == 0) return 3.0 * radiance * inv_r2 * INV_PI;
+        return radiance / (r2 * PI);
     }
 
     // PhotonMapper::sampleRay, photon-mapper.cpp:279-341. comp: the radiance split into PM_EMISSION (emission seen directly or
@@ -1655,10 +1693,10 @@ namespace
             }
             else
             {
-                add(PM_CAUSTIC, photonEstimate(pm, 0, ia, cnt));
+                add(PM_CAUSTIC, photonEstimate(pm, 0, ia, pm.gather_r2[0], cnt));
                 if (pm.direct_visualization || !(ray.dirac_delta || ray.depth == 0))
                 {
-                    add(PM_GLOBAL, photonEstimate(pm, 1, ia, cnt));
+                    add(PM_GLOBAL, photonEstimate(pm, 1, ia, pm.gather_r2[1], cnt));
                     return radiance;
                 }
                 uint64_t shadow = 0;
@@ -1684,15 +1722,19 @@ namespace
 // The photon pass: emissions * caustic_factor emissions over the scene's lights, the caustic and global photons built into
 // octrees (max_node_data photons per leaf, root box scene_bounds6) as oracle_octree_build does; emission[which] (n_photons of the
 // map): light << 32 | the light's emission index, the path that stored each photon, in map order. Memory owned by *handle
-// (oracle_photon_pass_free).
-void oracle_photon_pass(void* h, uint64_t emissions, double caustic_factor, uint32_t max_node_data, const double* scene_bounds6, uint32_t seed,
-                        void** handle, mcrt_photon_map_desc* caustic_out, mcrt_photon_map_desc* global_out, const uint64_t** emission,
-                        uint64_t* total_emissions)
+// (oracle_photon_pass_free). pass_index: the photon pass of progressive photon mapping (photonPass); returns 0, or -1 and
+// no handle when the pass's emission indices do not fit 32 bits.
+int oracle_photon_pass(void* h, uint64_t emissions, double caustic_factor, uint32_t max_node_data, const double* scene_bounds6,
+                       uint32_t pass_index, uint32_t seed, void** handle, mcrt_photon_map_desc* caustic_out, mcrt_photon_map_desc* global_out,
+                       const uint64_t** emission, uint64_t* total_emissions)
 {
     const Scene& s = *static_cast<Scene*>(h);
     PhotonList lists[2];
+    uint64_t total = 0;
+    *handle = nullptr;
+    if (!photonPass(s, emissions, caustic_factor, pass_index, seed, lists[0], lists[1], total)) return -1;
     auto* pass = new PhotonPass();
-    photonPass(s, emissions, caustic_factor, seed, lists[0], lists[1], pass->emissions);
+    pass->emissions = total;
     mcrt_photon_map_desc* out[2] = { caustic_out, global_out };
     for (int w = 0; w < 2; w++)
     {
@@ -1717,6 +1759,7 @@ void oracle_photon_pass(void* h, uint64_t emissions, double caustic_factor, uint
     }
     *total_emissions = pass->emissions;
     *handle = pass;
+    return 0;
 }
 
 void oracle_photon_pass_free(void* handle) { delete static_cast<PhotonPass*>(handle); }
@@ -1735,6 +1778,78 @@ void* oracle_pm_create(void* h, const mcrt_photon_map_desc* caustic, const mcrt_
 
 void oracle_pm_destroy(void* pm) { delete static_cast<PhotonMaps*>(pm); }
 
+// Following estimates gather every photon within r_caustic / r_global (k_gather, mcrt_photon_gather_radius); (0, 0): k-NN.
+// Returns -1, and changes nothing, for radii mcrt_photon_gather_radius refuses.
+int oracle_pm_gather_radius(void* pmh, double r_caustic, double r_global)
+{
+    PhotonMaps& pm = *static_cast<PhotonMaps*>(pmh);
+    if (r_caustic == 0.0 && r_global == 0.0) { pm.gather_r2[0] = pm.gather_r2[1] = 0.0; return 0; }
+    const double r[2] = { r_caustic, r_global };
+    for (int w = 0; w < 2; w++)
+        if (!(r[w] > 0.0) || !std::isfinite(r[w] * r[w])) return -1;
+    pm.gather_r2[0] = r_caustic * r_caustic; pm.gather_r2[1] = r_global * r_global;
+    return 0;
+}
+
+// The fixed-radius search on caller points, as mcrt_photon_gather_search: per point the number of photons of map `which`
+// within radius, the float64 sums of their flux and of their flux times the cone weight
+void oracle_pm_gather(void* pmh, int which, const double* points, size_t n, double radius, uint32_t* out_count, double* out_flux,
+                      double* out_cone)
+{
+    const PhotonMaps& pm = *static_cast<PhotonMaps*>(pmh);
+    const std::vector<float>& ph = pm.photons[which];
+    const double r2 = radius * radius, inv_r2 = 1.0 / r2;
+    PMCounts cnt;
+    for (size_t i = 0; i < n; i++)
+    {
+        const std::vector<std::pair<double, uint32_t>> d = gatherBrute(pm, which, D3(points + 3 * i), r2, cnt);
+        D3 f, c;
+        for (const auto& r : d)
+        {
+            const float* p = &ph[8 * (size_t)r.second];
+            const D3 flux((double)p[0], (double)p[1], (double)p[2]);
+            f = f + flux;
+            c = c + flux * coneWeight(r.first, inv_r2);
+        }
+        out_count[i] = (uint32_t)d.size();
+        const double v[6] = { f.x, f.y, f.z, c.x, c.y, c.z };
+        std::memcpy(out_flux + 3 * i, v, 24); std::memcpy(out_cone + 3 * i, v + 3, 24);
+    }
+}
+
+// The estimate of map `which` at the first vertex of each (ray, pixel, sample), as pmSampleRay makes it there, with
+// gather radius radius[i] (0: the k-NN estimate). out [n][3]: the estimate (0 where the ray misses or the vertex is a delta
+// one), position [n][3]: the vertex (NaN where the ray misses), estimated [n]: 1 where the estimate ran
+void oracle_pm_first_estimate(void* pmh, int which, const mcrt_ray* rays, const uint32_t* pixel, const uint32_t* sample, size_t n,
+                              uint32_t seed, const double* radius, double* out, double* position, uint8_t* estimated)
+{
+    const PhotonMaps& pm = *static_cast<PhotonMaps*>(pmh);
+    const Scene& s = *pm.s;
+    Sampler smp(seed);
+    PMCounts cnt;
+    for (size_t i = 0; i < n; i++)
+    {
+        smp.initiate(pixel[i]); smp.setIndex(sample[i]);
+        const Ray ray = makeRay(D3(rays[i].origin), D3(rays[i].direction), s.d.scene_ior);
+        smp.shuffle();
+        const Isect is = intersect(s, ray, nullptr);
+        D3 e, pos(std::nan(""), std::nan(""), std::nan(""));
+        estimated[i] = 0;
+        if (is.prim != 0xFFFFFFFFu)
+        {
+            const Interaction ia = makeInteraction(s, is, ray, ray.medium_ior, smp);
+            pos = ia.position;
+            if (!ia.dirac_delta)
+            {
+                e = photonEstimate(pm, which, ia, radius[i] * radius[i], cnt);
+                estimated[i] = 1;
+            }
+        }
+        const double v[6] = { e.x, e.y, e.z, pos.x, pos.y, pos.z };
+        std::memcpy(out + 3 * i, v, 24); std::memcpy(position + 3 * i, v + 3, 24);
+    }
+}
+
 namespace
 {
     void storeSample(const D3& r, const D3 comp[4], size_t i, double* rgb, double* comp_out)
@@ -1745,7 +1860,32 @@ namespace
     }
     void storeCounts(const PMCounts& c, uint64_t* counts)
     {
-        if (counts) { counts[0] = c.rays; counts[1] = c.shadow_rays; counts[2] = c.queries; counts[3] = c.ties; }
+        if (counts)
+        {
+            counts[0] = c.rays; counts[1] = c.shadow_rays; counts[2] = c.queries; counts[3] = c.ties; counts[4] = c.empty;
+            counts[5] = c.photons;
+        }
+    }
+
+    // body(first, last, smp, counts) over [0, n) in contiguous chunks on up to hardware_concurrency threads, each with its own
+    // sampler; -> the chunks' counts added up. Every sample sets its sampler's state from (pixel, sample), and the maps and
+    // the scene are only read, so the results do not depend on the split.
+    PMCounts parallelSamples(size_t n, uint32_t seed, const std::function<void(size_t, size_t, Sampler&, PMCounts&)>& body)
+    {
+        const size_t t_max = std::max(1u, std::thread::hardware_concurrency());
+        const size_t T = std::max<size_t>(1, std::min<size_t>(t_max, n / 64));
+        std::vector<PMCounts> cnt(T);
+        std::vector<std::thread> threads;
+        for (size_t t = 0; t < T; t++)
+            threads.emplace_back([&, t] { Sampler smp(seed); body(n * t / T, n * (t + 1) / T, smp, cnt[t]); });
+        for (std::thread& th : threads) th.join();
+        PMCounts total;
+        for (const PMCounts& c : cnt)
+        {
+            total.rays += c.rays; total.shadow_rays += c.shadow_rays; total.queries += c.queries; total.ties += c.ties;
+            total.empty += c.empty; total.photons += c.photons;
+        }
+        return total;
     }
 }
 
@@ -1754,16 +1894,16 @@ void oracle_pm_sample_rays(void* pmh, const mcrt_ray* rays, const uint32_t* pixe
                            double* rgb, double* comp, uint64_t* counts)
 {
     const PhotonMaps& pm = *static_cast<PhotonMaps*>(pmh);
-    Sampler smp(seed);
-    PMCounts cnt;
-    for (size_t i = 0; i < n; i++)
+    storeCounts(parallelSamples(n, seed, [&](size_t first, size_t last, Sampler& smp, PMCounts& cnt)
     {
-        smp.initiate(pixel[i]); smp.setIndex(sample[i]);
-        D3 c[4];
-        const D3 r = pmSampleRay(pm, makeRay(D3(rays[i].origin), D3(rays[i].direction), pm.s->d.scene_ior), smp, c, cnt);
-        storeSample(r, c, i, rgb, comp);
-    }
-    storeCounts(cnt, counts);
+        for (size_t i = first; i < last; i++)
+        {
+            smp.initiate(pixel[i]); smp.setIndex(sample[i]);
+            D3 c[4];
+            const D3 r = pmSampleRay(pm, makeRay(D3(rays[i].origin), D3(rays[i].direction), pm.s->d.scene_ior), smp, c, cnt);
+            storeSample(r, c, i, rgb, comp);
+        }
+    }), counts);
 }
 
 // the brute-force k-NN search on caller points: out_d2 / out_index [n][k] nearest first (unused slots: +inf / 0xFFFFFFFF),
@@ -1791,22 +1931,22 @@ void oracle_pm_sample_pixels(void* pmh, const mcrt_camera* cam, const uint32_t* 
                              double* rgb, double* comp, double* rays6, uint64_t* counts)
 {
     const PhotonMaps& pm = *static_cast<PhotonMaps*>(pmh);
-    Sampler smp(seed);
-    PMCounts cnt;
-    for (size_t i = 0; i < n; i++)
+    storeCounts(parallelSamples(n, seed, [&](size_t first, size_t last, Sampler& smp, PMCounts& cnt)
     {
-        smp.initiate(pixel[i]); smp.setIndex(sample[i]);
-        const Ray ray = cameraRay(*cam, pm.s->d.scene_ior, pixel[i], smp);
-        if (rays6)
+        for (size_t i = first; i < last; i++)
         {
-            const double v[6] = { ray.start.x, ray.start.y, ray.start.z, ray.direction.x, ray.direction.y, ray.direction.z };
-            std::memcpy(rays6 + 6 * i, v, sizeof(v));
+            smp.initiate(pixel[i]); smp.setIndex(sample[i]);
+            const Ray ray = cameraRay(*cam, pm.s->d.scene_ior, pixel[i], smp);
+            if (rays6)
+            {
+                const double v[6] = { ray.start.x, ray.start.y, ray.start.z, ray.direction.x, ray.direction.y, ray.direction.z };
+                std::memcpy(rays6 + 6 * i, v, sizeof(v));
+            }
+            D3 c[4];
+            const D3 r = pmSampleRay(pm, ray, smp, c, cnt);
+            storeSample(r, c, i, rgb, comp);
         }
-        D3 c[4];
-        const D3 r = pmSampleRay(pm, ray, smp, c, cnt);
-        storeSample(r, c, i, rgb, comp);
-    }
-    storeCounts(cnt, counts);
+    }), counts);
 }
 
 // rows [y0, y1) with the default box film, as oracle_render_rows; comp (may be null): [4][y1 - y0][width][3], each term's
@@ -1815,14 +1955,13 @@ void oracle_pm_render_rows(void* pmh, const mcrt_camera* cam, uint32_t y0, uint3
                            double* comp, uint64_t* counts)
 {
     const PhotonMaps& pm = *static_cast<PhotonMaps*>(pmh);
-    Sampler smp(seed);
-    PMCounts cnt;
     const uint32_t spp = sqrtspp * sqrtspp;
     const size_t plane = (size_t)(y1 - y0) * cam->width * 3;
-    for (uint32_t y = y0; y < y1; y++)
-        for (uint32_t x = 0; x < cam->width; x++)
+    storeCounts(parallelSamples((size_t)(y1 - y0) * cam->width, seed, [&](size_t first, size_t last, Sampler& smp, PMCounts& cnt)
+    {
+        for (size_t p = first; p < last; p++)
         {
-            const uint32_t pixel = y * cam->width + x;
+            const uint32_t pixel = y0 * cam->width + (uint32_t)p;
             smp.initiate(pixel);
             D3 sum, csum[4];
             for (uint32_t i = 0; i < spp; i++)
@@ -1833,7 +1972,7 @@ void oracle_pm_render_rows(void* pmh, const mcrt_camera* cam, uint32_t y0, uint3
                 sum = sum + r * 1.0; // Film::Splat::update, weight 1
                 for (int k = 0; k < 4; k++) csum[k] = csum[k] + c[k];
             }
-            const size_t at = ((size_t)(y - y0) * cam->width + x) * 3;
+            const size_t at = p * 3;
             const D3 v = sum / (double)spp;
             out[at] = v.x < 0.0 ? 0.0 : v.x; out[at + 1] = v.y < 0.0 ? 0.0 : v.y; out[at + 2] = v.z < 0.0 ? 0.0 : v.z;
             if (comp)
@@ -1843,7 +1982,7 @@ void oracle_pm_render_rows(void* pmh, const mcrt_camera* cam, uint32_t y0, uint3
                     comp[k * plane + at] = m.x; comp[k * plane + at + 1] = m.y; comp[k * plane + at + 2] = m.z;
                 }
         }
-    storeCounts(cnt, counts);
+    }), counts);
 }
 
 // Image::save without the file (image.cpp:37-88, histogram.cpp, pixel-operators.cpp, srgb.hpp:54-62)

@@ -39,12 +39,18 @@ def lib():
         L.oracle_octree_free.argtypes = [C.c_void_p]
         L.oracle_image_tonemap.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_double)]
         L.oracle_render_film.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]
-        L.oracle_photon_pass.argtypes = [C.c_void_p, C.c_uint64, C.c_double, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(C.c_void_p),
-                                         C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)]
+        L.oracle_photon_pass.restype = C.c_int
+        L.oracle_photon_pass.argtypes = [C.c_void_p, C.c_uint64, C.c_double, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint32,
+                                         C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)]
         L.oracle_photon_pass_free.argtypes = [C.c_void_p]
         L.oracle_pm_create.restype = C.c_void_p
         L.oracle_pm_create.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32]
         L.oracle_pm_destroy.argtypes = [C.c_void_p]
+        L.oracle_pm_gather_radius.restype = C.c_int
+        L.oracle_pm_gather_radius.argtypes = [C.c_void_p, C.c_double, C.c_double]
+        L.oracle_pm_gather.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.oracle_pm_first_estimate.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32, C.c_void_p,
+                                               C.c_void_p, C.c_void_p, C.c_void_p]
         L.oracle_pm_sample_rays.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32, C.c_void_p, C.c_void_p,
                                             C.c_void_p]
         L.oracle_pm_sample_pixels.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32, C.c_void_p, C.c_void_p,
@@ -190,17 +196,23 @@ class PortScene:
         return out, rays.value
 
     # ---------------------------------------------------------------------------------------- photon mapper
-    def photon_pass(self, emissions, caustic_factor, max_photons_per_octree_leaf, scene_bounds, seed):
+    def photon_pass(self, emissions, caustic_factor, max_photons_per_octree_leaf, scene_bounds, seed, pass_index=0):
         """PhotonMapper::PhotonMapper's photon pass restated -> (caustic map, global map, (caustic lights, global lights),
         total emissions, (caustic paths, global paths)). Maps are dicts as the product's _map_arrays returns; lights: the
-        emitting light of each photon; paths: light << 32 | the light's emission index, the path that stored each photon."""
+        emitting light of each photon; paths: light << 32 | the light's emission index, the path that stored each photon.
+        pass_index: pass i of progressive photon mapping (PhotonMapper.emit_pass), light l's emissions at the indices
+        [i * n_l, (i + 1) * n_l); raises ValueError, as the product refuses it, when they do not fit 32 bits."""
+        if not 0 <= int(pass_index) < 1 << 32:
+            raise ValueError(f"pass index {pass_index} is outside [0, 2^32)")
         bounds = np.ascontiguousarray(scene_bounds, dtype=np.float64).reshape(6)
         h = C.c_void_p()
         d = [self.pkg.PhotonMapDesc(), self.pkg.PhotonMapDesc()]
         path_ptrs = (C.c_void_p * 2)()
         total = C.c_uint64()
-        lib().oracle_photon_pass(self.h, int(emissions), float(caustic_factor), int(max_photons_per_octree_leaf), _p(bounds), int(seed),
-                                 C.byref(h), C.addressof(d[0]), C.addressof(d[1]), C.cast(path_ptrs, C.POINTER(C.c_void_p)), C.byref(total))
+        if lib().oracle_photon_pass(self.h, int(emissions), float(caustic_factor), int(max_photons_per_octree_leaf), _p(bounds),
+                                    int(pass_index), int(seed), C.byref(h), C.addressof(d[0]), C.addressof(d[1]),
+                                    C.cast(path_ptrs, C.POINTER(C.c_void_p)), C.byref(total)):
+            raise ValueError(f"photon pass {pass_index}: the pass's emission indices do not fit 32 bits")
         try:
             maps = [self.pkg._map_arrays(m) for m in d]
             paths = tuple(np.ctypeslib.as_array(C.cast(path_ptrs[w], C.POINTER(C.c_uint64)), shape=(int(d[w].n_photons),)).copy()
@@ -218,9 +230,10 @@ class PortScene:
 class PortPhotonMapper:
     """The restatement's PhotonMapper::sampleRay over given maps. Every call returns (rgb, components, counts): components
     [..., 4, 3] in the order of the product's PHOTON_COMPONENT_NAMES (emission, direct, caustic, global), counts a dict of
-    rays (every Scene::intersect call), shadow_rays, knn_queries and knn_ties (queries whose k-th distance is shared by a
+    rays (every Scene::intersect call), shadow_rays, knn_queries, knn_ties (queries whose k-th distance is shared by a
     photon left out: the reference's choice between them follows its octree walk, which the brute-force search does not
-    restate)."""
+    restate), empty_queries (queries that took no photon) and photons (photons taken by all queries).
+    gather_radius switches the estimates to progressive photon mapping's fixed-radius gather, as the product's."""
 
     def __init__(self, ps, maps):
         caustic, glob, k, dv = maps
@@ -247,7 +260,37 @@ class PortPhotonMapper:
 
     @staticmethod
     def _counts(c):
-        return dict(rays=int(c[0]), shadow_rays=int(c[1]), knn_queries=int(c[2]), knn_ties=int(c[3]))
+        return dict(rays=int(c[0]), shadow_rays=int(c[1]), knn_queries=int(c[2]), knn_ties=int(c[3]), empty_queries=int(c[4]),
+                    photons=int(c[5]))
+
+    def gather_radius(self, r_caustic, r_global):
+        """Following estimates take every photon within r_caustic / r_global of a query, normalised by r^2 (k_gather);
+        (0, 0) returns to the k-NN estimate. Raises ValueError for the radii PhotonMapper.gather_radius refuses."""
+        if lib().oracle_pm_gather_radius(self.h, float(r_caustic), float(r_global)):
+            raise ValueError(f"gather radii ({r_caustic}, {r_global}): (0, 0) or two positive finite numbers")
+        self.gather_radii = (float(r_caustic), float(r_global))
+
+    def gather(self, which, points, radius):
+        """brute-force fixed-radius search of map `which` -> (count uint32 [n], flux_sum [n, 3], cone_sum [n, 3]), as
+        PhotonMapper.gather"""
+        points = np.ascontiguousarray(points, dtype=np.float64).reshape(-1, 3)
+        n = len(points)
+        cnt = np.zeros(n, np.uint32); flux = np.zeros((n, 3)); cone = np.zeros((n, 3))
+        lib().oracle_pm_gather(self.h, int(which), _p(points), n, float(radius), _p(cnt), _p(flux), _p(cone))
+        return cnt, flux, cone
+
+    def first_estimate(self, which, rays, pixel, sample, seed, radius):
+        """The estimate of map `which` that sampleRay makes at the first vertex of each camera sample, gathered within
+        radius[i] (0: the k nearest photons) -> (estimate [n, 3], vertex position [n, 3] (NaN: no hit), bool [n]: the
+        vertex is not a delta one, so the estimate ran)"""
+        rays = np.ascontiguousarray(rays, dtype=np.float64).reshape(-1, 6)
+        pixel = np.ascontiguousarray(pixel, dtype=np.uint32); sample = np.ascontiguousarray(sample, dtype=np.uint32)
+        radius = np.ascontiguousarray(np.broadcast_to(np.asarray(radius, np.float64), (len(rays),)))
+        n = len(rays)
+        out = np.zeros((n, 3)); pos = np.zeros((n, 3)); ran = np.zeros(n, np.uint8)
+        lib().oracle_pm_first_estimate(self.h, int(which), _p(rays), _p(pixel), _p(sample), n, int(seed), _p(radius), _p(out), _p(pos),
+                                       _p(ran))
+        return out, pos, ran.astype(bool)
 
     def knn(self, which, points):
         """brute-force k nearest photons of map `which` -> (index [n, k], distance2 [n, k] nearest first, count [n], ties)"""
@@ -260,7 +303,7 @@ class PortPhotonMapper:
     def sample_rays(self, rays, pixel, sample, seed):
         rays = np.ascontiguousarray(rays, dtype=np.float64).reshape(-1, 6)
         pixel = np.ascontiguousarray(pixel, dtype=np.uint32); sample = np.ascontiguousarray(sample, dtype=np.uint32)
-        rgb = np.zeros((len(rays), 3)); comp = np.zeros((len(rays), 4, 3)); c = np.zeros(4, np.uint64)
+        rgb = np.zeros((len(rays), 3)); comp = np.zeros((len(rays), 4, 3)); c = np.zeros(6, np.uint64)
         lib().oracle_pm_sample_rays(self.h, _p(rays), _p(pixel), _p(sample), len(rays), seed, _p(rgb), _p(comp), _p(c))
         return rgb, comp, self._counts(c)
 
@@ -268,12 +311,12 @@ class PortPhotonMapper:
         """-> (rgb [n, 3], components [n, 4, 3], camera rays [n, 6], counts)"""
         pixel = np.ascontiguousarray(pixel, dtype=np.uint32); sample = np.ascontiguousarray(sample, dtype=np.uint32)
         n = len(pixel)
-        rgb = np.zeros((n, 3)); comp = np.zeros((n, 4, 3)); rays = np.zeros((n, 6)); c = np.zeros(4, np.uint64)
+        rgb = np.zeros((n, 3)); comp = np.zeros((n, 4, 3)); rays = np.zeros((n, 6)); c = np.zeros(6, np.uint64)
         lib().oracle_pm_sample_pixels(self.h, C.addressof(camera.rec), _p(pixel), _p(sample), n, seed, _p(rgb), _p(comp), _p(rays), _p(c))
         return rgb, comp, rays, self._counts(c)
 
     def render_rows(self, camera, y0, y1, sqrtspp, seed):
         """-> (frame [rows, width, 3], component frames [4, rows, width, 3] (per-pixel means), counts)"""
-        out = np.zeros((y1 - y0, camera.width, 3)); comp = np.zeros((4, y1 - y0, camera.width, 3)); c = np.zeros(4, np.uint64)
+        out = np.zeros((y1 - y0, camera.width, 3)); comp = np.zeros((4, y1 - y0, camera.width, 3)); c = np.zeros(6, np.uint64)
         lib().oracle_pm_render_rows(self.h, C.addressof(camera.rec), y0, y1, sqrtspp, seed, _p(out), _p(comp), _p(c))
         return out, comp, self._counts(c)
