@@ -543,6 +543,51 @@ int mcrt_render_accumulate_photon_components_dev(mcrt_ctx* ctx, const mcrt_camer
                                                  int integrator_kind, int precision, double* planes_dev, uint32_t n_planes,
                                                  mcrt_stats* stats);
 
+/* Light path expressions (LPEs): film planes chosen by regular expressions over each path-tracer contribution's event
+ * string. The string is C (the camera), then the event of each scattering vertex before the contribution, then its
+ * source: L for an emitter (hit, or sampled by next-event estimation at the last vertex), L'g' for an emitter whose
+ * light is in group g of the mcrt_set_light_groups table, B for the sky. Vertex events are <RD> (diffuse), <RS> / <RG>
+ * (reflection, smooth / rough: GGX and rough dielectrics), <TS> / <TG> (refraction, smooth / rough).
+ * Syntax (a subset of OSL's, anchored to the whole string, whitespace ignored): the events above, <XY> with X in {R,T,.}
+ * and Y in {D,G,S,.}, the shorthands D = <.D>, G = <.G>, S = <.S>, R = <R.>, T = <T.>, '.' for any one event, sets
+ * [...] and [^...] of events, ( ), |, and the repetitions * + ? {n} {n,} {n,m} (n, m <= 1000). '.' matches L and B
+ * too: the indirect diffuse light is C<RD>.+[LB], while C<RD>.+ also takes the direct C<RD>L and C<RD>B.
+ * The compiled union is a DFA: state 0 follows C, a state from which no expression can match any more is
+ * MCRT_LPE_DEAD, and every state carries a 32-bit accept mask, bit i for expression i. Symbols are the MCRT_LPE_SYM_*
+ * events, then one per distinct label (ascending group index); the lights of every unlabelled group read
+ * MCRT_LPE_SYM_L, which L matches together with every label. */
+enum {
+    MCRT_LPE_SYM_RD = 0, MCRT_LPE_SYM_RS = 1, MCRT_LPE_SYM_RG = 2, MCRT_LPE_SYM_TS = 3, MCRT_LPE_SYM_TG = 4,
+    MCRT_LPE_SYM_B = 5, MCRT_LPE_SYM_L = 6, MCRT_LPE_SYM_LABEL0 = 7,
+    MCRT_LPE_MAX_EXPRESSIONS = 32, MCRT_LPE_MAX_LABELS = 64, MCRT_LPE_MAX_STATES = 255, MCRT_LPE_DEAD = 255,
+    MCRT_LPE_MAX_SYMBOLS = MCRT_LPE_SYM_LABEL0 + MCRT_LPE_MAX_LABELS
+};
+/* Compiles exprs[n] and uploads the tables; exprs NULL with n = 0 clears them. Labels need the light-group table
+ * (mcrt_set_light_groups) and a group index below its n_groups; mcrt_set_light_groups and mcrt_scene_upload clear the
+ * LPE table. MCRT_ERR_NO_SCENE before an upload. MCRT_ERR_INVALID: a syntax error (the message names the expression and
+ * the character offset), n > MCRT_LPE_MAX_EXPRESSIONS, more than MCRT_LPE_MAX_LABELS distinct labels, an unknown label.
+ * MCRT_ERR_UNSUPPORTED: more than MCRT_LPE_MAX_STATES live states. A refused call leaves no table. */
+int mcrt_set_light_path_expressions(mcrt_ctx* ctx, const char* const* exprs, uint32_t n);
+/* mcrt_render_accumulate_dev (active_tiles NULL) or mcrt_render_accumulate_tiles_dev (active_tiles HOST, same mask
+ * layout) into planes_dev[n][n_rows*W][3], plane i the sums of the contributions whose event string expression i
+ * matches (path tracer, box film; the box film's weight is the sample count). Planes may overlap, or leave a
+ * contribution out; a path ends at the vertex where its state becomes MCRT_LPE_DEAD, and next-event estimation that no
+ * expression accepts traces no shadow ray, so every plane keeps its value while fewer rays are traced.
+ * MCRT_ERR_INVALID: no LPE table, n_planes other than its expression count, a null planes_dev, and every argument the
+ * one-plane entry points refuse. MCRT_ERR_UNSUPPORTED: a reconstruction filter, the photon mapper. Nothing is written
+ * when a call is refused. The other entry points ignore the table. */
+int mcrt_render_accumulate_lpe_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_t y_first, uint32_t y_step, uint32_t n_rows,
+                                   uint32_t tile, const uint8_t* active_tiles, uint32_t sample_first, uint32_t sample_count,
+                                   uint32_t global_seed, int integrator_kind, int precision, double* planes_dev,
+                                   uint32_t n_planes, mcrt_stats* stats);
+/* Test hook (host only, no CUDA call): the tables mcrt_set_light_path_expressions would upload, with labels below
+ * n_groups. next[MCRT_LPE_MAX_STATES * MCRT_LPE_MAX_SYMBOLS] receives [*n_states][*n_symbols], accept[256] the accept
+ * masks (accept[MCRT_LPE_DEAD] = 0), group_symbol[n_groups] (NULL when n_groups is 0) the symbol of each group's
+ * lights. error[error_capacity] receives the reason of a refusal (or ""). Returns what mcrt_set_light_path_expressions
+ * would. */
+int mcrt_lpe_compile_host(const char* const* exprs, uint32_t n, uint32_t n_groups, uint8_t* next, uint32_t* accept,
+                          uint8_t* group_symbol, uint32_t* n_states, uint32_t* n_symbols, char* error, uint32_t error_capacity);
+
 /* Denoising a progressive frame (mcrt_denoise_dev) needs per-pixel guides: the first hits of the camera rays of samples
  * [sample_first, sample_first + sample_count) of every pixel of the whole width x height frame add
  * {albedo.rgb, shading normal.xyz, t, 1} per hit into features_dev [height*width][8] (device, float64); a miss adds

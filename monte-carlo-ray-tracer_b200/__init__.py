@@ -42,6 +42,7 @@ ABI_SYMBOLS = [
     "mcrt_photon_emit_pass", "mcrt_photon_gather_radius", "mcrt_photon_gather_search",
     "mcrt_set_light_groups", "mcrt_render_accumulate_groups_dev", "mcrt_light_groups_combine_dev",
     "mcrt_render_accumulate_aovs_dev", "mcrt_photon_download_lights", "mcrt_render_accumulate_photon_components_dev",
+    "mcrt_set_light_path_expressions", "mcrt_render_accumulate_lpe_dev", "mcrt_lpe_compile_host",
 ]
 
 # The light-path AOV planes of mcrt_render_accumulate_aovs_dev, in plane order (MCRT_AOV_* of include/mcrt_abi.h):
@@ -52,6 +53,13 @@ AOV_NAMES = ("background", "emission", "diffuse_direct", "diffuse_indirect", "re
 # The photon mapper's component planes of mcrt_render_accumulate_photon_components_dev, in plane order (MCRT_PM_* of
 # include/mcrt_abi.h): emitters seen from the camera, Monte Carlo direct light, the caustic-map and global-map estimates
 PHOTON_COMPONENT_NAMES = ("emission", "direct", "caustic", "global")
+
+# Light path expressions (mcrt_set_light_path_expressions): the event symbols of the compiled table (MCRT_LPE_SYM_* of
+# include/mcrt_abi.h); label k of a table is symbol LPE_SYM_LABEL0 + k
+LPE_SYM_RD, LPE_SYM_RS, LPE_SYM_RG, LPE_SYM_TS, LPE_SYM_TG, LPE_SYM_B, LPE_SYM_L, LPE_SYM_LABEL0 = range(8)
+LPE_DEAD, LPE_MAX_STATES, LPE_MAX_SYMBOLS, LPE_MAX_EXPRESSIONS = 255, 255, 71, 32
+# The light-path AOV planes of AOV_NAMES as light path expressions, in the same order
+AOV_LPES = ("CB", "CL", "C<RD>[LB]", "C<RD>.+[LB]", "C[<RS><RG>][LB]", "C[<RS><RG>].+[LB]", "C<T.>[LB]", "C<T.>.+[LB]")
 
 
 class McrtError(RuntimeError):
@@ -255,6 +263,10 @@ def lib():
                                                         C.c_uint32, C.POINTER(Stats)]
         L.mcrt_render_accumulate_aovs_dev.argtypes = L.mcrt_render_accumulate_groups_dev.argtypes
         L.mcrt_render_accumulate_photon_components_dev.argtypes = L.mcrt_render_accumulate_groups_dev.argtypes
+        L.mcrt_set_light_path_expressions.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
+        L.mcrt_render_accumulate_lpe_dev.argtypes = L.mcrt_render_accumulate_groups_dev.argtypes
+        L.mcrt_lpe_compile_host.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.c_char_p, C.c_uint32]
         L.mcrt_light_groups_combine_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint64, C.c_void_p, C.c_void_p]
         L.mcrt_render_features_dev.argtypes = [C.c_void_p, C.POINTER(CameraRec), C.c_uint32, C.c_uint32, C.c_uint32, C.c_int,
                                                C.c_void_p, C.POINTER(Stats)]
@@ -702,6 +714,22 @@ class Integrator:
         return self._render_accumulate_planes(lib().mcrt_render_accumulate_aovs_dev, camera, planes_ptr, len(AOV_NAMES), sample_first,
                                               sample_count, tile, active, y_first, y_step, n_rows, precision)
 
+    # -- light path expressions (see Progressive's lpes)
+    def set_light_path_expressions(self, exprs):
+        """mcrt_set_light_path_expressions: the renders of render_accumulate_lpe_dev then have one plane per expression,
+        plane i the contributions whose event string exprs[i] matches. Labels L'g' name groups of the light-group table,
+        so set_light_groups comes first (it clears this table). exprs None or empty clears the table."""
+        exprs = list(exprs or ())
+        arr = _lpe_strings(exprs)
+        self._check(lib().mcrt_set_light_path_expressions(self.ctx, C.cast(arr, C.c_void_p) if exprs else None, len(exprs)))
+
+    def render_accumulate_lpe_dev(self, camera, planes_ptr, n_planes, sample_first, sample_count, tile=0, active=None,
+                                  y_first=0, y_step=1, n_rows=None, precision=None):
+        """mcrt_render_accumulate_lpe_dev: render_accumulate_dev (active None) or render_accumulate_tiles_dev into the
+        LPE planes planes_ptr [n_planes, n_rows, width, 3] (device), one per expression of set_light_path_expressions."""
+        return self._render_accumulate_planes(lib().mcrt_render_accumulate_lpe_dev, camera, planes_ptr, n_planes, sample_first,
+                                              sample_count, tile, active, y_first, y_step, n_rows, precision)
+
     def _render_accumulate_planes(self, fn, camera, planes_ptr, n_planes, sample_first, sample_count, tile, active, y_first,
                                   y_step, n_rows, precision):
         self.set_film(camera)
@@ -1144,6 +1172,36 @@ def bvh4_host(scene, max_leaf=0xFFFFFFFF):
         lib().mcrt_bvh4_host_free(h)
 
 
+def _lpe_strings(exprs):
+    arr = (C.c_char_p * max(len(exprs), 1))()
+    for i, e in enumerate(exprs):
+        arr[i] = str(e).encode()
+    return arr
+
+
+def lpe_compile(exprs, n_groups=0):
+    """The tables mcrt_set_light_path_expressions compiles from exprs (host only, mcrt_lpe_compile_host), with labels
+    below n_groups -> {"next": uint8 [n_states, n_symbols] (LPE_DEAD: no expression can match any more), "accept": uint32
+    [256] (bit i: expression i matches), "group_symbol": uint8 [n_groups] (the symbol of each group's lights)}. State 0
+    follows the camera event C. Raises McrtError with the compiler's reason (and .code, the MCRT_ERR_* value)."""
+    exprs = list(exprs)
+    arr = _lpe_strings(exprs)
+    nxt = np.zeros(LPE_MAX_STATES * LPE_MAX_SYMBOLS, np.uint8)
+    acc = np.zeros(256, np.uint32)
+    gs = np.zeros(max(int(n_groups), 1), np.uint8)
+    ns, nsym = C.c_uint32(), C.c_uint32()
+    err = C.create_string_buffer(1024)
+    rc = lib().mcrt_lpe_compile_host(C.cast(arr, C.c_void_p) if exprs else None, len(exprs), int(n_groups),
+                                     nxt.ctypes.data_as(C.c_void_p), acc.ctypes.data_as(C.c_void_p),
+                                     gs.ctypes.data_as(C.c_void_p), C.byref(ns), C.byref(nsym), err, len(err))
+    if rc:
+        e = McrtError(f"mcrt_lpe_compile_host failed with {rc}: {err.value.decode()}")
+        e.code = rc
+        raise e
+    return {"next": nxt[:ns.value * nsym.value].reshape(ns.value, nsym.value).copy(), "accept": acc,
+            "group_symbol": gs[:int(n_groups)].copy()}
+
+
 def light_groups_by_emittance(scene, rtol=1e-12):
     """Groups the scene's lights by emittance: a light joins the first group whose first light's emittance equals its
     own in every channel to within rtol (relative; the default only absorbs the last-bit differences a mesh light's
@@ -1254,13 +1312,26 @@ class Progressive:
     mcrt_render_accumulate_photon_components_dev - emitters seen from the camera, direct light, the caustic-map and the
     global-map estimates. Everything works on the planes' sum as with AOVs; component_frames() resolves each plane with
     its own noise estimate, which shows which estimator still dominates the error, and relight(weights) /
-    denoise(weights=...) recomposite the frame, e.g. relight([1, 1, 0, 1]) removes the caustics."""
+    denoise(weights=...) recomposite the frame, e.g. relight([1, 1, 0, 1]) removes the caustics.
+
+    Light path expressions (lpes = a list of expressions, see mcrt_set_light_path_expressions; box film, path tracer,
+    not together with AOVs or components): A and B hold one plane per expression and, last, the beauty plane "C.*",
+    [len(lpes) + 1, rows, width, 3], filled by mcrt_render_accumulate_lpe_dev. Expressions may overlap or leave
+    contributions out, so frame, error, render, render_adaptive and denoise work on the beauty plane alone and behave
+    as without expressions. At most 31 expressions, since the beauty plane takes the table's 32nd. light_groups here only
+    supplies the groups that labels L'g' name; without it labels are refused. lpe_frames() resolves each
+    expression's plane with its own noise estimate; relight(weights) and denoise(weights=...) take one weight per
+    expression (the beauty plane's weight is 0)."""
 
     _STATS = ("paths", "extension_rays", "shadow_rays")
 
     def __init__(self, integrator, camera, y_first=0, y_step=1, n_rows=None, tile=16, light_groups=None, aovs=False,
-                 components=False):
+                 components=False, lpes=None):
         import torch
+        if lpes is not None and integrator.kind == INTEGRATOR_PHOTON:
+            raise McrtError("the photon mapper has no light path expressions")
+        if lpes is not None and (aovs or components):
+            raise McrtError("light path expressions together with AOVs or components in one render are not supported")
         if components and integrator.kind != INTEGRATOR_PHOTON:
             raise McrtError("photon-mapper components need a PhotonMapper (the path tracer has light-path AOVs)")
         if components and (light_groups is not None or aovs):
@@ -1280,6 +1351,21 @@ class Progressive:
         self.filtered = rec is not None and not (rec.filter == FILM_FILTERS["box"] and rec.radius in (0.0, 0.5))
         self.rows = camera.height if self.filtered else self.n_rows   # rows of the sums and of the resolved frame
         self.light_groups, self.n_planes = None, 1
+        self.lpes, self.lpe_groups = None, None
+        if lpes is not None:
+            if self.filtered:
+                raise McrtError("light path expressions take the box film only")
+            self.lpes = [str(e) for e in lpes]
+            if not self.lpes:
+                raise McrtError("lpes: at least one expression")
+            if len(self.lpes) > LPE_MAX_EXPRESSIONS - 1:
+                raise McrtError(f"lpes: {len(self.lpes)} expressions, at most {LPE_MAX_EXPRESSIONS - 1}: the table holds "
+                                f"{LPE_MAX_EXPRESSIONS}, and Progressive adds the beauty plane \"C.*\"")
+            if light_groups is not None:
+                self.lpe_groups = np.ascontiguousarray(light_groups, dtype=np.uint32).reshape(-1)
+            self.n_planes = len(self.lpes) + 1
+            self._set_lpe_tables()   # refuses a wrong expression or table before anything is allocated
+            light_groups = None
         if light_groups is not None:
             if self.filtered:
                 raise McrtError("light groups take the box film only")
@@ -1296,7 +1382,7 @@ class Progressive:
             if self.filtered:
                 raise McrtError("photon-mapper components take the box film only")
             self.n_planes = len(PHOTON_COMPONENT_NAMES)
-        planes = (self.n_planes,) if self._planar else ()
+        planes = (self.n_planes,) if self._planar or self.lpes is not None else ()
         dev = torch.device("cuda", integrator.device)
         self.rgb = [torch.zeros(planes + (self.rows, camera.width, 3), dtype=torch.float64, device=dev) for _ in range(2)]
         self.wsum = [torch.zeros((self.rows, camera.width), dtype=torch.float64, device=dev) for _ in range(2)] if self.filtered else None
@@ -1321,6 +1407,16 @@ class Progressive:
         """A and B hold planes (light groups, AOVs or photon-mapper components) whose sum is the beauty frame's sums."""
         return self.light_groups is not None or self.aovs or self.components
 
+    def _set_lpe_tables(self):
+        # without light_groups the integrator's group table is cleared, so that labels L'g' are refused rather than
+        # resolved against whatever table it holds, which the checkpoint's identity would not record
+        if self.lpe_groups is not None:
+            n_groups = int(self.lpe_groups.max()) + 1 if self.lpe_groups.size else 0
+            self.integrator.set_light_groups(self.lpe_groups, n_groups)
+        else:
+            self.integrator.set_light_groups(None)
+        self.integrator.set_light_path_expressions(self.lpes + ["C.*"])
+
     def add(self, samples):
         """Renders samples [self.samples, self.samples + samples) of the active tiles into A (even pass) or B (odd pass)."""
         half = self.passes % 2
@@ -1330,6 +1426,11 @@ class Progressive:
             st = self.integrator.render_accumulate_groups_dev(self.camera, self.rgb[half].data_ptr(), self.n_planes, self.samples,
                                                               int(samples), self.tile, None if self.active.all() else self.active,
                                                               self.y_first, self.y_step, self.n_rows)
+        elif self.lpes is not None:
+            self._set_lpe_tables()   # the integrator may serve other renders
+            st = self.integrator.render_accumulate_lpe_dev(self.camera, self.rgb[half].data_ptr(), self.n_planes, self.samples,
+                                                           int(samples), self.tile, None if self.active.all() else self.active,
+                                                           self.y_first, self.y_step, self.n_rows)
         elif self.aovs:
             st = self.integrator.render_accumulate_aovs_dev(self.camera, self.rgb[half].data_ptr(), self.samples, int(samples), self.tile,
                                                             None if self.active.all() else self.active, self.y_first, self.y_step,
@@ -1363,9 +1464,14 @@ class Progressive:
         """The sums of halves A and B, [rows, width, 3] each: with planes (light groups, AOVs, components) the combination
         of the planes with weights [n_planes, 3] or [n_planes] (None: every weight 1, the beauty frame's sums)."""
         import torch
-        if not self._planar:
+        if self.lpes is not None:
+            if weights is None:
+                return [self.rgb[0][-1], self.rgb[1][-1]]   # the beauty plane
+            w = light_group_weights(weights, len(self.lpes))
+            weights = np.concatenate([w, np.zeros((1, 3))])   # the beauty plane's weight is 0
+        elif not self._planar:
             if weights is not None:
-                raise McrtError("weights need a render with light groups, AOVs or photon-mapper components")
+                raise McrtError("weights need a render with light groups, AOVs, photon-mapper components or light path expressions")
             return self.rgb
         w = np.ones(self.n_planes) if weights is None else weights
         out = []
@@ -1423,9 +1529,18 @@ class Progressive:
             raise McrtError("component_frames needs a render with components=True")
         return self._plane_frames()
 
-    def _plane_frames(self):
-        """Every plane of A and B resolved on its own -> (frames [n_planes, rows, width, 3], relative errors [n_planes])."""
-        res = [self._resolve_halves([self.rgb[0][k], self.rgb[1][k]]) for k in range(self.n_planes)]
+    # -- light path expressions
+    def lpe_frames(self):
+        """Each expression's plane resolved on its own (in the order of lpes) -> (frames float64 [len(lpes), rows, width,
+        3], each plane's relative error float64 [len(lpes)], estimated from the difference of its two halves like
+        error()'s)."""
+        if self.lpes is None:
+            raise McrtError("lpe_frames needs a render with lpes")
+        return self._plane_frames(len(self.lpes))
+
+    def _plane_frames(self, n=None):
+        """The first n (all) planes of A and B resolved on their own -> (frames [n, rows, width, 3], relative errors [n])."""
+        res = [self._resolve_halves([self.rgb[0][k], self.rgb[1][k]]) for k in range(self.n_planes if n is None else n)]
         return np.stack([r[0] for r in res]), np.array([r[1] for r in res])
 
     def relight(self, weights):
@@ -1433,7 +1548,8 @@ class Progressive:
         -> (frame, frame relative error, per-tile relative errors). Light groups: the last row weights the sky, and
         weight w_g on group g equals a render of the scene with group g's emittance scaled by w_g. AOVs: the rows weight
         the planes of AOV_NAMES, e.g. 0 on the reflection planes removes what the first vertex reflected. Components: the
-        rows weight the planes of PHOTON_COMPONENT_NAMES, e.g. [1, 1, 0, 1] removes the caustics."""
+        rows weight the planes of PHOTON_COMPONENT_NAMES, e.g. [1, 1, 0, 1] removes the caustics. Light path
+        expressions: one row per expression; the beauty plane is left out."""
         frame, err, tiles, _ = self._resolve_halves(self._halves(weights))
         return frame, err, tiles
 
@@ -1588,6 +1704,9 @@ class Progressive:
             ident["aovs"] = np.int64(len(AOV_NAMES))
         if self.components:
             ident["photon_components"] = np.int64(len(PHOTON_COMPONENT_NAMES))
+        if self.lpes is not None:
+            ident["lpes"] = np.array(self.lpes)
+            ident["lpe_groups"] = self.lpe_groups.copy() if self.lpe_groups is not None else np.zeros(0, np.int64)
         return ident
 
     def _photon_identity(self):
@@ -1617,15 +1736,15 @@ class Progressive:
             np.savez(f, **data)
 
     @classmethod
-    def load(cls, path, integrator, camera, tile=None, light_groups=None, aovs=False, components=False):
+    def load(cls, path, integrator, camera, tile=None, light_groups=None, aovs=False, components=False, lpes=None):
         """Resumes a checkpoint written by save() with `integrator` and `camera` (and `tile`, the checkpoint's if None).
         Raises McrtError, and resumes nothing, when the seed, precision, integrator kind, camera, film, tile, scene,
-        photon maps, light groups, AOVs or components differ from the checkpoint's. A checkpoint without tile state
-        resumes with every tile active."""
+        photon maps, light groups, AOVs, components or light path expressions (with their groups) differ from the
+        checkpoint's. A checkpoint without tile state resumes with every tile active."""
         data = _read_checkpoint(path)
         y_first, y_step, n_rows = (int(v) for v in data["row_set"])
         p = cls(integrator, camera, y_first, y_step, n_rows, int(data["tile"]) if tile is None else int(tile), light_groups, aovs,
-                components)
+                components, **({"lpes": lpes} if lpes is not None else {}))
         p._restore(path, data)
         return p
 
@@ -1639,6 +1758,8 @@ class Progressive:
             raise McrtError(f"checkpoint {path}: light-path AOVs differ from this render's; not resuming")
         if ("photon_components" in data) != ("photon_components" in ident):
             raise McrtError(f"checkpoint {path}: photon-mapper components differ from this render's; not resuming")
+        if ("lpes" in data) != ("lpes" in ident):
+            raise McrtError(f"checkpoint {path}: light path expressions differ from this render's; not resuming")
         for k, want in ident.items():
             if k not in data or not np.array_equal(data[k], want):
                 raise McrtError(f"checkpoint {path}: {k} differs from this render's; not resuming")

@@ -22,6 +22,7 @@ UNITS = [
     ("image.cu", ["--fmad=false"]),
     ("obj_abi.cu", ["--fmad=false"]),
     ("denoise.cu", ["--fmad=false"]),
+    ("lpe.cu", []),
     ("abi.cu", []),
 ]
 

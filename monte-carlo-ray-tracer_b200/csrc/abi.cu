@@ -15,6 +15,7 @@
 #include "bvh_build.h"
 #include "image.h"
 #include "denoise.h"
+#include "lpe.h"
 
 using namespace mcrt;
 
@@ -104,6 +105,14 @@ struct mcrt_ctx
     size_t group_of_light_values = 0;
     double* d_group_weights = nullptr;      // [n_planes][3] of mcrt_light_groups_combine_dev (grow-only)
     size_t group_weight_values = 0;
+    std::vector<uint32_t> h_group_of_light; // host copy of the table, for the LPE light symbols
+    // light path expressions (mcrt_set_light_path_expressions); mcrt_scene_upload and mcrt_set_light_groups clear them
+    uint32_t lpe_n = 0;                     // expressions = planes of an LPE render; 0: no table
+    uint32_t lpe_symbols = 0;
+    uint8_t* d_lpe_next = nullptr;          // [MCRT_LPE_MAX_STATES][MCRT_LPE_MAX_SYMBOLS] at most, [states][lpe_symbols] used
+    uint32_t* d_lpe_accept = nullptr;       // [256]
+    uint8_t* d_lpe_light_symbol = nullptr;  // [n_lights] (grow-only)
+    size_t lpe_light_values = 0;
     cudaEvent_t ev_start = nullptr, ev_stop = nullptr, ev_poll[2] = { nullptr, nullptr };
 
     // photon maps (PhotonMapper::caustic_map / global_map) + k-NN query queues
@@ -686,6 +695,7 @@ namespace
         bool aovs = false;       // ... or planes each deposit site names: the MCRT_AOV_COUNT light-path planes of the
                                  // path tracer (mcrt_render_accumulate_aovs_dev), the MCRT_PM_COMPONENT_COUNT estimator planes
                                  // of the photon mapper (mcrt_render_accumulate_photon_components_dev)
+        bool lpe = false;        // ... or one plane per light path expression (mcrt_render_accumulate_lpe_dev)
     };
 
     // The wavefront loop shared by mcrt_render_rows(_dev) and mcrt_sample_rays. Camera work item w is sample
@@ -755,6 +765,13 @@ namespace
             p.plane_values = film_pixels * 3;
             p.n_planes = accum->n_planes;
             p.aovs = accum->aovs ? 1u : 0u;
+            if (accum->lpe)
+            {
+                p.lpe_next = ctx->d_lpe_next;
+                p.lpe_accept = ctx->d_lpe_accept;
+                p.lpe_light_symbol = ctx->d_lpe_light_symbol;
+                p.lpe_symbols = ctx->lpe_symbols;
+            }
         }
         p.filmp.is_default_box = filtered ? 0u : 1u;
         if (filtered)
@@ -1137,6 +1154,9 @@ void mcrt_destroy(mcrt_ctx* ctx)
     if (ctx->d_pixel_list) cudaFree(ctx->d_pixel_list);
     if (ctx->d_group_of_light) cudaFree(ctx->d_group_of_light);
     if (ctx->d_group_weights) cudaFree(ctx->d_group_weights);
+    if (ctx->d_lpe_next) cudaFree(ctx->d_lpe_next);
+    if (ctx->d_lpe_accept) cudaFree(ctx->d_lpe_accept);
+    if (ctx->d_lpe_light_symbol) cudaFree(ctx->d_lpe_light_symbol);
     if (ctx->d_counters) cudaFree(ctx->d_counters);
     if (ctx->d_sobol_bytes) cudaFree(ctx->d_sobol_bytes);
     if (ctx->h_counters) cudaFreeHost(ctx->h_counters);
@@ -1201,6 +1221,7 @@ int mcrt_scene_upload(mcrt_ctx* ctx, const mcrt_scene_desc* scene, uint64_t* h2d
     ctx->has_scene = false;
     ctx->has_light_groups = false;
     ctx->n_light_groups = 0;
+    ctx->lpe_n = 0;
     ctx->photon_lights = false;   // the maps' light indices name the lights of the previous scene
 
     // scene scale for the fast mode's ray offsets
@@ -1887,6 +1908,7 @@ int mcrt_set_light_groups(mcrt_ctx* ctx, const uint32_t* group_of_light, uint32_
         if (n_lights || n_groups) { ctx->error = "mcrt_set_light_groups: a null table clears it; n_lights and n_groups must be 0"; return MCRT_ERR_INVALID; }
         ctx->has_light_groups = false;
         ctx->n_light_groups = 0;
+        ctx->lpe_n = 0;   // its labels named groups of the old table
         return MCRT_OK;
     }
     if (n_lights != ctx->scene64.n_lights)
@@ -1909,6 +1931,7 @@ int mcrt_set_light_groups(mcrt_ctx* ctx, const uint32_t* group_of_light, uint32_
     }
     CK(cudaSetDevice(ctx->device));
     ctx->has_light_groups = false;
+    ctx->lpe_n = 0;   // its labels named groups of the old table
     if (ctx->group_of_light_values < n_lights)
     {
         if (ctx->d_group_of_light) cudaFree(ctx->d_group_of_light);
@@ -1918,9 +1941,82 @@ int mcrt_set_light_groups(mcrt_ctx* ctx, const uint32_t* group_of_light, uint32_
     }
     if (n_lights) CK(cudaMemcpyAsync(ctx->d_group_of_light, group_of_light, n_lights * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
+    ctx->h_group_of_light.assign(group_of_light, group_of_light + n_lights);
     ctx->n_light_groups = n_groups;
     ctx->has_light_groups = true;
     return MCRT_OK;
+}
+
+int mcrt_set_light_path_expressions(mcrt_ctx* ctx, const char* const* exprs, uint32_t n)
+{
+    if (!ctx) return MCRT_ERR_INVALID;
+    const std::string name = "mcrt_set_light_path_expressions";
+    if (!ctx->has_scene) { ctx->error = name + ": no scene uploaded"; return MCRT_ERR_NO_SCENE; }
+    ctx->lpe_n = 0;
+    if (!exprs)
+    {
+        if (n) { ctx->error = name + ": a null list clears the table; n must be 0"; return MCRT_ERR_INVALID; }
+        return MCRT_OK;
+    }
+    LpeTable t;
+    std::string why;
+    const int rc = lpeCompile(exprs, n, ctx->has_light_groups ? ctx->n_light_groups : 0u, t, why);
+    if (rc != MCRT_OK) { ctx->error = name + ": " + why; return rc; }
+    // light l reads the symbol of its group's label, or the unlabelled L
+    const uint32_t n_lights = ctx->scene64.n_lights;
+    std::vector<uint8_t> light_symbol(std::max<uint32_t>(n_lights, 1u), (uint8_t)MCRT_LPE_SYM_L);
+    if (ctx->has_light_groups)
+        for (uint32_t l = 0; l < n_lights; l++)
+        {
+            auto it = std::lower_bound(t.labels.begin(), t.labels.end(), ctx->h_group_of_light[l]);
+            if (it != t.labels.end() && *it == ctx->h_group_of_light[l])
+                light_symbol[l] = (uint8_t)(MCRT_LPE_SYM_LABEL0 + (it - t.labels.begin()));
+        }
+    CK(cudaSetDevice(ctx->device));
+    if (!ctx->d_lpe_next)
+    {
+        CK(cudaMalloc((void**)&ctx->d_lpe_next, (size_t)MCRT_LPE_MAX_STATES * MCRT_LPE_MAX_SYMBOLS));
+        CK(cudaMalloc((void**)&ctx->d_lpe_accept, 256 * sizeof(uint32_t)));
+    }
+    if (ctx->lpe_light_values < light_symbol.size())
+    {
+        if (ctx->d_lpe_light_symbol) cudaFree(ctx->d_lpe_light_symbol);
+        ctx->d_lpe_light_symbol = nullptr; ctx->lpe_light_values = 0;
+        CK(cudaMalloc((void**)&ctx->d_lpe_light_symbol, light_symbol.size()));
+        ctx->lpe_light_values = light_symbol.size();
+    }
+    CK(cudaMemcpyAsync(ctx->d_lpe_next, t.next.data(), t.next.size(), cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->d_lpe_accept, t.accept.data(), 256 * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->d_lpe_light_symbol, light_symbol.data(), light_symbol.size(), cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    ctx->lpe_symbols = t.n_symbols;
+    ctx->lpe_n = n;
+    return MCRT_OK;
+}
+
+int mcrt_render_accumulate_lpe_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_t y_first, uint32_t y_step, uint32_t n_rows,
+                                   uint32_t tile, const uint8_t* active_tiles, uint32_t sample_first, uint32_t sample_count,
+                                   uint32_t global_seed, int integrator_kind, int precision, double* planes_dev,
+                                   uint32_t n_planes, mcrt_stats* stats)
+{
+    if (!ctx) return MCRT_ERR_INVALID;
+    const std::string name = "mcrt_render_accumulate_lpe_dev";
+    if (!ctx->film_default) { ctx->error = name + ": LPE planes take the box film only"; return MCRT_ERR_UNSUPPORTED; }
+    if (integrator_kind == MCRT_INTEGRATOR_PHOTON)
+    {
+        ctx->error = name + ": the photon mapper has no light path expressions (its estimates have no event strings)";
+        return MCRT_ERR_UNSUPPORTED;
+    }
+    if (!ctx->lpe_n) { ctx->error = name + ": no LPE table (mcrt_set_light_path_expressions)"; return MCRT_ERR_INVALID; }
+    if (n_planes != ctx->lpe_n)
+    {
+        ctx->error = name + ": n_planes " + std::to_string(n_planes) + ", the table has " + std::to_string(ctx->lpe_n) + " expressions";
+        return MCRT_ERR_INVALID;
+    }
+    FilmSums sums{ planes_dev, nullptr, n_planes };
+    sums.lpe = true;
+    return accumulatePlanes(ctx, name, camera, y_first, y_step, n_rows, tile, active_tiles, sample_first, sample_count, global_seed,
+                            integrator_kind, precision, sums, stats);
 }
 
 int mcrt_render_accumulate_groups_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_t y_first, uint32_t y_step, uint32_t n_rows,
@@ -2282,6 +2378,32 @@ int mcrt_bvh4_host(const mcrt_scene_desc* scene, uint32_t max_leaf, void** handl
 void mcrt_bvh4_host_free(void* handle)
 {
     delete static_cast<std::vector<Bvh4Node>*>(handle);
+}
+
+int mcrt_lpe_compile_host(const char* const* exprs, uint32_t n, uint32_t n_groups, uint8_t* next, uint32_t* accept,
+                          uint8_t* group_symbol, uint32_t* n_states, uint32_t* n_symbols, char* error, uint32_t error_capacity)
+{
+    if (!next || !accept || !n_states || !n_symbols || (n_groups && !group_symbol)) return MCRT_ERR_INVALID;
+    LpeTable t;
+    std::string why;
+    const int rc = lpeCompile(exprs, n, n_groups, t, why);
+    if (error && error_capacity)
+    {
+        const size_t len = std::min<size_t>(why.size(), error_capacity - 1);
+        std::memcpy(error, why.data(), len);
+        error[len] = '\0';
+    }
+    if (rc != MCRT_OK) return rc;
+    std::memcpy(next, t.next.data(), t.next.size());
+    std::memcpy(accept, t.accept.data(), 256 * sizeof(uint32_t));
+    for (uint32_t g = 0; g < n_groups; g++)
+    {
+        auto it = std::lower_bound(t.labels.begin(), t.labels.end(), g);
+        group_symbol[g] = (uint8_t)(it != t.labels.end() && *it == g ? MCRT_LPE_SYM_LABEL0 + (it - t.labels.begin()) : MCRT_LPE_SYM_L);
+    }
+    *n_states = t.n_states;
+    *n_symbols = t.n_symbols;
+    return MCRT_OK;
 }
 
 int mcrt_frame_alloc(mcrt_ctx* ctx, uint64_t bytes, void** dev_ptr, unsigned char ipc_handle[64])

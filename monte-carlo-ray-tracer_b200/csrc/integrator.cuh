@@ -264,6 +264,12 @@ namespace mcrt
         size_t plane_values;
         uint32_t n_planes;
         uint32_t aovs;
+        // LPE render (mcrt_render_accumulate_lpe_dev, lpe_next non-null): n_planes = the expressions; the DFA's
+        // transitions [states][lpe_symbols], accept masks [256] and the symbol of each light (lpe.h)
+        const uint8_t* lpe_next;
+        const uint32_t* lpe_accept;
+        const uint8_t* lpe_light_symbol;
+        uint32_t lpe_symbols;
     };
 
     // ------------------------------------------------------------------------------------------
@@ -362,8 +368,33 @@ namespace mcrt
     // Film modes of the depositing kernels. FILM_MODE_BOX: the default box film, the kernels every benchmark and parity
     // case runs; FILM_MODE_SPLAT: a reconstruction filter; FILM_MODE_GROUPS: the box film with one plane per light group;
     // FILM_MODE_AOV: the box film with one plane per class of contribution, the plane each deposit site names - the
-    // light-path planes (MCRT_AOV_*) in the path tracer, the estimator planes (MCRT_PM_*) in the photon mapper
-    enum FilmMode : int { FILM_MODE_BOX = 0, FILM_MODE_SPLAT = 1, FILM_MODE_GROUPS = 2, FILM_MODE_AOV = 3 };
+    // light-path planes (MCRT_AOV_*) in the path tracer, the estimator planes (MCRT_PM_*) in the photon mapper;
+    // FILM_MODE_LPE: the box film with one plane per light path expression, a deposit into every plane whose bit is set
+    // in the accept mask of its event string (path tracer only)
+    enum FilmMode : int { FILM_MODE_BOX = 0, FILM_MODE_SPLAT = 1, FILM_MODE_GROUPS = 2, FILM_MODE_AOV = 3, FILM_MODE_LPE = 4 };
+
+    // FILM_MODE_LPE: the DFA of the expressions (lpe.h). Lanes of a warp sit in different states, so the few-KB tables are
+    // read through the read-only data path rather than from constant memory.
+    template <class R>
+    MCRT_D uint32_t lpeNext(const WaveParams<R>& p, uint32_t state, uint32_t symbol)
+    {
+        return __ldg(&p.lpe_next[state * p.lpe_symbols + symbol]);
+    }
+    template <class R>
+    MCRT_D uint32_t lpeAccept(const WaveParams<R>& p, uint32_t state) { return __ldg(&p.lpe_accept[state]); }
+    // symbol of an emitter: its label's, or the unlabelled L (NO_PRIM: an emissive primitive that is not a light)
+    template <class R>
+    MCRT_D uint32_t lpeLightSymbol(const WaveParams<R>& p, uint32_t light)
+    {
+        return light == NO_PRIM ? (uint32_t)MCRT_LPE_SYM_L : (uint32_t)__ldg(&p.lpe_light_symbol[light]);
+    }
+    // event of a scattering vertex: the interaction type the reference selected, smooth (dirac_delta) or rough
+    MCRT_D uint32_t lpeVertexSymbol(uint32_t type, bool dirac_delta)
+    {
+        if (type == IA_DIFFUSE) return MCRT_LPE_SYM_RD;
+        if (type == IA_REFLECT) return dirac_delta ? MCRT_LPE_SYM_RS : MCRT_LPE_SYM_RG;
+        return dirac_delta ? MCRT_LPE_SYM_TS : MCRT_LPE_SYM_TG;
+    }
 
     // AOV plane of a contribution. lobe: interaction type + 1 of the path's first scattering vertex, 0 for the camera
     // ray's own miss (the sky: background) or emitter hit (emission); indirect: the light path has more than one
@@ -377,7 +408,8 @@ namespace mcrt
     }
 
     // Film::deposit of one radiance contribution of sample (pixel, sample). light: index of the emitter it comes from,
-    // NO_PRIM for the sky (read by FILM_MODE_GROUPS only); plane: its AOV plane (read by FILM_MODE_AOV only)
+    // NO_PRIM for the sky (read by FILM_MODE_GROUPS only); plane: its AOV plane (FILM_MODE_AOV), or its accept mask, one
+    // bit per plane (FILM_MODE_LPE)
     template <int FILM, class R>
     MCRT_D void depositRadiance(const WaveParams<R>& p, uint32_t film_index, uint32_t pixel, uint32_t sample, const V3<R>& v,
                                 uint32_t light = NO_PRIM, uint32_t plane = 0u)
@@ -394,6 +426,10 @@ namespace mcrt
         else if constexpr (FILM == FILM_MODE_AOV)
         {
             filmAddV(p.film + plane * p.plane_values, film_index, v);
+        }
+        else if constexpr (FILM == FILM_MODE_LPE)
+        {
+            for (uint32_t m = plane; m; m &= m - 1u) filmAddV(p.film + (uint32_t)(__ffs(m) - 1) * p.plane_values, film_index, v);
         }
         else
         {
@@ -684,6 +720,9 @@ namespace mcrt
             // FILM_MODE_AOV: interaction type + 1 of the path's first vertex (0 before it; path tracer only), the shadow
             // ray's plane
             uint32_t lobe = 0, sh_plane = 0;
+            // FILM_MODE_LPE: the DFA state after the events so far (bits 16-23 of meta2.y; 0 after C); sh_plane then holds
+            // the shadow ray's accept mask
+            uint32_t lpe_state = 0;
 
             if (alive)
             {
@@ -698,6 +737,7 @@ namespace mcrt
                 ior_count = meta2.y & 0xFFu;
                 ray.dirac_delta = (meta2.y >> 8) & 1u;
                 if constexpr (KIND == 0 && FILM == FILM_MODE_AOV) lobe = (meta2.y >> 9) & 3u;
+                if constexpr (FILM == FILM_MODE_LPE) lpe_state = (meta2.y >> 16) & 0xFFu;
                 ray.refraction = false;
                 const uint32_t film_index = meta2.z;
 
@@ -730,7 +770,10 @@ namespace mcrt
                 if (hit.prim == NO_PRIM)
                 {
                     // path-tracer.cpp:27-30; the photon mapper adds no sky (photon-mapper.cpp:292-295)
-                    if constexpr (KIND == 0)
+                    if constexpr (KIND == 0 && FILM == FILM_MODE_LPE)
+                        depositRadiance<FILM>(p, film_index, meta.x, meta.y, skyColor(ray.direction) * throughput, NO_PRIM,
+                                              lpeAccept(p, lpeNext(p, lpe_state, MCRT_LPE_SYM_B)));
+                    else if constexpr (KIND == 0)
                         depositRadiance<FILM>(p, film_index, meta.x, meta.y, skyColor(ray.direction) * throughput, NO_PRIM,
                                               FILM == FILM_MODE_AOV ? aovPlane(lobe, ray.depth > 1u, true) : 0u);
                     alive = false;
@@ -756,18 +799,26 @@ namespace mcrt
                     {
                         if (ray.depth == 0 || ray.dirac_delta)
                         {
-                            depositRadiance<FILM>(p, film_index, meta.x, meta.y, m.emittance * throughput, ps.light,
-                                                  FILM != FILM_MODE_AOV ? 0u : (KIND == 0 ? aovPlane(lobe, ray.depth > 1u, false)
-                                                                                          : (uint32_t)MCRT_PM_EMISSION));
+                            if constexpr (FILM == FILM_MODE_LPE)
+                                depositRadiance<FILM>(p, film_index, meta.x, meta.y, m.emittance * throughput, ps.light,
+                                                      lpeAccept(p, lpeNext(p, lpe_state, lpeLightSymbol(p, ps.light))));
+                            else
+                                depositRadiance<FILM>(p, film_index, meta.x, meta.y, m.emittance * throughput, ps.light,
+                                                      FILM != FILM_MODE_AOV ? 0u : (KIND == 0 ? aovPlane(lobe, ray.depth > 1u, false)
+                                                                                              : (uint32_t)MCRT_PM_EMISSION));
                         }
                         else if (ls_light != NO_PRIM && sc.lights[ls_light].prim == hit.prim)
                         {
                             R cos_light_theta = dot(ia.out, ia.normal);
                             R light_pdf = pow2(ia.t) / (ps.area * cos_light_theta);
                             R mis_weight = powerHeuristic(ls_bsdf_pdf, light_pdf);
-                            depositRadiance<FILM>(p, film_index, meta.x, meta.y, (mis_weight * m.emittance / ls_select) * throughput, ls_light,
-                                                  FILM != FILM_MODE_AOV ? 0u : (KIND == 0 ? aovPlane(lobe, ray.depth > 1u, false)
-                                                                                          : (uint32_t)MCRT_PM_DIRECT));
+                            if constexpr (FILM == FILM_MODE_LPE)
+                                depositRadiance<FILM>(p, film_index, meta.x, meta.y, (mis_weight * m.emittance / ls_select) * throughput, ls_light,
+                                                      lpeAccept(p, lpeNext(p, lpe_state, lpeLightSymbol(p, ls_light))));
+                            else
+                                depositRadiance<FILM>(p, film_index, meta.x, meta.y, (mis_weight * m.emittance / ls_select) * throughput, ls_light,
+                                                      FILM != FILM_MODE_AOV ? 0u : (KIND == 0 ? aovPlane(lobe, ray.depth > 1u, false)
+                                                                                              : (uint32_t)MCRT_PM_DIRECT));
                         }
                     }
 
@@ -776,6 +827,14 @@ namespace mcrt
 
                     // ---- PhotonMapper::sampleRay control flow, photon-mapper.cpp:299-332
                     bool do_direct = true, do_bsdf = true;
+                    if constexpr (FILM == FILM_MODE_LPE)
+                    {
+                        // this vertex's event, for NEE here and everything after; once no expression can match, nothing
+                        // the path could still add lands in a plane, and the sampler is a pure function of (pixel,
+                        // sample, depth), so ending it here changes no plane
+                        lpe_state = lpeNext(p, lpe_state, lpeVertexSymbol(ia.type, ia.dirac_delta));
+                        if (lpe_state == MCRT_LPE_DEAD) { do_direct = false; do_bsdf = false; alive = false; }
+                    }
                     if constexpr (KIND == 1)
                     {
                         if (ia.dirac_delta)
@@ -861,6 +920,12 @@ namespace mcrt
                                     sh_select = ls_select;
                                     sh_light = L.prim;
                                     if constexpr (FILM == FILM_MODE_AOV) sh_plane = KIND == 0 ? aovPlane(lobe, ray.depth > 0u, false) : (uint32_t)MCRT_PM_DIRECT;
+                                    if constexpr (FILM == FILM_MODE_LPE)
+                                    {
+                                        // a mask no expression sets traces no shadow ray, like a zero BSDF value
+                                        sh_plane = lpeAccept(p, lpeNext(p, lpe_state, lpeLightSymbol(p, ls_light)));
+                                        want_shadow = sh_plane != 0u;
+                                    }
                                 }
                             }
                         }
@@ -942,7 +1007,8 @@ namespace mcrt
                 }
                 stStream(&out.meta[slot], make_uint4(meta.x, meta.y, (nray.depth & 0xFFFFu) | (nray.diffuse_depth << 16),
                                                      (uint32_t)nray.refraction_level));
-                stStream(&out.meta2[slot], make_uint4(ls_light, ior_count | (nray.dirac_delta ? 256u : 0u) | (lobe << 9), meta2.z,
+                stStream(&out.meta2[slot], make_uint4(ls_light, ior_count | (nray.dirac_delta ? 256u : 0u) | (lobe << 9) |
+                                                                    (FILM == FILM_MODE_LPE ? lpe_state << 16 : 0u), meta2.z,
                                                       sc.shade[hit_prim].type == PRIM_TRIANGLE ? hit_prim : NO_PRIM));
                 if (sorting) { p.sort.path_key[cur ^ 1][slot] = pkey; p.sort.path_rank[cur ^ 1][slot] = prank; }
             }
@@ -952,7 +1018,7 @@ namespace mcrt
                 stStream(&srec.o, V4<R>(sh_o, sh_bsdf_pdf));
                 stStream(&srec.d, V4<R>(sh_d, sh_area_cos));
                 stStream(&srec.meta, make_uint4(sh_light, meta2.z, sc.shade[hit_prim].type == PRIM_TRIANGLE ? hit_prim : NO_PRIM,
-                                                FILM == FILM_MODE_AOV ? sh_plane : meta.y));
+                                                FILM == FILM_MODE_AOV || FILM == FILM_MODE_LPE ? sh_plane : meta.y));
                 // float64: also write the padding after meta, so that no 32-byte sector of the record is left half
                 // written (without this store the C2 shade stage measured 930 instead of 744 ms per frame)
                 if constexpr (sizeof(R) == 8) stStream(reinterpret_cast<uint4*>(&srec) + 5, make_uint4(0u, 0u, 0u, 0u));
@@ -979,7 +1045,7 @@ namespace mcrt
     }
 
     // FILM_MODE_GROUPS finds the sampled light's group through the light primitive's shading record (sm.x is L.prim);
-    // FILM_MODE_AOV reads the AOV plane k_shade stored in place of the sample index (sm.w)
+    // FILM_MODE_AOV reads the AOV plane k_shade stored in place of the sample index (sm.w), FILM_MODE_LPE the accept mask
     template <class R, int FILM, int PRIMS, int FAST>
     __global__ void __launch_bounds__(256, FAST == 2 ? MCRT_TRACE_MINBLOCKS_DYN : (FAST == 1 ? MCRT_TRACE_MINBLOCKS_FAST : (PRIMS == PRIMS_ALL ? Mode<R>::trace_minblocks : Mode<R>::trace_minblocks_pruned))) k_shadow(WaveParams<R> p)
     {

@@ -43,6 +43,11 @@ namespace mcrt
         // scenes whose materials use no Oren-Nayar / GGX / conductor Fresnel run the instantiation without that code
         const bool lite = (p.scene.material_flags_any & ~SHADE_FEATS_LITE) == 0;
         if (!p.filmp.is_default_box) k_shade<MCRT_REAL, 0, FILM_MODE_SPLAT, SHADE_FEATS_ALL><<<grid * 2, 128, 0, s>>>(p, cur);
+        else if (p.n_planes && p.lpe_next)
+        {
+            if (lite) k_shade<MCRT_REAL, 0, FILM_MODE_LPE, SHADE_FEATS_LITE><<<grid * 2, 128, 0, s>>>(p, cur);
+            else k_shade<MCRT_REAL, 0, FILM_MODE_LPE, SHADE_FEATS_ALL><<<grid * 2, 128, 0, s>>>(p, cur);
+        }
         else if (p.n_planes && p.aovs)
         {
             if (lite) k_shade<MCRT_REAL, 0, FILM_MODE_AOV, SHADE_FEATS_LITE><<<grid * 2, 128, 0, s>>>(p, cur);
@@ -134,7 +139,7 @@ namespace mcrt
         #undef MCRT_KNN_LAUNCH1
         #undef MCRT_KNN_LAUNCH2
     }
-    // k_shadow of the box film (one plane, light-group planes, or AOV / photon-mapper component planes) with the
+    // k_shadow of the box film (one plane, light-group planes, AOV / photon-mapper component planes, or LPE planes) with the
     // scene-specialised traversal
     template <int FILM> static void launchShadowBox(const WaveParams<MCRT_REAL>& p, int grid, cudaStream_t s)
     {
@@ -170,6 +175,7 @@ namespace mcrt
             }
             k_shadow<MCRT_REAL, FILM_MODE_SPLAT, PRIMS_ALL, 0><<<grid, 256, 0, s>>>(p);
         }
+        else if (p.n_planes && p.lpe_next) launchShadowBox<FILM_MODE_LPE>(p, grid, s);
         else if (p.n_planes && p.aovs) launchShadowBox<FILM_MODE_AOV>(p, grid, s);
         else if (p.n_planes) launchShadowBox<FILM_MODE_GROUPS>(p, grid, s);
         else launchShadowBox<FILM_MODE_BOX>(p, grid, s);
