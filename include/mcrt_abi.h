@@ -282,6 +282,11 @@ int mcrt_photon_download(mcrt_ctx* ctx, int which, mcrt_photon_map_desc* out);
  * mcrt_photon_emit_pass carry these indices; maps of mcrt_photon_upload and mcrt_photon_build_dev do not
  * (MCRT_ERR_UNSUPPORTED), and neither do maps emitted before the last mcrt_scene_upload. */
 int mcrt_photon_download_lights(mcrt_ctx* ctx, int which, uint32_t* out, uint64_t n);
+/* The reverse-DFA state (mcrt_lpe_compile_photon_host) of each photon of a built map before the event of the vertex
+ * where it was stored, out[n] HOST, in mcrt_photon_download's order; n must be the map's photon count. Only maps emitted
+ * by mcrt_photon_emit / _emit_pass while an LPE table the photon mapper takes was set carry them (else
+ * MCRT_ERR_UNSUPPORTED). A photon whose state is MCRT_LPE_DEAD is still stored: it counts for every estimate's radius. */
+int mcrt_photon_download_lpe_states(mcrt_ctx* ctx, int which, uint32_t* out, uint64_t n);
 
 /* The octree construction step of mcrt_photon_emit alone, on caller photons: Octree<Photon>
  * insertion + LinearOctree::compact (octree.cpp:34-81, linear-octree.cpp:201-244) on the GPU.
@@ -574,8 +579,17 @@ int mcrt_set_light_path_expressions(mcrt_ctx* ctx, const char* const* exprs, uin
  * contribution out; a path ends at the vertex where its state becomes MCRT_LPE_DEAD, and next-event estimation that no
  * expression accepts traces no shadow ray, so every plane keeps its value while fewer rays are traced.
  * MCRT_ERR_INVALID: no LPE table, n_planes other than its expression count, a null planes_dev, and every argument the
- * one-plane entry points refuse. MCRT_ERR_UNSUPPORTED: a reconstruction filter, the photon mapper. Nothing is written
- * when a call is refused. The other entry points ignore the table. */
+ * one-plane entry points refuse. MCRT_ERR_UNSUPPORTED: a reconstruction filter. Nothing is written when a call is
+ * refused. The other entry points ignore the table.
+ * The photon mapper (integrator_kind MCRT_INTEGRATOR_PHOTON) gives every photon term of its k-NN or gather estimates a
+ * string of its own: C, the camera's events up to the gather vertex x, x's event, then the photon's events from the one
+ * before x back to its first bounce (e_m .. e_1), then its light, C c1..ck x e_m..e_1 L'g'. Emitter hits and next-event
+ * estimation read as the path tracer's. Expressions select which terms land in a plane; they change neither the photons
+ * an estimate finds nor the radius it is normalised by. A camera path whose every possible photon term no expression
+ * accepts issues no k-NN query. The photon mapper needs maps emitted by mcrt_photon_emit / _emit_pass while this same
+ * table (same expressions, groups and light symbols) was set; the first refusal, MCRT_ERR_UNSUPPORTED, is of any other
+ * maps (none, mcrt_photon_upload, mcrt_photon_build_dev, no or another table, before the last mcrt_scene_upload), the
+ * second, MCRT_ERR_UNSUPPORTED, of a table whose reversed expressions need more than MCRT_LPE_MAX_STATES states. */
 int mcrt_render_accumulate_lpe_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_t y_first, uint32_t y_step, uint32_t n_rows,
                                    uint32_t tile, const uint8_t* active_tiles, uint32_t sample_first, uint32_t sample_count,
                                    uint32_t global_seed, int integrator_kind, int precision, double* planes_dev,
@@ -587,6 +601,15 @@ int mcrt_render_accumulate_lpe_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uin
  * would. */
 int mcrt_lpe_compile_host(const char* const* exprs, uint32_t n, uint32_t n_groups, uint8_t* next, uint32_t* accept,
                           uint8_t* group_symbol, uint32_t* n_states, uint32_t* n_symbols, char* error, uint32_t error_capacity);
+/* Test hook (host only, no CUDA call): the photon mapper's side of the same tables. rev_next[MCRT_LPE_MAX_STATES *
+ * MCRT_LPE_MAX_SYMBOLS] receives [*rev_n_states][n_symbols], the DFA of the reversed expressions, which reads a
+ * photon's events in emission order (its light's symbol first) from *rev_start (MCRT_LPE_DEAD when nothing can match);
+ * join[MCRT_LPE_MAX_STATES * MCRT_LPE_MAX_STATES] receives [n_states][*rev_n_states], the accept mask of a contribution
+ * whose camera prefix ends in forward state s and whose photon history ends in reverse state r. Returns what
+ * mcrt_lpe_compile_host would, or MCRT_ERR_UNSUPPORTED, with the reason in error, when the path tracer would take the
+ * table and the photon mapper would refuse it. */
+int mcrt_lpe_compile_photon_host(const char* const* exprs, uint32_t n, uint32_t n_groups, uint8_t* rev_next, uint32_t* rev_start,
+                                 uint32_t* rev_n_states, uint32_t* join, char* error, uint32_t error_capacity);
 
 /* Denoising a progressive frame (mcrt_denoise_dev) needs per-pixel guides: the first hits of the camera rays of samples
  * [sample_first, sample_first + sample_count) of every pixel of the whole width x height frame add

@@ -43,6 +43,7 @@ ABI_SYMBOLS = [
     "mcrt_set_light_groups", "mcrt_render_accumulate_groups_dev", "mcrt_light_groups_combine_dev",
     "mcrt_render_accumulate_aovs_dev", "mcrt_photon_download_lights", "mcrt_render_accumulate_photon_components_dev",
     "mcrt_set_light_path_expressions", "mcrt_render_accumulate_lpe_dev", "mcrt_lpe_compile_host",
+    "mcrt_lpe_compile_photon_host", "mcrt_photon_download_lpe_states",
 ]
 
 # The light-path AOV planes of mcrt_render_accumulate_aovs_dev, in plane order (MCRT_AOV_* of include/mcrt_abi.h):
@@ -60,6 +61,23 @@ LPE_SYM_RD, LPE_SYM_RS, LPE_SYM_RG, LPE_SYM_TS, LPE_SYM_TG, LPE_SYM_B, LPE_SYM_L
 LPE_DEAD, LPE_MAX_STATES, LPE_MAX_SYMBOLS, LPE_MAX_EXPRESSIONS = 255, 255, 71, 32
 # The light-path AOV planes of AOV_NAMES as light path expressions, in the same order
 AOV_LPES = ("CB", "CL", "C<RD>[LB]", "C<RD>.+[LB]", "C[<RS><RG>][LB]", "C[<RS><RG>].+[LB]", "C<T.>[LB]", "C<T.>.+[LB]")
+
+
+def PM_COMPONENT_LPES(direct_visualization):
+    """The photon mapper's component planes of PHOTON_COMPONENT_NAMES as light path expressions, in the same order, for
+    maps emitted with (True) or without (False) direct_visualization. N = [<RD><RG><TG>] is a non-delta event; the
+    camera path reaches its first non-delta vertex x through smooth events <.S>*.
+
+    Without direct visualization, light at x comes from next-event estimation (C S* x L, direct) and the caustic map
+    (C S* x <.S> ..., caustic); the global map is gathered one non-delta bounce later (C S* x N ..., global).
+
+    With it, both maps are gathered at x and no shadow ray is traced, so a direct photon stored at x reads C S* x L,
+    the string next-event estimation would have: that string belongs to the global estimate, and the direct plane,
+    which is then zero, takes "C.*B", which no photon-mapped path matches (the photon mapper has no sky)."""
+    n = "[<RD><RG><TG>]"
+    if direct_visualization:
+        return ("C<.S>*L", "C.*B", f"C<.S>*{n}<.S>.*L", f"C<.S>*{n}({n}.*)?L")
+    return ("C<.S>*L", f"C<.S>*{n}L", f"C<.S>*{n}{{1,2}}<.S>.*L", f"C<.S>*{n}{{2}}({n}.*)?L")
 
 
 class McrtError(RuntimeError):
@@ -224,6 +242,7 @@ def lib():
                                                 C.c_void_p, C.POINTER(Stats)]
         L.mcrt_photon_download.argtypes = [C.c_void_p, C.c_int, C.POINTER(PhotonMapDesc)]
         L.mcrt_photon_download_lights.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_uint64]
+        L.mcrt_photon_download_lpe_states.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_uint64]
         L.mcrt_octree_build.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p, C.POINTER(C.c_void_p),
                                         C.POINTER(PhotonMapDesc), C.POINTER(C.c_double)]
         L.mcrt_octree_free.argtypes = [C.c_void_p]
@@ -267,6 +286,8 @@ def lib():
         L.mcrt_render_accumulate_lpe_dev.argtypes = L.mcrt_render_accumulate_groups_dev.argtypes
         L.mcrt_lpe_compile_host.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p,
                                             C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.c_char_p, C.c_uint32]
+        L.mcrt_lpe_compile_photon_host.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint32),
+                                                   C.POINTER(C.c_uint32), C.c_void_p, C.c_char_p, C.c_uint32]
         L.mcrt_light_groups_combine_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint64, C.c_void_p, C.c_void_p]
         L.mcrt_render_features_dev.argtypes = [C.c_void_p, C.POINTER(CameraRec), C.c_uint32, C.c_uint32, C.c_uint32, C.c_int,
                                                C.c_void_p, C.POINTER(Stats)]
@@ -532,6 +553,8 @@ class Integrator:
     def upload_scene(self):
         d = self.scene.desc()
         n = C.c_uint64()
+        # the library clears the group and LPE tables and forgets which table the maps were emitted under
+        self._lpe_key = self._groups_key = self._photon_lpe_key = None
         self._check(lib().mcrt_scene_upload(self.ctx, C.byref(d), C.byref(n)))
         self.h2d_bytes = n.value
         return n.value
@@ -692,13 +715,17 @@ class Integrator:
         """mcrt_set_light_groups: light l (the scene's l-th light_prim) goes to group ids[l]; the renders of
         render_accumulate_groups_dev then have n_groups + 1 planes, the last one the sky's. n_groups: max(ids) + 1 if None.
         ids None clears the table."""
+        self._lpe_key = None   # the library clears the LPE table too
         if ids is None:
             self._check(lib().mcrt_set_light_groups(self.ctx, None, 0, 0))
+            self._groups_key = None
             return
         ids = np.ascontiguousarray(ids, dtype=np.uint32).reshape(-1)
         n_groups = (int(ids.max()) + 1 if ids.size else 0) if n_groups is None else int(n_groups)
         table = ids if ids.size else np.zeros(1, np.uint32)   # a lightless scene's sky-only table: any non-null pointer
+        self._groups_key = None
         self._check(lib().mcrt_set_light_groups(self.ctx, table.ctypes.data_as(C.c_void_p), ids.size, n_groups))
+        self._groups_key = (tuple(int(g) for g in ids), n_groups)
 
     def render_accumulate_groups_dev(self, camera, planes_ptr, n_planes, sample_first, sample_count, tile=0, active=None,
                                      y_first=0, y_step=1, n_rows=None, precision=None):
@@ -721,7 +748,10 @@ class Integrator:
         so set_light_groups comes first (it clears this table). exprs None or empty clears the table."""
         exprs = list(exprs or ())
         arr = _lpe_strings(exprs)
+        self._lpe_key = None
         self._check(lib().mcrt_set_light_path_expressions(self.ctx, C.cast(arr, C.c_void_p) if exprs else None, len(exprs)))
+        # what the table is made of, for PhotonMapper.has_photon_lpe_states
+        self._lpe_key = (tuple(str(e) for e in exprs), getattr(self, "_groups_key", None)) if exprs else None
 
     def render_accumulate_lpe_dev(self, camera, planes_ptr, n_planes, sample_first, sample_count, tile=0, active=None,
                                   y_first=0, y_step=1, n_rows=None, precision=None):
@@ -863,7 +893,11 @@ class PhotonMapper(Integrator):
     the scene pack, of photon_maps= and of emit_sharded do not.
 
     Components (render_accumulate_components_dev, Progressive(components=True)) split a frame by the estimator behind
-    each contribution (PHOTON_COMPONENT_NAMES) and work with every kind of map."""
+    each contribution (PHOTON_COMPONENT_NAMES) and work with every kind of map.
+
+    Light path expressions (render_accumulate_lpe_dev, Progressive(lpes=...)) need each photon's own events, which
+    only maps of emit() / emit_pass() record, and only while the table is set: set_light_path_expressions, then emit
+    (has_photon_lpe_states). Progressive does this itself, emitting again with the arguments of the last emit."""
     kind = INTEGRATOR_PHOTON
 
     def __init__(self, scene, device=0, precision=PRECISION_F64, global_seed=0x12345678, photon_maps=None, emit=None):
@@ -884,6 +918,27 @@ class PhotonMapper(Integrator):
     def has_photon_lights(self):
         """True when the current maps record the light that emitted each photon (maps of emit / emit_pass)."""
         return getattr(self, "_photon_lights", False)
+
+    @property
+    def has_photon_lpe_states(self):
+        """True when the current maps were emitted (emit / emit_pass) while the current LPE table, with the same
+        expressions and light groups, was set: each photon then carries the state of its own path."""
+        key = getattr(self, "_photon_lpe_key", None)
+        return key is not None and getattr(self, "_emitted", None) is not None and key == getattr(self, "_lpe_key", None)
+
+    def photon_lpe_states(self, which):
+        """The reverse-DFA state of each photon of map `which` before the event of its storage vertex, uint32 [n_photons],
+        in the order of the photons of _maps[which] (mcrt_photon_download_lpe_states; lpe_compile_photon's rev_next)."""
+        out = np.zeros(self.n_photons[which], np.uint32)
+        self._check(lib().mcrt_photon_download_lpe_states(self.ctx, int(which), _ptr(out), out.size))
+        return out
+
+    def emit_again(self):
+        """Repeats the last emit() / emit_pass() with the same arguments: the same photons (the passes are deterministic),
+        now with the states of the LPE table set since. -> (n_caustic, n_global)"""
+        if getattr(self, "_emit_args", None) is None:
+            raise McrtError("the photon maps did not come from emit() / emit_pass()")
+        return self.emit_pass(*self._emit_args)
 
     def photon_lights(self, which):
         """The index of the light that emitted each photon of map `which` (0 caustic, 1 global), uint32 [n_photons], in
@@ -960,6 +1015,7 @@ class PhotonMapper(Integrator):
         self._host_maps = None
         self._emitted = (int(k_nearest_photons), int(bool(direct_visualization)))
         self._photon_lights = False   # the gathered arrays carry no light index
+        self._emit_args = self._photon_lpe_key = None
         self.n_photons = (gathered[0].numel() // 8, gathered[1].numel() // 8)
         return self.n_photons
 
@@ -986,6 +1042,9 @@ class PhotonMapper(Integrator):
         self._host_maps = None
         self._emitted = (int(k_nearest_photons), int(bool(direct_visualization)))
         self._photon_lights = True
+        self._emit_args = (pass_index, emissions, caustic_factor, max_photons_per_octree_leaf, k_nearest_photons, scene_bounds,
+                           direct_visualization, precision)
+        self._photon_lpe_key = getattr(self, "_lpe_key", None)
         self.n_photons = (nc.value, ng.value)
         return nc.value, ng.value
 
@@ -1005,6 +1064,7 @@ class PhotonMapper(Integrator):
         self._host_maps = value
         self._emitted = None
         self._photon_lights = False
+        self._emit_args = self._photon_lpe_key = None
 
     @staticmethod
     def _map_desc(m):
@@ -1202,6 +1262,32 @@ def lpe_compile(exprs, n_groups=0):
             "group_symbol": gs[:int(n_groups)].copy()}
 
 
+def lpe_compile_photon(exprs, n_groups=0):
+    """lpe_compile plus the photon mapper's side of the table (mcrt_lpe_compile_photon_host): "rev_next": uint8
+    [rev_n_states, n_symbols], the DFA of the reversed expressions, which reads a photon's events in emission order
+    (its light's symbol first) from "rev_start" (LPE_DEAD when nothing can match); "join": uint32 [n_states,
+    rev_n_states], the accept mask of a contribution whose camera prefix ends in forward state s and whose photon history
+    ends in reverse state r. Raises McrtError (.code MCRT_ERR_UNSUPPORTED) when only the path tracer can take the table."""
+    out = lpe_compile(exprs, n_groups)
+    exprs = list(exprs)
+    arr = _lpe_strings(exprs)
+    rev = np.zeros(LPE_MAX_STATES * LPE_MAX_SYMBOLS, np.uint8)
+    join = np.zeros(LPE_MAX_STATES * LPE_MAX_STATES, np.uint32)
+    start, nr = C.c_uint32(), C.c_uint32()
+    err = C.create_string_buffer(1024)
+    rc = lib().mcrt_lpe_compile_photon_host(C.cast(arr, C.c_void_p) if exprs else None, len(exprs), int(n_groups),
+                                            rev.ctypes.data_as(C.c_void_p), C.byref(start), C.byref(nr),
+                                            join.ctypes.data_as(C.c_void_p), err, len(err))
+    if rc:
+        e = McrtError(f"mcrt_lpe_compile_photon_host failed with {rc}: {err.value.decode()}")
+        e.code = rc
+        raise e
+    ns, nsym = out["next"].shape
+    out.update(rev_next=rev[:nr.value * nsym].reshape(nr.value, nsym).copy(), rev_start=int(start.value),
+               join=join[:ns * nr.value].reshape(ns, nr.value).copy())
+    return out
+
+
 def light_groups_by_emittance(scene, rtol=1e-12):
     """Groups the scene's lights by emittance: a light joins the first group whose first light's emittance equals its
     own in every channel to within rtol (relative; the default only absorbs the last-bit differences a mesh light's
@@ -1314,8 +1400,10 @@ class Progressive:
     its own noise estimate, which shows which estimator still dominates the error, and relight(weights) /
     denoise(weights=...) recomposite the frame, e.g. relight([1, 1, 0, 1]) removes the caustics.
 
-    Light path expressions (lpes = a list of expressions, see mcrt_set_light_path_expressions; box film, path tracer,
-    not together with AOVs or components): A and B hold one plane per expression and, last, the beauty plane "C.*",
+    Light path expressions (lpes = a list of expressions, see mcrt_set_light_path_expressions; box film, not together
+    with AOVs or components; the path tracer, or the photon mapper with maps of emit() / emit_pass(), which this emits
+    again with the same arguments once the table is set, so that every photon carries its path's state - the same
+    photons, since the passes are deterministic): A and B hold one plane per expression and, last, the beauty plane "C.*",
     [len(lpes) + 1, rows, width, 3], filled by mcrt_render_accumulate_lpe_dev. Expressions may overlap or leave
     contributions out, so frame, error, render, render_adaptive and denoise work on the beauty plane alone and behave
     as without expressions. At most 31 expressions, since the beauty plane takes the table's 32nd. light_groups here only
@@ -1328,8 +1416,9 @@ class Progressive:
     def __init__(self, integrator, camera, y_first=0, y_step=1, n_rows=None, tile=16, light_groups=None, aovs=False,
                  components=False, lpes=None):
         import torch
-        if lpes is not None and integrator.kind == INTEGRATOR_PHOTON:
-            raise McrtError("the photon mapper has no light path expressions")
+        if lpes is not None and integrator.kind == INTEGRATOR_PHOTON and getattr(integrator, "_emit_args", None) is None:
+            raise McrtError("the photon mapper has light path expressions only with maps of emit() / emit_pass(): a photon's "
+                            "events are recorded while it is emitted")
         if lpes is not None and (aovs or components):
             raise McrtError("light path expressions together with AOVs or components in one render are not supported")
         if components and integrator.kind != INTEGRATOR_PHOTON:
@@ -1365,6 +1454,8 @@ class Progressive:
                 self.lpe_groups = np.ascontiguousarray(light_groups, dtype=np.uint32).reshape(-1)
             self.n_planes = len(self.lpes) + 1
             self._set_lpe_tables()   # refuses a wrong expression or table before anything is allocated
+            if integrator.kind == INTEGRATOR_PHOTON:
+                integrator.emit_again()   # the same photons, now carrying their states under this table
             light_groups = None
         if light_groups is not None:
             if self.filtered:
@@ -1820,6 +1911,8 @@ class ProgressivePhotonMapping(Progressive):
     light_groups: as Progressive's. Every pass emits its own map, and emitted maps record each photon's light, so the
     passes split their estimates by group; the pass-0 map is emitted before the table is set.
 
+    lpes: as Progressive's. Every pass emits its map while the table is set, so every photon carries its path's state.
+
     components: as Progressive's. component_frames() then shows whether the caustic or the global estimate, whose radii
     shrink on their own schedules, still dominates the error.
 
@@ -1831,7 +1924,7 @@ class ProgressivePhotonMapping(Progressive):
     the next add() emits again (the passes are deterministic)."""
 
     def __init__(self, photon_mapper, camera, emissions, caustic_factor, max_photons_per_octree_leaf=200, alpha=2 / 3,
-                 radius=None, k_nearest_photons=50, tile=16, light_groups=None, aovs=False, components=False):
+                 radius=None, k_nearest_photons=50, tile=16, light_groups=None, aovs=False, components=False, lpes=None):
         if not isinstance(photon_mapper, PhotonMapper):
             raise McrtError("ProgressivePhotonMapping needs a PhotonMapper")
         if aovs:
@@ -1840,10 +1933,13 @@ class ProgressivePhotonMapping(Progressive):
         self.emissions, self.caustic_factor = int(emissions), float(caustic_factor)
         self.max_photons_per_octree_leaf, self.k_nearest_photons = int(max_photons_per_octree_leaf), int(k_nearest_photons)
         self.alpha = float(alpha)
-        if light_groups is not None and not photon_mapper.has_photon_lights:
-            # Progressive sets the table on maps that carry light indices: the pass-0 map
+        if (light_groups is not None and not photon_mapper.has_photon_lights) or \
+                (lpes is not None and getattr(photon_mapper, "_emit_args", None) is None):
+            # Progressive sets the table on maps that carry light indices, and emits again the maps of emit_pass: the
+            # pass-0 map
             photon_mapper.emit_pass(0, self.emissions, self.caustic_factor, self.max_photons_per_octree_leaf, self.k_nearest_photons)
-        super().__init__(photon_mapper, camera, tile=tile, light_groups=light_groups, components=components)
+        super().__init__(photon_mapper, camera, tile=tile, light_groups=light_groups, components=components,
+                         **({"lpes": lpes} if lpes is not None else {}))
         if radius is None:
             radius = self._initial_radii()
         r = (float(radius), float(radius)) if np.ndim(radius) == 0 else tuple(float(x) for x in radius)
@@ -1881,6 +1977,8 @@ class ProgressivePhotonMapping(Progressive):
 
     def add(self, samples):
         """Emits the map of pass self.passes, gathers with that pass's radii and renders the next samples (Progressive.add)."""
+        if self.lpes is not None:
+            self._set_lpe_tables()   # the pass's photons carry their states under this render's table
         self._emit(self.passes)
         self.integrator.gather_radius(*self.pass_radii(self.passes))
         return super().add(samples)
@@ -1892,13 +1990,13 @@ class ProgressivePhotonMapping(Progressive):
 
     @classmethod
     def load(cls, path, photon_mapper, camera, emissions, caustic_factor, max_photons_per_octree_leaf=200, alpha=2 / 3,
-             radius=None, k_nearest_photons=50, tile=None, light_groups=None, components=False):
+             radius=None, k_nearest_photons=50, tile=None, light_groups=None, components=False, lpes=None):
         """Resumes a checkpoint written by save(). Raises McrtError, and resumes nothing, when the seed, precision,
-        camera, film, tile, scene, emissions, caustic factor, leaf size, alpha, initial radii, light groups or components
-        differ from the checkpoint's (radius None derives them from the pass-0 maps again)."""
+        camera, film, tile, scene, emissions, caustic factor, leaf size, alpha, initial radii, light groups, components
+        or light path expressions differ from the checkpoint's (radius None derives them from the pass-0 maps again)."""
         data = _read_checkpoint(path)
         p = cls(photon_mapper, camera, emissions, caustic_factor, max_photons_per_octree_leaf, alpha, radius, k_nearest_photons,
-                int(data["tile"]) if tile is None else int(tile), light_groups, components=components)
+                int(data["tile"]) if tile is None else int(tile), light_groups, components=components, lpes=lpes)
         p._restore(path, data)
         return p
 

@@ -113,6 +113,15 @@ struct mcrt_ctx
     uint32_t* d_lpe_accept = nullptr;       // [256]
     uint8_t* d_lpe_light_symbol = nullptr;  // [n_lights] (grow-only)
     size_t lpe_light_values = 0;
+    // the photon mapper's side of the table (lpe.h): reversed expressions' DFA, join with the forward states
+    uint8_t* d_lpe_rev_next = nullptr;      // [MCRT_LPE_MAX_STATES][MCRT_LPE_MAX_SYMBOLS] at most, [states][lpe_symbols] used
+    uint32_t* d_lpe_join = nullptr;         // [MCRT_LPE_MAX_STATES][MCRT_LPE_MAX_STATES] at most, [states][lpe_rev_states] used
+    uint8_t* d_lpe_join_any = nullptr;      // [256]
+    uint32_t lpe_rev_states = 0, lpe_rev_start = MCRT_LPE_DEAD;
+    std::string lpe_photon_error;           // non-empty: the photon mapper refuses the table, for this reason
+    // the table's content (every compiled array and the lights' symbols): maps emitted under a table carry its identity,
+    // so that setting the same expressions and groups again keeps them valid
+    std::string lpe_identity;
     cudaEvent_t ev_start = nullptr, ev_stop = nullptr, ev_poll[2] = { nullptr, nullptr };
 
     // photon maps (PhotonMapper::caustic_map / global_map) + k-NN query queues
@@ -133,6 +142,10 @@ struct mcrt_ctx
     // the uploaded maps carry the emitting light of each photon (maps of mcrt_photon_emit / _emit_pass), even when a map
     // holds no photon; maps of mcrt_photon_upload and mcrt_photon_build_dev do not
     bool photon_lights = false;
+    // the identity (lpe_identity) of the LPE table the maps were emitted under, empty without one; photon_lpe_states: the
+    // maps carry each photon's reverse-DFA state (the table was one the photon mapper takes)
+    std::string photon_lpe_identity;
+    bool photon_lpe_states = false;
     // maps built on the device by mcrt_photon_emit / mcrt_octree_build; host copies are made on demand
     PhotonOctreeDevice built_dev[2];
     bool built_host_current[2] = { false, false };
@@ -142,6 +155,7 @@ struct mcrt_ctx
     const void* d_emit_flux = nullptr;
     float4* d_emit_photons[2] = { nullptr, nullptr };
     uint32_t* d_emit_lights[2] = { nullptr, nullptr };   // the emitting light of each photon of d_emit_photons
+    uint32_t* d_emit_lpe_states[2] = { nullptr, nullptr };   // ... and its reverse-DFA state (emission under an LPE table)
     unsigned long long emit_capacity[2] = { 0, 0 };
     std::vector<void*> emit_allocs;          // emission buffers (kept until the next emission / mcrt_destroy)
     unsigned long long emit_stored[2] = { 0, 0 };
@@ -827,6 +841,14 @@ namespace
             p.emit.capacity[0] = ctx->emit_capacity[0]; p.emit.capacity[1] = ctx->emit_capacity[1];
             p.emit.non_caustic_reject = (R)ctx->emit_non_caustic_reject;
             p.emit.pass = ctx->emit_pass;
+            if (ctx->d_emit_lpe_states[0])
+            {
+                p.emit.lpe_states[0] = ctx->d_emit_lpe_states[0]; p.emit.lpe_states[1] = ctx->d_emit_lpe_states[1];
+                p.emit.lpe_rev_next = ctx->d_lpe_rev_next;
+                p.emit.lpe_rev_start = ctx->lpe_rev_start;
+                p.lpe_light_symbol = ctx->d_lpe_light_symbol;
+                p.lpe_symbols = ctx->lpe_symbols;
+            }
         }
         if (integrator == MCRT_INTEGRATOR_PHOTON)
         {
@@ -837,6 +859,13 @@ namespace
             p.pm.query_capacity = knn_capacity;
             p.pm.gather_r2[0] = ctx->gather_r2[0]; p.pm.gather_r2[1] = ctx->gather_r2[1];
             if (ctx->photon_lights) { p.pm.lights[0] = ctx->built_dev[0].lights; p.pm.lights[1] = ctx->built_dev[1].lights; }
+            if (accum && accum->lpe)
+            {
+                p.pm.lpe_states[0] = ctx->built_dev[0].lpe_states; p.pm.lpe_states[1] = ctx->built_dev[1].lpe_states;
+                p.pm.lpe_join = ctx->d_lpe_join;
+                p.pm.lpe_join_any = ctx->d_lpe_join_any;
+                p.pm.lpe_rev_states = ctx->lpe_rev_states;
+            }
         }
 
         Counters init;
@@ -1157,6 +1186,9 @@ void mcrt_destroy(mcrt_ctx* ctx)
     if (ctx->d_lpe_next) cudaFree(ctx->d_lpe_next);
     if (ctx->d_lpe_accept) cudaFree(ctx->d_lpe_accept);
     if (ctx->d_lpe_light_symbol) cudaFree(ctx->d_lpe_light_symbol);
+    if (ctx->d_lpe_rev_next) cudaFree(ctx->d_lpe_rev_next);
+    if (ctx->d_lpe_join) cudaFree(ctx->d_lpe_join);
+    if (ctx->d_lpe_join_any) cudaFree(ctx->d_lpe_join_any);
     if (ctx->d_counters) cudaFree(ctx->d_counters);
     if (ctx->d_sobol_bytes) cudaFree(ctx->d_sobol_bytes);
     if (ctx->h_counters) cudaFreeHost(ctx->h_counters);
@@ -1223,6 +1255,8 @@ int mcrt_scene_upload(mcrt_ctx* ctx, const mcrt_scene_desc* scene, uint64_t* h2d
     ctx->n_light_groups = 0;
     ctx->lpe_n = 0;
     ctx->photon_lights = false;   // the maps' light indices name the lights of the previous scene
+    ctx->photon_lpe_identity.clear();
+    ctx->photon_lpe_states = false;
 
     // scene scale for the fast mode's ray offsets
     double scale = 0.0;
@@ -1313,6 +1347,8 @@ int mcrt_photon_upload(mcrt_ctx* ctx, const mcrt_photon_map_desc* caustic_map, c
     freeAll(ctx->photon_allocs);
     ctx->has_photons = false;
     ctx->photon_lights = false;
+    ctx->photon_lpe_identity.clear();
+    ctx->photon_lpe_states = false;
     uint64_t bytes = 0;
     const mcrt_photon_map_desc* maps[2] = { caustic_map, global_map };
     for (int w = 0; w < 2; w++)
@@ -1404,6 +1440,7 @@ static void freeEmission(mcrt_ctx* ctx)
     freeAll(ctx->emit_allocs);
     ctx->d_emit_offsets = nullptr; ctx->d_emit_flux = nullptr; ctx->d_emit_photons[0] = ctx->d_emit_photons[1] = nullptr;
     ctx->d_emit_lights[0] = ctx->d_emit_lights[1] = nullptr;
+    ctx->d_emit_lpe_states[0] = ctx->d_emit_lpe_states[1] = nullptr;
     ctx->emit_stored[0] = ctx->emit_stored[1] = 0;
 }
 
@@ -1420,9 +1457,10 @@ int mcrt_photon_emit_total(mcrt_ctx* ctx, const mcrt_photon_emit_params* params,
 
 // Work items [work_first, work_first + work_count) of the emission plan; light l's emissions take the reference's
 // emission indices pass * n_l + j, j < n_l (pass 0: the reference's own pass).
+// lpe: the photons also record their reverse-DFA states when an LPE table the photon mapper takes is set.
 static int emitRange(mcrt_ctx* ctx, const mcrt_photon_emit_params* params, int precision, uint32_t pass, uint64_t work_first,
                      uint64_t work_count, const float** caustic_dev, uint64_t* n_caustic, const float** global_dev, uint64_t* n_global,
-                     mcrt_stats* stats)
+                     mcrt_stats* stats, bool lpe = false)
 {
     std::vector<unsigned long long> offsets; std::vector<V4<double>> flux64; std::vector<V4<float>> flux32;
     int rc = emissionPlan(ctx, params, offsets, flux64, flux32);
@@ -1449,6 +1487,8 @@ static int emitRange(mcrt_ctx* ctx, const mcrt_photon_emit_params* params, int p
         ctx->emit_capacity[w] = 4ull * work_count + 1024;
         if ((rc = devAlloc(ctx, ctx->emit_allocs, &ctx->d_emit_photons[w], (size_t)ctx->emit_capacity[w] * 2))) { freeEmission(ctx); return rc; }
         if ((rc = devAlloc(ctx, ctx->emit_allocs, &ctx->d_emit_lights[w], (size_t)ctx->emit_capacity[w]))) { freeEmission(ctx); return rc; }
+        if (lpe && ctx->lpe_n && ctx->lpe_photon_error.empty() &&
+            (rc = devAlloc(ctx, ctx->emit_allocs, &ctx->d_emit_lpe_states[w], (size_t)ctx->emit_capacity[w]))) { freeEmission(ctx); return rc; }
     }
     ctx->d_emit_offsets = d_off; ctx->d_emit_flux = d_flux;
     ctx->emit_non_caustic_reject = 1.0 / params->caustic_factor;
@@ -1484,9 +1524,11 @@ int mcrt_photon_emit_range(mcrt_ctx* ctx, const mcrt_photon_emit_params* params,
 }
 
 // mcrt_photon_build_dev; lights_dev: null (the maps carry no light index), or the emitting light of each photon of the
-// two arrays (mcrt_photon_emit_pass), reordered with the photons
+// two arrays (mcrt_photon_emit_pass), reordered with the photons; lpe_states_dev likewise, each photon's reverse-DFA
+// state; lpe_identity: null, or the identity of the LPE table the photons were emitted under
 static int buildPhotonMaps(mcrt_ctx* ctx, const mcrt_photon_emit_params* params, const float* caustic_dev, uint64_t n_caustic,
-                           const float* global_dev, uint64_t n_global, const uint32_t* const lights_dev[2], double* build_ms)
+                           const float* global_dev, uint64_t n_global, const uint32_t* const lights_dev[2], double* build_ms,
+                           const uint32_t* const lpe_states_dev[2] = nullptr, const std::string* lpe_identity = nullptr)
 {
     if (!params || params->max_photons_per_octree_leaf == 0 || params->k_nearest_photons == 0 || params->k_nearest_photons > 1024 ||
         (n_caustic && !caustic_dev) || (n_global && !global_dev))
@@ -1500,6 +1542,8 @@ static int buildPhotonMaps(mcrt_ctx* ctx, const mcrt_photon_emit_params* params,
     freeAll(ctx->photon_allocs);
     ctx->has_photons = false;
     ctx->photon_lights = false;
+    ctx->photon_lpe_identity.clear();
+    ctx->photon_lpe_states = false;
     ctx->photon_build_ms = 0.0;
     const float4* src[2] = { reinterpret_cast<const float4*>(caustic_dev), reinterpret_cast<const float4*>(global_dev) };
     const uint64_t n[2] = { n_caustic, n_global };
@@ -1507,7 +1551,7 @@ static int buildPhotonMaps(mcrt_ctx* ctx, const mcrt_photon_emit_params* params,
     {
         const int rc = buildPhotonOctreeOnDevice(src[w], (uint32_t)n[w], params->scene_bounds, params->max_photons_per_octree_leaf,
                                                  ctx->sm_count, ctx->stream, ctx->photon_allocs, ctx->built_dev[w], ctx->error,
-                                                 lights_dev ? lights_dev[w] : nullptr);
+                                                 lights_dev ? lights_dev[w] : nullptr, lpe_states_dev ? lpe_states_dev[w] : nullptr);
         if (rc) return rc;
         ctx->photon_map[w].octants = ctx->built_dev[w].octants;
         ctx->photon_map[w].photons = ctx->built_dev[w].photons;
@@ -1520,6 +1564,8 @@ static int buildPhotonMaps(mcrt_ctx* ctx, const mcrt_photon_emit_params* params,
     ctx->has_photons = true;
     ctx->built_valid = true;
     ctx->photon_lights = lights_dev != nullptr;
+    ctx->photon_lpe_identity = lpe_identity ? *lpe_identity : std::string();
+    ctx->photon_lpe_states = lpe_states_dev != nullptr;
     if (build_ms) *build_ms = ctx->photon_build_ms;
     freeEmission(ctx);   // the raw emission buffers have been consumed (or superseded by the gathered arrays of a sharded pass)
     return MCRT_OK;
@@ -1547,12 +1593,15 @@ int mcrt_photon_emit_pass(mcrt_ctx* ctx, const mcrt_photon_emit_params* params, 
     if (rc) return rc;
     const float* raw[2] = { nullptr, nullptr };
     uint64_t n[2] = { 0, 0 };
-    if ((rc = emitRange(ctx, params, precision, pass, 0, total, &raw[0], &n[0], &raw[1], &n[1], stats))) return rc;
+    if ((rc = emitRange(ctx, params, precision, pass, 0, total, &raw[0], &n[0], &raw[1], &n[1], stats, true))) return rc;
     if (n_caustic) *n_caustic = n[0];
     if (n_global) *n_global = n[1];
     double build_ms = 0.0;
     const uint32_t* const lights[2] = { ctx->d_emit_lights[0], ctx->d_emit_lights[1] };
-    rc = buildPhotonMaps(ctx, params, raw[0], n[0], raw[1], n[1], lights, &build_ms);
+    const uint32_t* const lpe_states[2] = { ctx->d_emit_lpe_states[0], ctx->d_emit_lpe_states[1] };
+    const std::string identity = ctx->lpe_identity;   // the table the photons were emitted under
+    rc = buildPhotonMaps(ctx, params, raw[0], n[0], raw[1], n[1], lights, &build_ms, lpe_states[0] ? lpe_states : nullptr,
+                         ctx->lpe_n ? &identity : nullptr);
     freeEmission(ctx);
     if (rc) return rc;
     if (stats) stats->gpu_ms_knn = build_ms;   // emission pass: this field reports the octree build
@@ -1662,6 +1711,29 @@ int mcrt_photon_download_lights(mcrt_ctx* ctx, int which, uint32_t* out, uint64_
     }
     CK(cudaSetDevice(ctx->device));
     if (n) CK(cudaMemcpy(out, d.lights, (size_t)n * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    return MCRT_OK;
+}
+
+int mcrt_photon_download_lpe_states(mcrt_ctx* ctx, int which, uint32_t* out, uint64_t n)
+{
+    if (!ctx) return MCRT_ERR_INVALID;
+    const std::string name = "mcrt_photon_download_lpe_states";
+    if (which != 0 && which != 1) { ctx->error = name + ": invalid arguments"; return MCRT_ERR_INVALID; }
+    if (!ctx->built_valid) { ctx->error = "no maps built by mcrt_photon_emit"; return MCRT_ERR_NO_PHOTONS; }
+    if (!ctx->photon_lpe_states)
+    {
+        ctx->error = name + ": the maps carry no LPE states (only maps emitted by mcrt_photon_emit / _emit_pass under an LPE "
+                            "table the photon mapper takes do)";
+        return MCRT_ERR_UNSUPPORTED;
+    }
+    const PhotonOctreeDevice& d = ctx->built_dev[which];
+    if (n != d.n_photons || (n && !out))
+    {
+        ctx->error = name + ": n " + std::to_string(n) + ", the map has " + std::to_string(d.n_photons) + " photons";
+        return MCRT_ERR_INVALID;
+    }
+    CK(cudaSetDevice(ctx->device));
+    if (n) CK(cudaMemcpy(out, d.lpe_states, (size_t)n * sizeof(uint32_t), cudaMemcpyDeviceToHost));
     return MCRT_OK;
 }
 
@@ -1988,8 +2060,36 @@ int mcrt_set_light_path_expressions(mcrt_ctx* ctx, const char* const* exprs, uin
     CK(cudaMemcpyAsync(ctx->d_lpe_next, t.next.data(), t.next.size(), cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaMemcpyAsync(ctx->d_lpe_accept, t.accept.data(), 256 * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaMemcpyAsync(ctx->d_lpe_light_symbol, light_symbol.data(), light_symbol.size(), cudaMemcpyHostToDevice, ctx->stream));
+    if (t.photon_error.empty())
+    {
+        if (!ctx->d_lpe_rev_next)
+        {
+            CK(cudaMalloc((void**)&ctx->d_lpe_rev_next, (size_t)MCRT_LPE_MAX_STATES * MCRT_LPE_MAX_SYMBOLS));
+            CK(cudaMalloc((void**)&ctx->d_lpe_join, (size_t)MCRT_LPE_MAX_STATES * MCRT_LPE_MAX_STATES * sizeof(uint32_t)));
+            CK(cudaMalloc((void**)&ctx->d_lpe_join_any, 256));
+        }
+        CK(cudaMemcpyAsync(ctx->d_lpe_rev_next, t.rev_next.data(), t.rev_next.size(), cudaMemcpyHostToDevice, ctx->stream));
+        CK(cudaMemcpyAsync(ctx->d_lpe_join, t.join.data(), t.join.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+        CK(cudaMemcpyAsync(ctx->d_lpe_join_any, t.join_any.data(), 256, cudaMemcpyHostToDevice, ctx->stream));
+    }
     CK(cudaStreamSynchronize(ctx->stream));
     ctx->lpe_symbols = t.n_symbols;
+    ctx->lpe_rev_states = t.rev_n_states;
+    ctx->lpe_rev_start = t.rev_start;
+    ctx->lpe_photon_error = t.photon_error;
+    {
+        std::string& id = ctx->lpe_identity;
+        id.clear();
+        auto put = [&](const void* data, size_t bytes) { id.append(static_cast<const char*>(data), bytes); };
+        const uint32_t head[4] = { n, t.n_symbols, t.rev_n_states, t.rev_start };
+        put(head, sizeof(head));
+        put(t.next.data(), t.next.size());
+        put(t.accept.data(), t.accept.size() * sizeof(uint32_t));
+        put(light_symbol.data(), light_symbol.size());
+        put(t.rev_next.data(), t.rev_next.size());
+        put(t.join.data(), t.join.size() * sizeof(uint32_t));
+        put(t.photon_error.data(), t.photon_error.size());
+    }
     ctx->lpe_n = n;
     return MCRT_OK;
 }
@@ -2004,8 +2104,18 @@ int mcrt_render_accumulate_lpe_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uin
     if (!ctx->film_default) { ctx->error = name + ": LPE planes take the box film only"; return MCRT_ERR_UNSUPPORTED; }
     if (integrator_kind == MCRT_INTEGRATOR_PHOTON)
     {
-        ctx->error = name + ": the photon mapper has no light path expressions (its estimates have no event strings)";
-        return MCRT_ERR_UNSUPPORTED;
+        // a photon term's string needs the photon's own events, which only maps emitted under this table record
+        if (!ctx->has_photons || !ctx->lpe_n || ctx->photon_lpe_identity.empty() || ctx->photon_lpe_identity != ctx->lpe_identity)
+        {
+            ctx->error = name + ": the photon maps carry no LPE states for this table (only maps emitted by mcrt_photon_emit / "
+                                "_emit_pass after mcrt_set_light_path_expressions with the same expressions do)";
+            return MCRT_ERR_UNSUPPORTED;
+        }
+        if (!ctx->lpe_photon_error.empty())
+        {
+            ctx->error = name + ": the photon mapper cannot take this table: " + ctx->lpe_photon_error;
+            return MCRT_ERR_UNSUPPORTED;
+        }
     }
     if (!ctx->lpe_n) { ctx->error = name + ": no LPE table (mcrt_set_light_path_expressions)"; return MCRT_ERR_INVALID; }
     if (n_planes != ctx->lpe_n)
@@ -2403,6 +2513,28 @@ int mcrt_lpe_compile_host(const char* const* exprs, uint32_t n, uint32_t n_group
     }
     *n_states = t.n_states;
     *n_symbols = t.n_symbols;
+    return MCRT_OK;
+}
+
+int mcrt_lpe_compile_photon_host(const char* const* exprs, uint32_t n, uint32_t n_groups, uint8_t* rev_next, uint32_t* rev_start,
+                                 uint32_t* rev_n_states, uint32_t* join, char* error, uint32_t error_capacity)
+{
+    if (!rev_next || !rev_start || !rev_n_states || !join) return MCRT_ERR_INVALID;
+    LpeTable t;
+    std::string why;
+    int rc = lpeCompile(exprs, n, n_groups, t, why);
+    if (rc == MCRT_OK && !t.photon_error.empty()) { why = t.photon_error; rc = MCRT_ERR_UNSUPPORTED; }
+    if (error && error_capacity)
+    {
+        const size_t len = std::min<size_t>(why.size(), error_capacity - 1);
+        std::memcpy(error, why.data(), len);
+        error[len] = '\0';
+    }
+    if (rc != MCRT_OK) return rc;
+    std::memcpy(rev_next, t.rev_next.data(), t.rev_next.size());
+    std::memcpy(join, t.join.data(), t.join.size() * sizeof(uint32_t));
+    *rev_start = t.rev_start;
+    *rev_n_states = t.rev_n_states;
     return MCRT_OK;
 }
 

@@ -877,7 +877,7 @@ int buildBvhOnDevice(const double* prim_bounds_host, uint32_t n, const double sc
 // contained photons.
 int buildPhotonOctreeOnDevice(const float4* d_photons, uint32_t n, const double cell[6], uint32_t max_node_data, int sm_count,
                               cudaStream_t s, std::vector<void*>& keep, PhotonOctreeDevice& out, std::string& error,
-                              const uint32_t* d_lights)
+                              const uint32_t* d_lights, const uint32_t* d_lpe_states)
 {
     out = PhotonOctreeDevice();
     if (n == 0) return MCRT_OK;
@@ -917,15 +917,23 @@ int buildPhotonOctreeOnDevice(const float4* d_photons, uint32_t n, const double 
         { error = "photon octree: out of device memory"; return MCRT_ERR_CUDA; }
         keep.push_back(d_sorted_lights);
     }
+    uint32_t* d_sorted_states = nullptr;
+    if (d_lpe_states)
+    {
+        if (cudaMalloc((void**)&d_sorted_states, (size_t)n * sizeof(uint32_t)) != cudaSuccess)
+        { error = "photon octree: out of device memory"; return MCRT_ERR_CUDA; }
+        keep.push_back(d_sorted_states);
+    }
     k_emit_octants<<<(core.n_nodes + 127) / 128, 128, 0, s>>>(core.d_nodes, core.n_nodes, d_oct, d_next);
     k_gather_points<<<sm_count * 8, 256, 0, s>>>(core.d_idx, d_photons, d_sorted, n);
     if (d_lights) k_gather_lights<<<sm_count * 8, 256, 0, s>>>(core.d_idx, d_lights, d_sorted_lights, n);
+    if (d_lpe_states) k_gather_lights<<<sm_count * 8, 256, 0, s>>>(core.d_idx, d_lpe_states, d_sorted_states, n);
     BK(cudaEventRecord(ev1, s));
     BK(cudaStreamSynchronize(s));
     BK(cudaGetLastError());
     float ms = 0.f;
     BK(cudaEventElapsedTime(&ms, ev0, ev1));
-    out.octants = d_oct; out.next_sibling = d_next; out.photons = d_sorted; out.lights = d_sorted_lights;
+    out.octants = d_oct; out.next_sibling = d_next; out.photons = d_sorted; out.lights = d_sorted_lights; out.lpe_states = d_sorted_states;
     out.n_octants = core.n_nodes; out.n_photons = n; out.gpu_ms = ms; out.rounds = core.rounds;
     return MCRT_OK;
 }

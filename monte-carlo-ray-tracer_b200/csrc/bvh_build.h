@@ -29,16 +29,18 @@ namespace mcrt
         const uint32_t* next_sibling = nullptr;   // LinearOctant::next_sibling (OCTANT_NULL terminated), for downloads
         const float4* photons = nullptr;          // LinearOctree::ordered_data, 2 float4 per photon
         const uint32_t* lights = nullptr;         // the emitting light of each photon, in the same order (built with lights only)
+        const uint32_t* lpe_states = nullptr;     // the reverse-DFA state of each photon, in the same order (built with states only)
         uint32_t n_octants = 0, rounds = 0;
         uint64_t n_photons = 0;
         double gpu_ms = 0.0;
     };
 
     // d_photons: device, 2 float4 per photon as k_emit_shade stores them; cell: the root Octree box;
-    // d_lights: null, or device, the emitting light of each photon (k_emit_shade), reordered with the photons
+    // d_lights / d_lpe_states: null, or device, the emitting light / reverse-DFA state of each photon (k_emit_shade),
+    // reordered with the photons
     int buildPhotonOctreeOnDevice(const float4* d_photons, uint32_t n_photons, const double cell[6], uint32_t max_node_data,
                                   int sm_count, cudaStream_t stream, std::vector<void*>& keep, PhotonOctreeDevice& out,
-                                  std::string& error, const uint32_t* d_lights = nullptr);
+                                  std::string& error, const uint32_t* d_lights = nullptr, const uint32_t* d_lpe_states = nullptr);
 
     // type: MCRT_BVH_*; returns an mcrt_status code, message in `error`
     int buildBvhOnDevice(const double* prim_bounds_host, uint32_t n_prims, const double scene_bounds[6], int type,

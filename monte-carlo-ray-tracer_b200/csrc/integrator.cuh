@@ -225,6 +225,11 @@ namespace mcrt
         unsigned long long capacity[2];
         R non_caustic_reject;                    // 1 / caustic_factor
         uint32_t pass;                           // emissions of light l take the indices pass * n_l + j (mcrt_photon_emit_pass)
+        // k_emit_*<R, true> (an LPE table is set): the reversed expressions' DFA (lpe.h; symbols of WaveParams::lpe_*),
+        // its start state, and the output, the state of each photon before its storage vertex's event
+        const uint8_t* lpe_rev_next;
+        uint32_t lpe_rev_start;
+        uint32_t* lpe_states[2];
     };
 
     template <class R> struct WaveParams
@@ -855,13 +860,20 @@ namespace mcrt
                                 do_direct = false; do_bsdf = false; alive = false;
                             }
                         }
+                        // a dead path, or one whose every photon term no expression accepts, queries no map (its
+                        // estimates would land in no plane), as a zero mask traces no shadow ray
+                        if constexpr (FILM == FILM_MODE_LPE)
+                            if (lpe_state == MCRT_LPE_DEAD || !__ldg(&p.pm.lpe_join_any[lpe_state])) want_knn = 0;
                         if (want_knn)
                         {
                             knn_q.pos_n1 = V4<R>(ia.position, ia.n1);
                             knn_q.nrm_n2 = V4<R>(ia.shading_cs.c2, ia.n2);
                             knn_q.out_rf = V4<R>(ia.out, ia.Rf);
                             knn_q.weight_t = V4<R>(throughput, ia.T);
-                            knn_q.meta = make_uint4(ps.material, film_index, ia.inside ? 1u : 0u, meta.y);
+                            // FILM_MODE_LPE: the forward state after x's event in bits 16-23 (k_knn / k_gather join it
+                            // with each photon's)
+                            knn_q.meta = make_uint4(ps.material, film_index, (ia.inside ? 1u : 0u) |
+                                                                             (FILM == FILM_MODE_LPE ? lpe_state << 16 : 0u), meta.y);
                         }
                     }
 
@@ -1285,6 +1297,57 @@ namespace mcrt
         if (g != NO_PRIM) { run = g; run_sum += term; }
     }
 
+    // The LPE split of a photon estimate (FILM_MODE_LPE of k_knn / k_gather): groupRunStep / depositGroupRuns with runs
+    // keyed by the photon's accept mask, join[query state][photon state], and a run's sum deposited into every plane of
+    // its mask. Every 32-bit value is a mask, so `has` marks a run; a mask of 0 starts none, so its photon adds nothing.
+    template <class R, class Scale>
+    MCRT_D void depositMaskRuns(const WaveParams<R>& p, uint32_t film_index, bool has, uint32_t mask, const V3<R>& sum,
+                                const V3<R>& weight, Scale&& scale)
+    {
+        const unsigned lane = threadIdx.x & 31u;
+        unsigned pending = __ballot_sync(0xFFFFFFFFu, has);
+        while (pending)
+        {
+            const int leader = __ffs(pending) - 1;
+            const uint32_t g = __shfl_sync(0xFFFFFFFFu, mask, leader);
+            const bool mine = has && mask == g;
+            V3<R> v = mine ? sum : V3<R>(R(0));
+            for (int off = 16; off > 0; off >>= 1)
+            {
+                v.x += __shfl_xor_sync(0xFFFFFFFFu, v.x, off);
+                v.y += __shfl_xor_sync(0xFFFFFFFFu, v.y, off);
+                v.z += __shfl_xor_sync(0xFFFFFFFFu, v.z, off);
+            }
+            if ((int)lane == leader)
+            {
+                const V3<R> d = scale(v) * weight;
+                for (uint32_t m = g; m; m &= m - 1u) filmAddV(p.film + (uint32_t)(__ffs(m) - 1) * p.plane_values, film_index, d);
+            }
+            pending &= ~__ballot_sync(0xFFFFFFFFu, mine);
+        }
+    }
+
+    template <class R, class Scale>
+    MCRT_D void maskRunStep(const WaveParams<R>& p, uint32_t film_index, const V3<R>& weight, Scale&& scale, uint32_t mask,
+                            const V3<R>& term, bool& run_has, uint32_t& run, V3<R>& run_sum)
+    {
+        const bool flush = mask != 0u && run_has && mask != run;
+        if (__any_sync(0xFFFFFFFFu, flush))
+        {
+            depositMaskRuns(p, film_index, flush, run, run_sum, weight, scale);
+            if (flush) { run_has = false; run_sum = V3<R>(R(0)); }
+        }
+        if (mask != 0u) { run_has = true; run = mask; run_sum += term; }
+    }
+
+    // accept mask of a photon term: the query's forward state (KnnQuery::meta.z bits 16-23) joined with the photon's
+    template <class R>
+    MCRT_D uint32_t lpePhotonMask(const WaveParams<R>& p, uint32_t query_state, uint32_t which, unsigned long long idx)
+    {
+        const uint32_t r = __ldg(&p.pm.lpe_states[which][idx]);
+        return r == MCRT_LPE_DEAD ? 0u : __ldg(&p.pm.lpe_join[query_state * p.pm.lpe_rev_states + r]);
+    }
+
     // ------------------------------------------------------------------------------------------
     // k_knn: one warp per photon-map query emitted by k_shade<R,1>; search + radiance estimate.
     // FILM_MODE_GROUPS splits the estimate by the light group of each photon (depositGroupRuns); FILM_MODE_AOV deposits
@@ -1337,6 +1400,33 @@ namespace mcrt
                     groupRunStep(p, qr.meta.y, weight, scale, g, term, run, run_sum);
                 }
                 depositGroupRuns(p, qr.meta.y, run, run_sum, weight, scale);
+                __syncwarp();
+                continue;
+            }
+            if constexpr (FILM == FILM_MODE_LPE)
+            {
+                const auto scale = [&](const V3<R>& v) { return which == 0 ? R(3) * v * inv_max_r2 * Consts<R>::INV_PI : v / (top_d2 * Consts<R>::PI); };
+                const V3<R> weight = qr.weight_t.xyz();
+                const uint32_t state = (qr.meta.z >> 16) & 0xFFu;
+                bool run_has = false;
+                uint32_t run = 0;
+                V3<R> run_sum(R(0));
+                for (uint32_t base = 0; base < found; base += 32)
+                {
+                    const uint32_t s = base + lane;
+                    uint32_t mask = 0;
+                    V3<R> term(R(0));
+                    if (s < found)
+                    {
+                        const uint32_t idx = sh.res_idx[s];
+                        mask = lpePhotonMask(p, state, which, idx);
+                        const float4 a = __ldg(&map.photons[2 * (size_t)idx]);
+                        const float4 b = __ldg(&map.photons[2 * (size_t)idx + 1]);
+                        if (!photonTerm(ia, which, a, b, (R)sh.res_d2[s], inv_max_r2, term)) term = V3<R>(R(0));
+                    }
+                    maskRunStep(p, qr.meta.y, weight, scale, mask, term, run_has, run, run_sum);
+                }
+                depositMaskRuns(p, qr.meta.y, run_has, run, run_sum, weight, scale);
                 __syncwarp();
                 continue;
             }
@@ -1456,6 +1546,29 @@ namespace mcrt
                 __syncwarp();
                 continue;
             }
+            if constexpr (FILM == FILM_MODE_LPE)
+            {
+                const auto scale = [&](const V3<R>& v) { return which == 0 ? R(3) * v * inv_r2 * Consts<R>::INV_PI : v / ((R)r2 * Consts<R>::PI); };
+                const V3<R> weight = qr.weight_t.xyz();
+                const uint32_t state = (qr.meta.z >> 16) & 0xFFu;
+                uint32_t mask = 0, run = 0;   // mask: the accept mask of this lane's photon of the current step
+                bool run_has = false;
+                V3<R> term(R(0)), run_sum(R(0));
+                gatherWarp(p.pm.map[which], (double)qr.pos_n1.x, (double)qr.pos_n1.y, (double)qr.pos_n1.z, r2, stack, &overflow,
+                           [&](unsigned long long idx, double d2, const float4& a, const float4& b)
+                           {
+                               mask = lpePhotonMask(p, state, which, idx);
+                               if (!photonTerm(ia, which, a, b, (R)d2, inv_r2, term)) term = V3<R>(R(0));
+                           },
+                           [&]
+                           {
+                               maskRunStep(p, qr.meta.y, weight, scale, mask, term, run_has, run, run_sum);
+                               mask = 0;
+                           });
+                depositMaskRuns(p, qr.meta.y, run_has, run, run_sum, weight, scale);
+                __syncwarp();
+                continue;
+            }
             V3<R> sum(R(0));
             bool found = false;
             gatherWarp(p.pm.map[which], (double)qr.pos_n1.x, (double)qr.pos_n1.y, (double)qr.pos_n1.z, r2, stack, &overflow,
@@ -1501,7 +1614,10 @@ namespace mcrt
     // Photon emission pass on the device (SURVEY.md §8f-1). Same wavefront as the camera paths:
     // k_emit_generate -> [sort] -> k_extend -> k_emit_shade -> ... ; photons are appended to the
     // caustic / global arrays with one atomic per warp per array.
-    template <class R>
+    // LPE (an LPE table is set): the path carries its reverse-DFA state in bits 16-23 of meta2.y, as camera paths carry
+    // theirs; every photon is traced and stored as without it, whatever its state, since it counts for the radius of
+    // every estimate near it.
+    template <class R, bool LPE>
     __global__ void __launch_bounds__(256) k_emit_generate(WaveParams<R> p, int next)
     {
         Counters* c = p.counters;
@@ -1543,7 +1659,11 @@ namespace mcrt
                 out.ray_d[slot] = V4<R>(dir, R(1));
                 out.thr[slot] = V4<R>(flux.x, flux.y, flux.z, R(0));
                 out.meta[slot] = make_uint4(light, index, 0u, 0u);
-                out.meta2[slot] = make_uint4(NO_PRIM, 1u, 0u, sc.lights[light].type == PRIM_TRIANGLE ? sc.lights[light].prim : NO_PRIM);
+                uint32_t lpe_state = 0;
+                if constexpr (LPE)
+                    lpe_state = p.emit.lpe_rev_start == MCRT_LPE_DEAD ? (uint32_t)MCRT_LPE_DEAD
+                              : (uint32_t)__ldg(&p.emit.lpe_rev_next[p.emit.lpe_rev_start * p.lpe_symbols + lpeLightSymbol(p, light)]);
+                out.meta2[slot] = make_uint4(NO_PRIM, 1u | (lpe_state << 16), 0u, sc.lights[light].type == PRIM_TRIANGLE ? sc.lights[light].prim : NO_PRIM);
                 if (p.sort.path_order) key = rayKey(p.sort, pos, dir, sc.lights[light].prim);
             }
             if (p.sort.path_order)
@@ -1563,7 +1683,7 @@ namespace mcrt
         arr[2 * idx + 1] = make_float4((float)pos.y, (float)pos.z, phi, theta);
     }
 
-    template <class R>
+    template <class R, bool LPE>
     __global__ void __launch_bounds__(128, MCRT_SHADE_MINBLOCKS) k_emit_shade(WaveParams<R> p, int cur)
     {
         __shared__ SobolByteTables sobol_tab;
@@ -1588,11 +1708,14 @@ namespace mcrt
             uint4 meta, meta2;
             uint32_t ior_count = 1, hit_prim = NO_PRIM;
             R iors[IOR_STACK_CAPACITY];
+            // LPE: the state before this vertex's event (stored with its photon) and after it (for the next bounce)
+            uint32_t lpe_state = 0, lpe_next = 0;
 
             if (alive)
             {
                 const V4<R> ro = ldStream(&in.ray_o[i]), rd = ldStream(&in.ray_d[i]), th = ldStream(&in.thr[i]), hv = ldStream(&p.hits[i]);
                 meta = ldStream(&in.meta[i]); meta2 = ldStream(&in.meta2[i]);
+                if constexpr (LPE) lpe_state = (meta2.y >> 16) & 0xFFu;
                 ray.start = ro.xyz(); ray.medium_ior = ro.w;
                 ray.direction = rd.xyz(); ray.refraction_scale = rd.w;
                 flux = th.xyz();
@@ -1627,6 +1750,9 @@ namespace mcrt
                     Interaction<R> ia;
                     buildInteraction(ia, sc, hit, ray, iors[ext_idx], smp);
                     const Material<R>& m = *ia.material;
+                    if constexpr (LPE)
+                        lpe_next = lpe_state == MCRT_LPE_DEAD ? (uint32_t)MCRT_LPE_DEAD
+                                 : (uint32_t)__ldg(&p.emit.lpe_rev_next[lpe_state * p.lpe_symbols + lpeVertexSymbol(ia.type, ia.dirac_delta)]);
 
                     // photon-mapper.cpp:245-256: store only where non-delta interactions are possible
                     if (!(m.flags & MAT_DIRAC_DELTA))
@@ -1695,6 +1821,7 @@ namespace mcrt
                                         V3<double>((double)ph_pos.x, (double)ph_pos.y, (double)ph_pos.z),
                                         V3<double>((double)ph_dir.x, (double)ph_dir.y, (double)ph_dir.z));
                             p.emit.lights[which][idx] = meta.x;   // the light k_emit_generate emitted the path from
+                            if constexpr (LPE) p.emit.lpe_states[which][idx] = lpe_state;
                         }
                         else c->photon_overflow = 1u;
                     }
@@ -1719,7 +1846,7 @@ namespace mcrt
                     if (ior_count > 5) out.iors_b[slot] = V4<R>(iors[5], iors[6], iors[7], R(0));
                 }
                 out.meta[slot] = make_uint4(meta.x, meta.y, (nray.depth & 0xFFFFu) | (nray.diffuse_depth << 16), (uint32_t)nray.refraction_level);
-                out.meta2[slot] = make_uint4(NO_PRIM, ior_count | (nray.dirac_delta ? 256u : 0u), 0u,
+                out.meta2[slot] = make_uint4(NO_PRIM, ior_count | (nray.dirac_delta ? 256u : 0u) | (lpe_next << 16), 0u,
                                              sc.shade[hit_prim].type == PRIM_TRIANGLE ? hit_prim : NO_PRIM);
                 if (sorting) { p.sort.path_key[cur ^ 1][slot] = pkey; p.sort.path_rank[cur ^ 1][slot] = prank; }
             }

@@ -65,6 +65,11 @@ namespace mcrt
     {
         const bool lite = (p.scene.material_flags_any & ~SHADE_FEATS_LITE) == 0;
         if (!p.filmp.is_default_box) k_shade<MCRT_REAL, 1, FILM_MODE_SPLAT, SHADE_FEATS_ALL><<<grid * 2, 128, 0, s>>>(p, cur);
+        else if (p.n_planes && p.lpe_next)
+        {
+            if (lite) k_shade<MCRT_REAL, 1, FILM_MODE_LPE, SHADE_FEATS_LITE><<<grid * 2, 128, 0, s>>>(p, cur);
+            else k_shade<MCRT_REAL, 1, FILM_MODE_LPE, SHADE_FEATS_ALL><<<grid * 2, 128, 0, s>>>(p, cur);
+        }
         else if (p.n_planes && p.aovs)
         {
             // photon-mapper components: FILM_MODE_AOV deposits into the plane each site names (MCRT_PM_*)
@@ -87,6 +92,11 @@ namespace mcrt
             // fixed-radius gather (mcrt_photon_gather_radius) in place of the k-NN estimate
             const bool lite = (p.scene.material_flags_any & ~SHADE_FEATS_LITE) == 0;
             if (!p.filmp.is_default_box) k_gather<MCRT_REAL, FILM_MODE_SPLAT, SHADE_FEATS_ALL><<<g, b, 0, s>>>(p);
+            else if (p.n_planes && p.lpe_next)
+            {
+                if (lite) k_gather<MCRT_REAL, FILM_MODE_LPE, SHADE_FEATS_LITE><<<g, b, 0, s>>>(p);
+                else k_gather<MCRT_REAL, FILM_MODE_LPE, SHADE_FEATS_ALL><<<g, b, 0, s>>>(p);
+            }
             else if (p.n_planes && p.aovs)
             {
                 if (lite) k_gather<MCRT_REAL, FILM_MODE_AOV, SHADE_FEATS_LITE><<<g, b, 0, s>>>(p);
@@ -113,8 +123,9 @@ namespace mcrt
             return;
         }
         const bool lite = (p.scene.material_flags_any & ~SHADE_FEATS_LITE) == 0;
-        // film mode of the box film: one plane, light-group planes, or the photon mapper's component planes (FILM_MODE_AOV)
-        const int film_mode = !p.n_planes ? FILM_MODE_BOX : (p.aovs ? FILM_MODE_AOV : FILM_MODE_GROUPS);
+        // film mode of the box film: one plane, light-group planes, the photon mapper's component planes (FILM_MODE_AOV)
+        // or LPE planes
+        const int film_mode = !p.n_planes ? FILM_MODE_BOX : (p.lpe_next ? FILM_MODE_LPE : (p.aovs ? FILM_MODE_AOV : FILM_MODE_GROUPS));
         const int slots = knnSlotsFor(p.pm.k_nearest);
         // k > 672 needs more than the default 48 KB of dynamic shared memory (knnSharedBytes)
         #define MCRT_KNN_LAUNCH2(SL, FM, FE) \
@@ -124,6 +135,7 @@ namespace mcrt
         #define MCRT_KNN_LAUNCH1(SL, FE) \
             do { if (film_mode == FILM_MODE_GROUPS) MCRT_KNN_LAUNCH2(SL, FILM_MODE_GROUPS, FE); \
                  else if (film_mode == FILM_MODE_AOV) MCRT_KNN_LAUNCH2(SL, FILM_MODE_AOV, FE); \
+                 else if (film_mode == FILM_MODE_LPE) MCRT_KNN_LAUNCH2(SL, FILM_MODE_LPE, FE); \
                  else MCRT_KNN_LAUNCH2(SL, FILM_MODE_BOX, FE); } while (0)
         #define MCRT_KNN_LAUNCH(SL) \
             do { if (lite) MCRT_KNN_LAUNCH1(SL, SHADE_FEATS_LITE); else MCRT_KNN_LAUNCH1(SL, SHADE_FEATS_ALL); } while (0)
@@ -186,11 +198,13 @@ namespace mcrt
     }
     template <> void Launch<MCRT_REAL>::emitGenerate(const WaveParams<MCRT_REAL>& p, int next, int grid, cudaStream_t s)
     {
-        k_emit_generate<MCRT_REAL><<<grid, 256, 0, s>>>(p, next);
+        if (p.emit.lpe_states[0]) k_emit_generate<MCRT_REAL, true><<<grid, 256, 0, s>>>(p, next);
+        else k_emit_generate<MCRT_REAL, false><<<grid, 256, 0, s>>>(p, next);
     }
     template <> void Launch<MCRT_REAL>::emitShade(const WaveParams<MCRT_REAL>& p, int cur, int grid, cudaStream_t s)
     {
-        k_emit_shade<MCRT_REAL><<<grid * 2, 128, 0, s>>>(p, cur);
+        if (p.emit.lpe_states[0]) k_emit_shade<MCRT_REAL, true><<<grid * 2, 128, 0, s>>>(p, cur);
+        else k_emit_shade<MCRT_REAL, false><<<grid * 2, 128, 0, s>>>(p, cur);
     }
     template <> void Launch<MCRT_REAL>::traceUser(const DeviceScene<MCRT_REAL>& sc, const double* rays6, size_t n,
                                                   double* out_tuv, uint32_t* out_prim, Counters* c, int grid, cudaStream_t s)

@@ -333,6 +333,177 @@ namespace mcrt
         std::string quoted(const char* s) { return std::string("\"") + s + "\""; }
     }
 
+    // The photon side of the table (lpe.h): the DFA of the reversed expressions, read in emission order, and the join of
+    // its states with the forward table's. Fills out.rev_* / join / join_any; returns "" or why the photon mapper must
+    // refuse the table (the forward table stays valid for the path tracer).
+    static std::string compileReverse(const Nfa& nfa, const std::vector<std::pair<int, int>>& ends, uint32_t n_symbols,
+                                      LpeTable& out)
+    {
+        const size_t nq = nfa.eps.size();
+        std::vector<std::vector<int>> reps(nq), rin(nq);   // reversed epsilon and symbol edges
+        for (size_t q = 0; q < nq; q++)
+        {
+            for (int r : nfa.eps[q]) reps[r].push_back((int)q);
+            if (nfa.out[q] >= 0) rin[nfa.out[q]].push_back((int)q);
+        }
+        std::vector<uint32_t> first_of(nq, 0);   // reversed, an expression accepts at its own start
+        for (size_t i = 0; i < ends.size(); i++) first_of[ends[i].first] |= 1u << i;
+
+        // subset construction over the device symbols and C (column n_symbols), from the expressions' accepting states
+        const uint32_t cols = n_symbols + 1;
+        std::map<std::vector<int>, uint32_t> index;
+        std::vector<std::vector<int>> sets;
+        std::vector<uint32_t> dfa_next, dfa_accept;
+        std::vector<uint8_t> mark(nq, 0);
+        uint64_t steps = 0;
+        auto intern = [&](std::vector<int>& set) -> uint32_t
+        {
+            std::vector<int> stack(set);
+            for (int q : set) mark[q] = 1;
+            while (!stack.empty())
+            {
+                const int q = stack.back();
+                stack.pop_back();
+                for (int r : reps[q])
+                    if (!mark[r]) { mark[r] = 1; set.push_back(r); stack.push_back(r); }
+            }
+            for (int q : set) mark[q] = 0;
+            std::sort(set.begin(), set.end());
+            steps += set.size();
+            auto it = index.find(set);
+            if (it != index.end()) return it->second;
+            const uint32_t id = (uint32_t)sets.size();
+            uint32_t acc = 0;
+            for (int q : set) acc |= first_of[q];
+            index.emplace(set, id);
+            sets.push_back(set);
+            dfa_accept.push_back(acc);
+            dfa_next.resize(dfa_next.size() + cols, 0);
+            return id;
+        };
+        {
+            std::vector<int> s0;
+            for (const auto& e : ends) s0.push_back(e.second);
+            std::sort(s0.begin(), s0.end());
+            s0.erase(std::unique(s0.begin(), s0.end()), s0.end());
+            intern(s0);
+        }
+        for (uint32_t d = 0; d < sets.size(); d++)
+        {
+            if (sets.size() > MAX_DFA_STATES)
+                return "the reversed expressions need more than " + std::to_string(MAX_DFA_STATES) + " automaton states";
+            for (uint32_t col = 0; col < cols; col++)
+            {
+                steps += sets[d].size();
+                if (steps > MAX_SUBSET_WORK)
+                    return "the reversed expressions' automaton is too large to build (more than " + std::to_string(MAX_SUBSET_WORK) +
+                           " subset-construction steps)";
+                const uint32_t sym = col < n_symbols ? col : SYM_C;
+                std::vector<int> moved;
+                for (int q : sets[d])
+                    for (int p : rin[q])
+                        if (nfa.on[p].test(sym)) moved.push_back(p);
+                std::sort(moved.begin(), moved.end());
+                moved.erase(std::unique(moved.begin(), moved.end()), moved.end());
+                const uint32_t t = intern(moved);
+                dfa_next[(size_t)d * cols + col] = t;
+            }
+        }
+
+        // A string's C comes first and only once, so a photon history is complete once C is read after it: a state's
+        // mask is the accept mask after C. Live: a state from which device symbols lead to a nonzero mask.
+        const uint32_t nd = (uint32_t)sets.size();
+        std::vector<uint32_t> mask_c(nd);
+        for (uint32_t d = 0; d < nd; d++) mask_c[d] = dfa_accept[dfa_next[(size_t)d * cols + n_symbols]];
+        std::vector<std::vector<uint32_t>> pred(nd);
+        for (uint32_t d = 0; d < nd; d++)
+            for (uint32_t col = 0; col < n_symbols; col++) pred[dfa_next[(size_t)d * cols + col]].push_back(d);
+        std::vector<uint8_t> live(nd, 0);
+        std::vector<uint32_t> work;
+        for (uint32_t d = 0; d < nd; d++) if (mask_c[d]) { live[d] = 1; work.push_back(d); }
+        while (!work.empty())
+        {
+            const uint32_t d = work.back();
+            work.pop_back();
+            for (uint32_t p : pred[d]) if (!live[p]) { live[p] = 1; work.push_back(p); }
+        }
+
+        // Moore's refinement of the live states, by mask after C and device-symbol transitions
+        std::vector<uint32_t> cls(nd, UINT32_MAX);
+        size_t n_cls = 0;
+        {
+            std::map<uint32_t, uint32_t> by_mask;
+            for (uint32_t d = 0; d < nd; d++)
+                if (live[d]) cls[d] = by_mask.emplace(mask_c[d], (uint32_t)by_mask.size()).first->second;
+            n_cls = by_mask.size();
+            std::vector<uint32_t> sig(n_symbols + 1);
+            for (;;)
+            {
+                std::map<std::vector<uint32_t>, uint32_t> by_sig;
+                std::vector<uint32_t> refined(nd, UINT32_MAX);
+                for (uint32_t d = 0; d < nd; d++)
+                {
+                    if (!live[d]) continue;
+                    sig[0] = cls[d];
+                    for (uint32_t col = 0; col < n_symbols; col++) sig[col + 1] = cls[dfa_next[(size_t)d * cols + col]];
+                    refined[d] = by_sig.emplace(sig, (uint32_t)by_sig.size()).first->second;
+                }
+                const bool stable = by_sig.size() == n_cls;
+                cls.swap(refined);
+                n_cls = by_sig.size();
+                if (stable) break;
+            }
+        }
+
+        // breadth-first numbering from the start (no photon event read yet); each class keeps the shortest history
+        // that reaches it, as its parent class and last symbol
+        std::vector<uint32_t> number(n_cls, MCRT_LPE_DEAD), order, parent, via;
+        if (live[0]) { number[cls[0]] = 0; order.push_back(0); parent.push_back(MCRT_LPE_DEAD); via.push_back(0); }
+        for (size_t k = 0; k < order.size(); k++)
+            for (uint32_t col = 0; col < n_symbols; col++)
+            {
+                const uint32_t t = dfa_next[(size_t)order[k] * cols + col];
+                if (!live[t] || number[cls[t]] != MCRT_LPE_DEAD) continue;
+                if (order.size() >= MCRT_LPE_MAX_STATES)
+                    return "the reversed expressions need more than " + std::to_string(MCRT_LPE_MAX_STATES) +
+                           " live automaton states (a photon's state keeps 8 bits)";
+                number[cls[t]] = (uint32_t)order.size();
+                order.push_back(t);
+                parent.push_back((uint32_t)k);
+                via.push_back(col);
+            }
+
+        out.rev_n_states = order.empty() ? 1u : (uint32_t)order.size();
+        out.rev_start = order.empty() ? (uint32_t)MCRT_LPE_DEAD : 0u;
+        out.rev_next.assign((size_t)out.rev_n_states * n_symbols, (uint8_t)MCRT_LPE_DEAD);
+        for (uint32_t k = 0; k < order.size(); k++)
+            for (uint32_t col = 0; col < n_symbols; col++)
+            {
+                const uint32_t t = dfa_next[(size_t)order[k] * cols + col];
+                out.rev_next[(size_t)k * n_symbols + col] = (uint8_t)(live[t] ? number[cls[t]] : MCRT_LPE_DEAD);
+            }
+
+        // join[s][r]: the forward table from s over r's representative history, read backwards (the string's order).
+        // Histories that reach one reverse state match after the same camera prefixes, so any representative will do.
+        out.join.assign((size_t)out.n_states * out.rev_n_states, 0u);
+        out.join_any.assign(256, 0u);
+        std::vector<uint32_t> history;
+        for (uint32_t r = 0; r < order.size(); r++)
+        {
+            history.clear();
+            for (uint32_t k = r; k != 0; k = parent[k]) history.push_back(via[k]);   // last event first
+            for (uint32_t s = 0; s < out.n_states; s++)
+            {
+                uint32_t f = s;
+                for (size_t k = 0; k < history.size() && f != MCRT_LPE_DEAD; k++) f = out.next[(size_t)f * n_symbols + history[k]];
+                const uint32_t m = f == MCRT_LPE_DEAD ? 0u : out.accept[f];
+                out.join[(size_t)s * out.rev_n_states + r] = m;
+                if (m) out.join_any[s] = 1u;
+            }
+        }
+        return std::string();
+    }
+
     // lpeCompile without its exception guard
     static int compile(const char* const* exprs, uint32_t n, uint32_t n_groups, LpeTable& out, std::string& error)
     {
@@ -405,12 +576,14 @@ namespace mcrt
             nfa.leaf_sets[id] = s;
         }
         int start;
+        std::vector<std::pair<int, int>> ends(n);   // each expression's own start and accepting NFA state
         try
         {
             start = nfa.state();
             for (uint32_t i = 0; i < n; i++)
             {
                 const std::pair<int, int> f = nfa.build(nodes, roots[i]);
+                ends[i] = f;
                 nfa.eps[start].push_back(f.first);
                 nfa.accept[f.second] |= 1u << i;
             }
@@ -552,6 +725,12 @@ namespace mcrt
             }
         }
         out.labels = labels;
+        out.photon_error = compileReverse(nfa, ends, n_symbols, out);
+        if (!out.photon_error.empty())
+        {
+            out.rev_n_states = 0; out.rev_start = MCRT_LPE_DEAD;
+            out.rev_next.clear(); out.join.clear(); out.join_any.clear();
+        }
         return MCRT_OK;
     }
 

@@ -18,11 +18,24 @@ namespace mcrt
         std::vector<uint8_t> next;
         std::vector<uint32_t> accept;   // [256]
         std::vector<uint32_t> labels;
+        // The photon mapper's side. A photon's events are read in emission order, its light's symbol first, by the DFA
+        // of the reversed expressions: rev_next[r * n_symbols + symbol] (MCRT_LPE_DEAD once no camera prefix can make
+        // the history match), starting at rev_start (MCRT_LPE_DEAD when nothing can match). A contribution whose camera
+        // prefix ends in forward state s and whose photon history ends in reverse state r matches the expressions of
+        // join[s * rev_n_states + r]; join_any[s] (256 entries) is 1 when some history completes s. photon_error is
+        // non-empty, and the rest empty, when the reversed expressions exceed the limits: the photon mapper refuses the
+        // table, the path tracer still takes it.
+        uint32_t rev_n_states = 0, rev_start = 0;
+        std::vector<uint8_t> rev_next;
+        std::vector<uint32_t> join;
+        std::vector<uint8_t> join_any;
+        std::string photon_error;
     };
 
     // Parses, builds the Thompson NFA of each expression and the subset-construction DFA of their union, collapses the
-    // states from which nothing is accepted into MCRT_LPE_DEAD and numbers the others breadth-first from state 0.
-    // Labels must be below n_groups. Returns MCRT_OK, MCRT_ERR_INVALID (syntax, counts, labels) or
-    // MCRT_ERR_UNSUPPORTED (more than MCRT_LPE_MAX_STATES live states), with the reason in error.
+    // states from which nothing is accepted into MCRT_LPE_DEAD and numbers the others breadth-first from state 0; then
+    // the same for the reversed expressions and the join of the two (photon side, above). Labels must be below
+    // n_groups. Returns MCRT_OK, MCRT_ERR_INVALID (syntax, counts, labels) or MCRT_ERR_UNSUPPORTED (more than
+    // MCRT_LPE_MAX_STATES live forward states), with the reason in error.
     int lpeCompile(const char* const* exprs, uint32_t n, uint32_t n_groups, LpeTable& out, std::string& error);
 }

@@ -59,6 +59,13 @@ namespace mcrt
         // per map, the index of the light that emitted each photon, in map order (maps emitted on the device; read by the
         // light-group estimates only). Kept out of DevicePhotonMap so that the search kernels' parameters keep their layout.
         const uint32_t* lights[2];
+        // FILM_MODE_LPE: per map, the reverse-DFA state of each photon in map order (lpe_states), and the join of the
+        // forward states with those states, [forward][lpe_rev_states] accept masks; lpe_join_any[s]: some photon history
+        // completes forward state s, so k_shade queries the maps there (lpe.h)
+        const uint32_t* lpe_states[2];
+        const uint32_t* lpe_join;
+        const uint8_t* lpe_join_any;
+        uint32_t lpe_rev_states;
     };
 
     MCRT_D double octantDistance2(const DeviceOctant& o, double px, double py, double pz)
