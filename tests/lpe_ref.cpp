@@ -12,14 +12,17 @@
 namespace
 {
     // One character per event: the camera 'C', the vertex events 'a' <RD>, 'b' <RS>, 'c' <RG>, 'd' <TS>, 'e' <TG>, the
-    // sky 'B', an emitter of light group g chr('0' + g), an emitter without a group (not a listed light, or a light the
-    // caller's table leaves out) '*'
+    // sky 'B', an emitter of light group g the byte 0x80 + g (read as latin-1, so no group collides with another event
+    // or with a character of Python's re), an emitter without a group (not a listed light, or a light the caller's table
+    // leaves out) '*'
     char vertexChar(const Interaction& ia)
     {
         if (ia.type == DIFFUSE) return 'a';
         if (ia.type == REFLECT) return ia.dirac_delta ? 'b' : 'c';
         return ia.dirac_delta ? 'd' : 'e';
     }
+
+    char groupChar(uint32_t g) { return (char)(0x80u + g); }
 
     struct LpeStrings
     {
@@ -104,7 +107,7 @@ extern "C"
 {
 
 // The per-pixel means (over the sqrtspp^2 samples) of the contributions of each distinct event string of rows [y0, y1).
-// group_of_light[n_lights]: light l (the scene's l-th light_prim) is in group group_of_light[l] (< 78); NULL: no groups.
+// group_of_light[n_lights]: light l (the scene's l-th light_prim) is in group group_of_light[l] (< 128); NULL: no groups.
 // -> a handle for oracle_lpe_sizes / oracle_lpe_get / oracle_lpe_free.
 void* oracle_lpe_render(void* h, const mcrt_camera* cam, uint32_t y0, uint32_t y1, uint32_t sqrtspp, uint32_t seed,
                         const uint32_t* group_of_light, uint32_t n_lights)
@@ -112,7 +115,7 @@ void* oracle_lpe_render(void* h, const mcrt_camera* cam, uint32_t y0, uint32_t y
     const Scene& s = *static_cast<Scene*>(h);
     Labels label;
     if (group_of_light)
-        for (uint32_t l = 0; l < n_lights && l < s.light_prim.size(); l++) label.of_prim[s.light_prim[l]] = (char)('0' + group_of_light[l]);
+        for (uint32_t l = 0; l < n_lights && l < s.light_prim.size(); l++) label.of_prim[s.light_prim[l]] = groupChar(group_of_light[l]);
     auto* out = new LpeStrings();
     out->pixels.resize((size_t)(y1 - y0) * cam->width);
     Sampler smp(seed);

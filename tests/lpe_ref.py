@@ -18,7 +18,14 @@ SOURCES = [os.path.join(HERE, "lpe_ref.cpp"), os.path.join(ROOT, "oracle", "mcrt
 # the restatement's characters of the vertex events (tests/lpe_ref.cpp)
 VERTEX = {"RD": "a", "RS": "b", "RG": "c", "TS": "d", "TG": "e"}
 UNGROUPED = "*"
+# the strings' bytes are read as latin-1: the character of light group g is chr(0x80 + g), which collides with no
+# other event and with no character of Python's re
+ENCODING = "latin-1"
 _lib = None
+
+
+def group_char(g):
+    return chr(0x80 + int(g))
 
 
 def lib():
@@ -94,7 +101,7 @@ def render_strings(scene, camera, y0, y1, sqrtspp, seed, group_of_light=None):
             chars = C.create_string_buffer(max(c.value, 1))
             L.oracle_lpe_get(handle, pixel.ctypes.data_as(C.c_void_p), string.ctypes.data_as(C.c_void_p),
                              value.ctypes.data_as(C.c_void_p), chars)
-            strings = chars.raw[:c.value].decode().split("\0")[:n.value]
+            strings = chars.raw[:c.value].decode(ENCODING).split("\0")[:n.value]
         finally:
             L.oracle_lpe_free(handle)
         return Strings(strings, pixel.astype(np.int64), string.astype(np.int64), value, y1 - y0, camera.width, n_groups)
@@ -119,7 +126,7 @@ def render_rows(scene, camera, y0, y1, sqrtspp, seed):
 def to_regex(expr, n_groups):
     """The Python regular expression of a light path expression (the grammar of include/mcrt_abi.h) over the
     restatement's encoding with n_groups light groups. L matches every emitter, L'g' those of group g."""
-    lights = {chr(ord("0") + g) for g in range(n_groups)} | {UNGROUPED}
+    lights = {group_char(g) for g in range(n_groups)} | {UNGROUPED}
     alphabet = {"C", "B"} | set(VERTEX.values()) | lights
     s = "".join(expr.split())
     i = 0
@@ -140,7 +147,7 @@ def to_regex(expr, n_groups):
                 j = s.index("'", i + 1)
                 g = int(s[i + 1:j])
                 i = j + 1
-                return {chr(ord("0") + g)}
+                return {group_char(g)}
             return set(lights)
         if ch == "<":
             x, y = s[i], s[i + 1]

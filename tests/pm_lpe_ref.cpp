@@ -18,13 +18,15 @@
 namespace
 {
     // the encoding of tests/lpe_ref.cpp: 'C', the vertex events 'a' <RD>, 'b' <RS>, 'c' <RG>, 'd' <TS>, 'e' <TG>, a light
-    // of group g chr('0' + g), an emitter without a group '*'
+    // of group g the byte 0x80 + g (latin-1), an emitter without a group '*'
     char eventChar(const Interaction& ia)
     {
         if (ia.type == DIFFUSE) return 'a';
         if (ia.type == REFLECT) return ia.dirac_delta ? 'b' : 'c';
         return ia.dirac_delta ? 'd' : 'e';
     }
+
+    char groupChar(uint32_t g) { return (char)(0x80u + g); }
 
     // emitPhoton (mcrt_oracle.cpp) with each stored photon's events e1..em recorded (emission order, the storing vertex
     // excluded)
@@ -291,7 +293,7 @@ void* oracle_pm_lpe_render(void* h, const float* caustic, uint64_t n_caustic, co
         for (uint64_t i = 0; i < cnts[w]; i++) { history[w].emplace_back(src[w]); src[w] += history[w].back().size() + 1; }
     Labels label;
     if (group_of_light)
-        for (uint32_t l = 0; l < n_lights && l < s.light_prim.size(); l++) label.of_prim[s.light_prim[l]] = (char)('0' + group_of_light[l]);
+        for (uint32_t l = 0; l < n_lights && l < s.light_prim.size(); l++) label.of_prim[s.light_prim[l]] = groupChar(group_of_light[l]);
     auto* out = new LpeStrings();
     out->pixels.resize((size_t)(y1 - y0) * cam->width);
     Sampler smp(seed);

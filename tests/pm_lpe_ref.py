@@ -10,7 +10,7 @@ import tempfile
 
 import numpy as np
 
-from lpe_ref import Strings
+from lpe_ref import ENCODING, Strings, group_char
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
@@ -83,7 +83,7 @@ def photon_events(scene, emissions, caustic_factor, seed, pass_index=0):
                 li = np.zeros(n[w], np.uint32)
                 buf = C.create_string_buffer(max(chars[w], 1))
                 L.oracle_pm_photon_events_get(handle, w, ph.ctypes.data_as(C.c_void_p), li.ctypes.data_as(C.c_void_p), buf)
-                ev = buf.raw[:chars[w]].decode().split("\0")[:n[w]]
+                ev = buf.raw[:chars[w]].decode(ENCODING).split("\0")[:n[w]]
                 maps.append((ph, li, ev))
         finally:
             L.oracle_pm_photon_events_free(handle)
@@ -94,7 +94,7 @@ def history(events, lights, group_of_light=None):
     """The string a photon adds after x: its events from the last to the first, then its light's character."""
     out = []
     for ev, l in zip(events, lights):
-        light = "*" if group_of_light is None else chr(ord("0") + int(group_of_light[l]))
+        light = "*" if group_of_light is None else group_char(group_of_light[l])
         out.append(ev[::-1] + light)
     return out
 
@@ -105,7 +105,7 @@ def render_strings(scene, camera, y0, y1, sqrtspp, seed, maps, k, dv, gather_r2=
     g = None if group_of_light is None else np.ascontiguousarray(group_of_light, np.uint32)
     n_groups = 0 if g is None or g.size == 0 else int(g.max()) + 1
     ph = [np.ascontiguousarray(m[0], np.float32).reshape(-1, 8) for m in maps]
-    hs = [b"".join(s.encode() + b"\0" for s in m[1]) or b"\0" for m in maps]
+    hs = [b"".join(s.encode(ENCODING) + b"\0" for s in m[1]) or b"\0" for m in maps]
     r2 = np.ascontiguousarray(gather_r2, np.float64)
     with _Scene(scene) as h:
         handle = L.oracle_pm_lpe_render(h, ph[0].ctypes.data_as(C.c_void_p), len(ph[0]), hs[0], ph[1].ctypes.data_as(C.c_void_p),
@@ -121,7 +121,7 @@ def render_strings(scene, camera, y0, y1, sqrtspp, seed, maps, k, dv, gather_r2=
             chars = C.create_string_buffer(max(c.value, 1))
             L.oracle_pm_lpe_get(handle, pixel.ctypes.data_as(C.c_void_p), string.ctypes.data_as(C.c_void_p),
                                 value.ctypes.data_as(C.c_void_p), chars)
-            strings = chars.raw[:c.value].decode().split("\0")[:n.value]
+            strings = chars.raw[:c.value].decode(ENCODING).split("\0")[:n.value]
         finally:
             L.oracle_pm_lpe_free(handle)
     return Strings(strings, pixel.astype(np.int64), string.astype(np.int64), value, y1 - y0, camera.width, n_groups)
