@@ -545,7 +545,9 @@ class Integrator:
 
     def _check(self, rc):
         if rc:
-            raise McrtError(f"mcrt error {rc}: {lib().mcrt_last_error(self.ctx).decode()}")
+            e = McrtError(f"mcrt error {rc}: {lib().mcrt_last_error(self.ctx).decode()}")
+            e.code = rc       # the MCRT_ERR_* value
+            raise e
 
     def set_option(self, key, value):
         self._check(lib().mcrt_set_option(self.ctx, key.encode(), float(value)))

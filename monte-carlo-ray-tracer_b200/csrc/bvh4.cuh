@@ -195,11 +195,13 @@ namespace mcrt
             sstack = fast_stack_smem + threadIdx.x;
         }
 
-        MCRT_D void push(uint32_t ref, uint32_t tn_bits, uint32_t& overflow)
+        // A full stack drops the entry and hands the ray to the replay, which answers in the reference's order with a heap of its own:
+        // the closest hit is marked degenerate, the occlusion query a tie unless it still finds an occluder (which answers it anyway).
+        MCRT_D void push(uint32_t ref, uint32_t tn_bits)
         {
             if (sp < FAST_SMEM_STACK) sstack[sp * blockDim.x] = make_uint2(ref, tn_bits);
             else if (sp < FAST_STACK) lstack[sp - FAST_SMEM_STACK] = make_uint2(ref, tn_bits);
-            else { overflow = 1; return; }
+            else { if constexpr (OCC) verdict = 2u; else degenerate = true; return; }
             sp++;
         }
 
@@ -216,7 +218,7 @@ namespace mcrt
 
         // One inner node: tests its four child boxes, pushes the far hits, continues with the nearest (or with the next
         // pending entry when nothing is hit). -> false: nothing left to visit.
-        MCRT_D bool visitNode(const DeviceScene<double>& sc, TraceCounters& cnt, uint32_t& overflow)
+        MCRT_D bool visitNode(const DeviceScene<double>& sc, TraceCounters& cnt)
         {
             const float4* __restrict__ n = reinterpret_cast<const float4*>(sc.bvh4) + 8 * (size_t)cur;
             // float4 rows of a node: lo.x lo.y lo.z hi.x hi.y hi.z; the near plane of axis k is lo for d_k >= 0
@@ -249,9 +251,9 @@ namespace mcrt
 
             if (key0 == 0xFFFFFFFFu) return pop();     // nothing hit: next pending entry, if any
             // far children first, so the nearest pending one is on top
-            if (key3 != 0xFFFFFFFFu) push(refOf(key3), key3 & ~3u, overflow);
-            if (key2 != 0xFFFFFFFFu) push(refOf(key2), key2 & ~3u, overflow);
-            if (key1 != 0xFFFFFFFFu) push(refOf(key1), key1 & ~3u, overflow);
+            if (key3 != 0xFFFFFFFFu) push(refOf(key3), key3 & ~3u);
+            if (key2 != 0xFFFFFFFFu) push(refOf(key2), key2 & ~3u);
+            if (key1 != 0xFFFFFFFFu) push(refOf(key1), key1 & ~3u);
             cur = refOf(key0);
             return true;
         }
@@ -296,7 +298,7 @@ namespace mcrt
             return true;
         }
 
-        MCRT_D bool step(const DeviceScene<double>& sc, const RayQ<double>& ray, TraceCounters& cnt, uint32_t& overflow)
+        MCRT_D bool step(const DeviceScene<double>& sc, const RayQ<double>& ray, TraceCounters& cnt)
         {
 #if MCRT_SPECULATIVE
             // Speculative form (Aila & Laine): a lane that reaches a leaf stashes it and keeps walking inner nodes until every
@@ -315,7 +317,7 @@ namespace mcrt
                 }
                 else
                 {
-                    have_cur = visitNode(sc, cnt, overflow);
+                    have_cur = visitNode(sc, cnt);
                     if (!have_cur) break;
                 }
                 if (stashed && !__any_sync(__activemask(), stashed == 0u)) break;
@@ -325,7 +327,7 @@ namespace mcrt
 #else
             while (!(cur & BVH4_LEAF))
             {
-                if (!visitNode(sc, cnt, overflow)) return false;
+                if (!visitNode(sc, cnt)) return false;
             }
             if (!testLeaf(cur, sc, ray, cnt)) return false;
             return pop();
@@ -342,12 +344,11 @@ namespace mcrt
 
     // -> closest hit; `ambiguous` set when another hit lies within delta of it
     template <int PRIMS>
-    MCRT_D Hit<double> traverseFast(const DeviceScene<double>& sc, const RayQ<double>& ray, TraceCounters& cnt,
-                                    uint32_t& overflow, bool& ambiguous)
+    MCRT_D Hit<double> traverseFast(const DeviceScene<double>& sc, const RayQ<double>& ray, TraceCounters& cnt, bool& ambiguous)
     {
         FastSearch<PRIMS> fs;
         fs.begin(ray);
-        while (fs.step(sc, ray, cnt, overflow)) { }
+        while (fs.step(sc, ray, cnt)) { }
         ambiguous = fs.ambiguous(sc);
         return fs.best;
     }
@@ -423,7 +424,7 @@ namespace mcrt
             }
             while (active)
             {
-                if (!fs.step(sc, ray, cnt, overflow))
+                if (!fs.step(sc, ray, cnt))
                 {
                     Hit<double> h = fs.best;
                     bool replay;

@@ -298,7 +298,7 @@ namespace mcrt
                 // order-free search; the rare ray whose answer could depend on the visiting order is
                 // replayed in the reference's order (bvh4.cuh)
                 bool ambiguous;
-                Hit<R> h = traverseFast<PRIMS>(sc, rq, cnt, overflow, ambiguous);
+                Hit<R> h = traverseFast<PRIMS>(sc, rq, cnt, ambiguous);
                 if (ambiguous)
                 {
                     const DeviceScene<R> sc_copy = sc;   // the out-of-line call takes addresses: keep those copies off the hot path
@@ -333,7 +333,7 @@ namespace mcrt
         if constexpr (PRIMS == PRIMS_ALL) rq.inv_d = 1.0 / d;
         FastSearch<PRIMS, true> fs;
         if (!fs.beginOcclusion(sc, rq, target, cnt)) { Hit<double> miss = fs.best; miss.prim = NO_PRIM; return miss; }
-        if (fs.verdict != 2u) { while (fs.step(sc, rq, cnt, overflow)) { } }     // 2 already: a degenerate ray goes straight to the replay
+        if (fs.verdict != 2u) { while (fs.step(sc, rq, cnt)) { } }     // 2 already: a degenerate ray goes straight to the replay
         Hit<double> h = fs.best;
         if (fs.verdict == 1u) h.prim = NO_PRIM;
         else if (fs.verdict == 2u)

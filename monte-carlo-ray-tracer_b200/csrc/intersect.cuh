@@ -201,7 +201,10 @@ namespace mcrt
 
     // ------------------------------------------------------------------------------------------
     // Parity traversal: same visiting order as BVH::intersect.
-    constexpr int REF_HEAP_CAPACITY = 96; // reference max observed: 35 (SURVEY.md §3.2)
+    // Fixed: a ray that needs more entries sets `overflow`, and the call is refused (DESIGN.md §8). Restated peaks
+    // (tests/test_traversal_peaks_cpu.py): within it on the golden scenes' rays; 64 on 512 nested shells under the SAH builders and
+    // 112 under the octree builder.
+    constexpr int REF_HEAP_CAPACITY = 96;
 
     template <class R>
     struct RefHeap
@@ -313,6 +316,9 @@ namespace mcrt
 
     // ------------------------------------------------------------------------------------------
     // Fast traversal (float): wide child records, depth-first, nearest child first.
+    // Fixed: a full stack sets `overflow` and the call is refused. Depth first with up to (children - 1) pushes per node, so the tree
+    // bounds the peak by its largest sum of (children - 1) along a root-to-leaf path: 354 for the octree of 512 nested shells
+    // (DESIGN.md §8).
     constexpr int WIDE_STACK = 48;
 
     MCRT_D bool slabTestWide(const float4& lo, const float4& hi, const RayQ<float>& ray, float best, float& t)

@@ -262,7 +262,7 @@ namespace
     // optional cross-check of every Scene::intersect call of a render against the order-free search (oracle_render_rows_checked)
     struct SearchCheck { const void* nodes; double scale; uint64_t calls, flagged, mismatches; };
     SearchCheck* g_search_check = nullptr;
-    Isect intersectReferenceOrder(const Scene& s, const Ray& r, uint64_t* counter);
+    Isect intersectReferenceOrder(const Scene& s, const Ray& r, uint64_t* counter, size_t* peak = nullptr);
     void (*g_cross_fn)(const Scene& s, const Ray& r, const Isect& ref) = nullptr;
 
     Isect intersect(const Scene& s, const Ray& r, uint64_t* counter)
@@ -272,7 +272,8 @@ namespace
         return is;
     }
 
-    Isect intersectReferenceOrder(const Scene& s, const Ray& r, uint64_t* counter)
+    // peak: largest number of entries the heap held (the device's replay heap has REF_HEAP_CAPACITY of them, intersect.cuh)
+    Isect intersectReferenceOrder(const Scene& s, const Ray& r, uint64_t* counter, size_t* peak)
     {
         if (counter) (*counter)++;
         Isect best;
@@ -304,6 +305,7 @@ namespace
                     if (slab(&s.node_bounds[6 * child], r, t) && t < best.t) heap.push({ t, child });
                     child = s.node_next[child];
                 }
+                if (peak) *peak = std::max(*peak, heap.H.size());
             }
             if (heap.H.empty() || heap.H.front().t >= best.t) break;
             node = heap.H.front().node;
@@ -776,17 +778,27 @@ namespace
         return std::fabs(r.direction.x) < e || std::fabs(r.direction.y) < e || std::fabs(r.direction.z) < e;
     }
 
-    Isect searchFast(const Scene& s, const Node4* nodes, const Ray& r, double scene_scale, bool& ambiguous, uint64_t& box_tests, uint64_t& prim_tests)
+    // FastRay (bvh4.cuh) restated: 1 / d and o / d raised and lowered for the near and far planes
+    struct FastRay4 { float id[3], on[3], of[3]; };
+    // MCRT_FAST_STACK (bvh4.cuh) of the default build: a ray that needs more entries is replayed. The peaks below are those of the
+    // default walk (MCRT_SPECULATIVE = 0); the speculative form visits more nodes and can hold more entries.
+    constexpr size_t kFastStack = 40;
+    FastRay4 fastRay(const Ray& r)
     {
         auto inv = [](double v) { float f = (float)v; if (!(std::fabs(f) >= 1e-18f)) f = std::copysign(1e-18f, f); return 1.0f / f; };
-        const float id[3] = { inv(r.direction.x), inv(r.direction.y), inv(r.direction.z) };
-        const float od[3] = { (float)r.start.x * id[0], (float)r.start.y * id[1], (float)r.start.z * id[2] };
-        float on[3], of[3];
-        for (int k = 0; k < 3; k++) { const float m = std::fabs(od[k]) * 1.9073486e-6f; on[k] = od[k] + m; of[k] = od[k] - m; }
-        Isect best;
-        bool best_edge = false;
-        double second_t = std::numeric_limits<double>::max();
-        float limit = INFINITY;
+        FastRay4 f;
+        f.id[0] = inv(r.direction.x); f.id[1] = inv(r.direction.y); f.id[2] = inv(r.direction.z);
+        const float od[3] = { (float)r.start.x * f.id[0], (float)r.start.y * f.id[1], (float)r.start.z * f.id[2] };
+        for (int k = 0; k < 3; k++) { const float m = std::fabs(od[k]) * 1.9073486e-6f; f.on[k] = od[k] + m; f.of[k] = od[k] - m; }
+        return f;
+    }
+
+    // FastSearch::step / visitNode / pop (bvh4.cuh) restated with an unbounded stack: depth first, nearest child next, the other hit
+    // children pushed farthest first, entries culled against `limit` on pop. leaf(ref) tests a leaf and may lower `limit`; it returns
+    // false to end the search. peak: the largest number of pending entries (the device's stack holds FAST_STACK of them).
+    extern "C++" template <class Leaf>
+    void walkFast(const Node4* nodes, const FastRay4& f, const float& limit, Leaf leaf, uint64_t& box_tests, size_t& peak)
+    {
         struct Entry { uint32_t ref; float tn; };
         std::vector<Entry> stack;
         uint32_t cur = 0;
@@ -804,9 +816,9 @@ namespace
                     float tn = 0.0f, tf = INFINITY;
                     for (int k = 0; k < 3; k++)
                     {
-                        const float bn = id[k] < 0.0f ? n.hi[k][c] : n.lo[k][c], bf = id[k] < 0.0f ? n.lo[k][c] : n.hi[k][c];
-                        tn = std::fmax(tn, std::fmaf(bn, id[k], -on[k]));
-                        tf = std::fmin(tf, std::fmaf(bf, id[k], -of[k]));
+                        const float bn = f.id[k] < 0.0f ? n.hi[k][c] : n.lo[k][c], bf = f.id[k] < 0.0f ? n.lo[k][c] : n.hi[k][c];
+                        tn = std::fmax(tn, std::fmaf(bn, f.id[k], -f.on[k]));
+                        tf = std::fmin(tf, std::fmaf(bf, f.id[k], -f.of[k]));
                     }
                     tn *= 0.99999619f; tf *= 1.00000381f;
                     const bool hit = n.child[c] != 0u && tn <= tf && tn <= limit;
@@ -817,9 +829,26 @@ namespace
                 if (key[0] == 0xFFFFFFFFu) { if (!pop()) { have = false; break; } continue; }
                 for (int j = 3; j >= 1; j--)
                     if (key[j] != 0xFFFFFFFFu) { const uint32_t b = key[j] & ~3u; float tn; std::memcpy(&tn, &b, 4); stack.push_back({ n.child[key[j] & 3u], tn }); }
+                peak = std::max(peak, stack.size());
                 cur = n.child[key[0] & 3u];
             }
             if (!have) break;
+            if (!leaf(cur)) break;
+            if (!pop()) break;
+        }
+    }
+
+    Isect searchFast(const Scene& s, const Node4* nodes, const Ray& r, double scene_scale, bool& ambiguous, uint64_t& box_tests, uint64_t& prim_tests,
+                     size_t* peak = nullptr)
+    {
+        const FastRay4 f = fastRay(r);
+        Isect best;
+        bool best_edge = false;
+        double second_t = std::numeric_limits<double>::max();
+        float limit = INFINITY;
+        size_t stack_peak = 0;
+        walkFast(nodes, f, limit, [&](uint32_t cur)
+        {
             const uint32_t first = (cur >> 8) & 0x7FFFFFu, count = cur & 0xFFu;
             for (uint32_t i = first; i < first + count; i++)
             {
@@ -832,11 +861,13 @@ namespace
                     else if (c.t < second_t) second_t = c.t;
                 }
             }
-            if (!pop()) break;
-        }
+            return true;
+        }, box_tests, stack_peak);
+        if (peak) *peak = stack_peak;
         ambiguous = best.prim != 0xFFFFFFFFu && second_t <= best.t + ambiguityDelta(best.t, scene_scale);
         if (best.prim != 0xFFFFFFFFu && best_edge) ambiguous = true;      // R2: the winner is hit on its boundary
         if (degenerateDirection(r)) ambiguous = true;                     // R1: a direction component is (nearly) zero
+        if (stack_peak > kFastStack) ambiguous = true;                    // R3: the device's stack is full (FastSearch::push)
         return best;
     }
 }
@@ -898,6 +929,43 @@ namespace
     }
 }
 
+// FastSearch<PRIMS, true> in the device's visiting order (walkFast): the verdict and the largest number of pending stack entries. The
+// verdict equals searchVisible's unless a ray holds both an occluder and a tie (either is a correct verdict: both keep the reference's answer).
+namespace
+{
+    int searchVisibleOrdered(const Scene& s, const Node4* nodes, const Ray& r, double scene_scale, uint32_t target, double& t_target, size_t& peak)
+    {
+        Isect tgt;
+        double tu = 0.5, tv = 0.25;
+        peak = 0;
+        if (!hitPrimUV(s, target, r, tgt, tu, tv)) return 1;
+        t_target = tgt.t;
+        if (degenerateDirection(r) || onBoundary(tu, tv, tgt.t, scene_scale)) return 2;
+        const double delta = ambiguityDelta(tgt.t, scene_scale);
+        const float limit = roundUpToFloat(tgt.t + 2.0 * delta);
+        int verdict = 0;
+        uint64_t box_tests = 0;
+        walkFast(nodes, fastRay(r), limit, [&](uint32_t cur)
+        {
+            const uint32_t first = (cur >> 8) & 0x7FFFFFu, count = cur & 0xFFu;
+            for (uint32_t i = first; i < first + count; i++)
+            {
+                if (i == target) continue;
+                Isect c;
+                double cu = 0.5, cv = 0.25;
+                if (hitPrimUV(s, i, r, c, cu, cv))
+                {
+                    if (c.t <= tgt.t + delta && onBoundary(cu, cv, c.t, scene_scale)) { verdict = 2; return false; }
+                    if (c.t < tgt.t - delta) { verdict = 1; return false; }
+                    if (c.t <= tgt.t + delta) { verdict = 2; return false; }
+                }
+            }
+            return true;
+        }, box_tests, peak);
+        return verdict == 0 && peak > kFastStack ? 2 : verdict;     // a full stack hands the ray to the replay unless an occluder was found
+    }
+}
+
 void oracle_trace_visible(void* h, const void* nodes128, double scene_scale, const mcrt_ray* rays, const uint32_t* target, size_t n,
                           uint8_t* verdict, double* t_target)
 {
@@ -954,6 +1022,87 @@ void oracle_trace_fast(void* h, const void* nodes128, uint32_t n_nodes, double s
     }
     if (box_tests) *box_tests = bt;
     if (prim_tests) *prim_tests = pt;
+}
+
+// Peaks of the traversal structures per ray. oracle_trace_peaks: the reference-order traversal (hits as oracle_trace) and the largest
+// size of its heap. oracle_trace_fast_peaks: the order-free search (hits and flags as oracle_trace_fast) and the largest size of its
+// stack. oracle_trace_visible_peaks: the occlusion query in the device's visiting order (verdict, t of the target, largest stack size).
+void oracle_trace_peaks(void* h, const mcrt_ray* rays, size_t n, mcrt_hit* hits, uint32_t* heap_peak)
+{
+    const Scene& s = *static_cast<Scene*>(h);
+    for (size_t i = 0; i < n; i++)
+    {
+        size_t peak = 0;
+        Isect is = intersectReferenceOrder(s, makeRay(D3(rays[i].origin), D3(rays[i].direction), s.d.scene_ior), nullptr, &peak);
+        hits[i].t = is.t; hits[i].u = is.u; hits[i].v = is.v; hits[i].prim = is.prim; hits[i].interpolate = is.interpolate;
+        heap_peak[i] = (uint32_t)peak;
+    }
+}
+
+void oracle_trace_fast_peaks(void* h, const void* nodes128, double scene_scale, const mcrt_ray* rays, size_t n, mcrt_hit* hits, uint8_t* flags,
+                             uint32_t* stack_peak)
+{
+    const Scene& s = *static_cast<Scene*>(h);
+    uint64_t bt = 0, pt = 0;
+    for (size_t i = 0; i < n; i++)
+    {
+        bool amb = false;
+        size_t peak = 0;
+        Isect is = searchFast(s, static_cast<const Node4*>(nodes128), makeRay(D3(rays[i].origin), D3(rays[i].direction), s.d.scene_ior), scene_scale, amb, bt, pt, &peak);
+        hits[i].t = is.t; hits[i].u = is.u; hits[i].v = is.v; hits[i].prim = is.prim; hits[i].interpolate = is.interpolate;
+        flags[i] = amb ? 1 : 0;
+        stack_peak[i] = (uint32_t)peak;
+    }
+}
+
+// An upper bound, per ray, on the entries of fast mode's depth-first stack (traverseWide, intersect.cuh). That walk pushes every hit
+// child of a visited node but the nearest, so its stack never holds more than the largest sum of (hit children - 1) over the nodes of
+// one path of boxes the ray hits. Fast mode rounds the ray and the boxes to float and prunes by its best hit; boxes grown by `margin` on
+// every side cover the rounding, and pruning only removes entries. The bound does not depend on the visiting order.
+namespace
+{
+    uint32_t widePathBound(const Scene& s, const Ray& r, double margin, uint32_t node)
+    {
+        if (s.node_count[node]) return 0;
+        uint32_t hits = 0, deepest = 0;
+        for (uint32_t child = node + 1; child != 0; child = s.node_next[child])
+        {
+            const double* b = &s.node_bounds[6 * child];
+            double tn = 0.0, tf = INFINITY;
+            for (int k = 0; k < 3; k++)
+            {
+                const double o = k == 0 ? r.start.x : k == 1 ? r.start.y : r.start.z, d = k == 0 ? r.direction.x : k == 1 ? r.direction.y : r.direction.z;
+                const double t0 = (b[k] - margin - o) / d, t1 = (b[3 + k] + margin - o) / d;
+                tn = std::fmax(tn, std::fmin(t0, t1)); tf = std::fmin(tf, std::fmax(t0, t1));
+            }
+            if (tn > tf) continue;       // NaN (a zero direction component on a plane) counts as a hit
+            hits++;
+            deepest = std::max(deepest, widePathBound(s, r, margin, child));
+        }
+        return hits ? hits - 1 + deepest : 0;
+    }
+}
+
+void oracle_wide_stack_bound(void* h, const mcrt_ray* rays, size_t n, double margin, uint32_t* bound)
+{
+    const Scene& s = *static_cast<Scene*>(h);
+    for (size_t i = 0; i < n; i++)
+        bound[i] = s.node_first.empty() ? 0u : widePathBound(s, makeRay(D3(rays[i].origin), D3(rays[i].direction), s.d.scene_ior), margin, 0);
+}
+
+void oracle_trace_visible_peaks(void* h, const void* nodes128, double scene_scale, const mcrt_ray* rays, const uint32_t* target, size_t n,
+                                uint8_t* verdict, double* t_target, uint32_t* stack_peak)
+{
+    const Scene& s = *static_cast<Scene*>(h);
+    for (size_t i = 0; i < n; i++)
+    {
+        double t = 0.0;
+        size_t peak = 0;
+        verdict[i] = (uint8_t)searchVisibleOrdered(s, static_cast<const Node4*>(nodes128), makeRay(D3(rays[i].origin), D3(rays[i].direction), s.d.scene_ior),
+                                                   scene_scale, target[i], t, peak);
+        t_target[i] = t;
+        stack_peak[i] = (uint32_t)peak;
+    }
 }
 
 void oracle_sample_rays(void* h, const mcrt_ray* rays, const uint32_t* pixel, const uint32_t* sample, size_t n, uint32_t seed, double* out)

@@ -31,6 +31,11 @@ def lib():
         L.oracle_trace_fast.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_double, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
                                         C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
         L.oracle_trace_visible.argtypes = [C.c_void_p, C.c_void_p, C.c_double, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
+        L.oracle_trace_peaks.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
+        L.oracle_trace_fast_peaks.argtypes = [C.c_void_p, C.c_void_p, C.c_double, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.oracle_trace_visible_peaks.argtypes = [C.c_void_p, C.c_void_p, C.c_double, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
+                                                 C.c_void_p]
+        L.oracle_wide_stack_bound.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_double, C.c_void_p]
         L.oracle_render_rows_checked.argtypes = [C.c_void_p, C.c_void_p, C.c_double, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
                                                  C.c_void_p, C.c_void_p]
         L.oracle_bvh_build.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_void_p), C.c_void_p]
@@ -173,6 +178,42 @@ class PortScene:
         verdict = np.zeros(len(rays), dtype=np.uint8); t = np.zeros(len(rays))
         lib().oracle_trace_visible(self.h, _p(nodes), float(scene_scale), _p(rays), _p(target), len(rays), _p(verdict), _p(t))
         return verdict, t
+
+    def trace_peaks(self, rays):
+        """trace() and, per ray, the largest number of entries the reference-order heap held -> (hits, heap peaks)"""
+        rays = np.ascontiguousarray(rays, dtype=np.float64).reshape(-1, 6)
+        hits = np.zeros(len(rays), dtype=self.pkg.HIT_DTYPE)
+        peak = np.zeros(len(rays), dtype=np.uint32)
+        lib().oracle_trace_peaks(self.h, _p(rays), len(rays), _p(hits), _p(peak))
+        return hits, peak
+
+    def trace_fast_peaks(self, nodes, scene_scale, rays):
+        """trace_fast() and, per ray, the largest number of entries the order-free search's stack held -> (hits, flags, stack peaks);
+        a ray whose peak exceeds the device's stack is flagged"""
+        rays = np.ascontiguousarray(rays, dtype=np.float64).reshape(-1, 6)
+        nodes = np.ascontiguousarray(nodes)
+        hits = np.zeros(len(rays), dtype=self.pkg.HIT_DTYPE)
+        flags = np.zeros(len(rays), dtype=np.uint8)
+        peak = np.zeros(len(rays), dtype=np.uint32)
+        lib().oracle_trace_fast_peaks(self.h, _p(nodes), float(scene_scale), _p(rays), len(rays), _p(hits), _p(flags), _p(peak))
+        return hits, flags.astype(bool), peak
+
+    def trace_visible_peaks(self, nodes, scene_scale, rays, target):
+        """The occlusion query in the device's visiting order -> (verdict as trace_visible, t of the target, stack peaks)"""
+        rays = np.ascontiguousarray(rays, dtype=np.float64).reshape(-1, 6)
+        target = np.ascontiguousarray(target, dtype=np.uint32)
+        nodes = np.ascontiguousarray(nodes)
+        verdict = np.zeros(len(rays), dtype=np.uint8); t = np.zeros(len(rays)); peak = np.zeros(len(rays), dtype=np.uint32)
+        lib().oracle_trace_visible_peaks(self.h, _p(nodes), float(scene_scale), _p(rays), _p(target), len(rays), _p(verdict), _p(t), _p(peak))
+        return verdict, t, peak
+
+    def wide_stack_bound(self, rays, margin):
+        """Per ray, an upper bound on the entries of fast mode's depth-first stack: the largest sum of (hit children - 1) along a path of
+        boxes, grown by `margin`, that the ray hits"""
+        rays = np.ascontiguousarray(rays, dtype=np.float64).reshape(-1, 6)
+        out = np.zeros(len(rays), dtype=np.uint32)
+        lib().oracle_wide_stack_bound(self.h, _p(rays), len(rays), float(margin), _p(out))
+        return out
 
     def sample_pixels(self, camera, pixel, sample, seed):
         """-> (rgb [n,3], camera rays [n,6]) for (pixel, sample) pairs"""
