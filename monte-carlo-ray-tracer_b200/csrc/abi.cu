@@ -178,7 +178,10 @@ struct mcrt_ctx
     // options
     int sort_rays = 1;
     int sort_shade = 0;
-    int sort_shade_class = 1;   // k_shade walks paths grouped by the material class of their hit
+    // 1: k_shade walks paths grouped by the material class of their hit. Off by default: on the H100 the class key, its
+    // scan and scatter (three launches per bounce) and the gathers through shade_order cost more than the coherent
+    // material branches save - C2 parity 1653 against 1713 ms per frame, fast mode 1213 against 1287 (DESIGN.md §3)
+    int sort_shade_class = 0;
     int sort_prim_key = -1;   // -1 auto (>= 4096 primitives), 0 origin-cell keys, 1 source-primitive keys
     uint32_t pool_paths = 1u << 23;   // measured on C2: 2 Mi 2269, 4 Mi 2378, 8 Mi 2463, 16 Mi 2503 Mray/s (coarser bins fill better)
     int blocks_per_sm = 16;   // grid = SMs x this for the grid-stride stage kernels (more CTAs than fit at once keep every SM busy to the end of a stage)
