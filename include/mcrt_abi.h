@@ -667,6 +667,24 @@ int mcrt_denoise_dev(mcrt_ctx* ctx, const double* a_rgb_dev, const double* a_wei
                      uint32_t tile, const double* features_dev, uint32_t width, uint32_t height,
                      const mcrt_denoise_params* params, double* out_rgb_dev, double* frame_error);
 
+/* Denoising film planes (light groups, AOVs, components, LPE planes; box film, whole frame): every plane is filtered with
+ * the edge weights mcrt_denoise_dev computes for the guide frame, the box-film half sums a_rgb_dev / b_rgb_dev. The
+ * filter is linear once its weights are fixed, so planes that sum to the guide give filtered sums that sum to the
+ * guide's, up to rounding. a_planes_dev / b_planes_dev [n_planes][height*width][3] are each half's plane sums;
+ * a_out_planes_dev / b_out_planes_dev (same layout) receive the filtered sums, unresolved, which
+ * mcrt_progressive_resolve[_tiles]_dev resolves (with its residual-noise estimate) and mcrt_light_groups_combine_dev
+ * recomposites; a pixel with an empty half keeps its input sums. out_rgb_dev and frame_error (optional, given together
+ * or not at all) receive exactly what mcrt_denoise_dev writes for the guide. Scratch: 400 B per pixel plus 48 B per
+ * pixel per plane, kept by the context. MCRT_ERR_INVALID, writing nothing: every argument mcrt_denoise_dev refuses,
+ * n_planes 0, an output buffer that overlaps an input or another output, out_rgb_dev without frame_error or the
+ * reverse. */
+int mcrt_denoise_planes_dev(mcrt_ctx* ctx, const double* a_rgb_dev, const double* b_rgb_dev,
+                            const double* a_planes_dev, const double* b_planes_dev, uint32_t n_planes,
+                            const uint32_t* tile_samples, uint32_t tile, const double* features_dev,
+                            uint32_t width, uint32_t height, const mcrt_denoise_params* params,
+                            double* a_out_planes_dev, double* b_out_planes_dev,
+                            double* out_rgb_dev, double* frame_error);
+
 /* A device buffer that other processes on the node can map: *dev_ptr (zero-filled) and its 64-byte CUDA IPC
  * handle, to be sent to the peers by whatever channel the host uses (torch.distributed in this repository). */
 int mcrt_frame_alloc(mcrt_ctx* ctx, uint64_t bytes, void** dev_ptr, unsigned char ipc_handle[64]);

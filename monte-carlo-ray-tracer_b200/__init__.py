@@ -43,7 +43,7 @@ ABI_SYMBOLS = [
     "mcrt_set_light_groups", "mcrt_render_accumulate_groups_dev", "mcrt_light_groups_combine_dev",
     "mcrt_render_accumulate_aovs_dev", "mcrt_photon_download_lights", "mcrt_render_accumulate_photon_components_dev",
     "mcrt_set_light_path_expressions", "mcrt_render_accumulate_lpe_dev", "mcrt_lpe_compile_host",
-    "mcrt_lpe_compile_photon_host", "mcrt_photon_download_lpe_states",
+    "mcrt_lpe_compile_photon_host", "mcrt_photon_download_lpe_states", "mcrt_denoise_planes_dev",
 ]
 
 # The light-path AOV planes of mcrt_render_accumulate_aovs_dev, in plane order (MCRT_AOV_* of include/mcrt_abi.h):
@@ -296,6 +296,9 @@ def lib():
         L.mcrt_denoise_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32,
                                        C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(DenoiseParams), C.c_void_p,
                                        C.POINTER(C.c_double)]
+        L.mcrt_denoise_planes_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p,
+                                              C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(DenoiseParams), C.c_void_p,
+                                              C.c_void_p, C.c_void_p, C.POINTER(C.c_double)]
         L.mcrt_photon_emit_total.argtypes = [C.c_void_p, C.POINTER(PhotonEmitParams), C.POINTER(C.c_uint64)]
         L.mcrt_photon_emit_range.argtypes = [C.c_void_p, C.POINTER(PhotonEmitParams), C.c_int, C.c_uint64, C.c_uint64, C.POINTER(C.c_void_p),
                                              C.POINTER(C.c_uint64), C.POINTER(C.c_void_p), C.POINTER(C.c_uint64), C.POINTER(Stats)]
@@ -821,6 +824,24 @@ class Integrator:
                                            counts.ctypes.data_as(C.c_void_p), tile, p(features_ptr), width, height,
                                            C.byref(params) if params is not None else None, p(out_ptr), C.byref(err)))
         return err.value
+
+    def denoise_planes_dev(self, a_rgb_ptr, b_rgb_ptr, a_planes_ptr, b_planes_ptr, n_planes, tile_samples, tile, features_ptr,
+                           width, height, a_out_ptr, b_out_ptr, params=None, out_ptr=None):
+        """mcrt_denoise_planes_dev: every plane of a_planes / b_planes [n_planes, height, width, 3] (box-film sums)
+        filtered with the weights mcrt_denoise_dev computes for the guide halves a_rgb / b_rgb, into a_out / b_out (same
+        layout, unresolved sums). out_ptr (optional): the guide's denoised frame [height, width, 3], as denoise_dev
+        writes it. -> its residual error, or None without out_ptr. tile_samples and params as denoise_dev's."""
+        def p(x):
+            return C.c_void_p(x) if x else None
+        counts = np.ascontiguousarray(tile_samples, dtype=np.uint32)
+        if counts.shape != tile_grid(height, width, tile) + (2,):
+            raise McrtError(f"tile_samples has shape {counts.shape}, expected {tile_grid(height, width, tile) + (2,)}")
+        err = C.c_double()
+        self._check(lib().mcrt_denoise_planes_dev(self.ctx, p(a_rgb_ptr), p(b_rgb_ptr), p(a_planes_ptr), p(b_planes_ptr), n_planes,
+                                                  counts.ctypes.data_as(C.c_void_p), tile, p(features_ptr), width, height,
+                                                  C.byref(params) if params is not None else None, p(a_out_ptr), p(b_out_ptr),
+                                                  p(out_ptr), C.byref(err) if out_ptr else None))
+        return err.value if out_ptr else None
 
     def frame_alloc(self, nbytes):
         """-> (device pointer, 64-byte CUDA IPC handle) of a zero-filled buffer other ranks can map"""
@@ -1490,6 +1511,7 @@ class Progressive:
         self.history = []                                           # one record per render_adaptive pass
         self.stop_reason = None                                     # why the last render_adaptive stopped
         self._features = None                                       # ((samples, specular_depth), device sums [height, width, 8]) of features()
+        self._denoised_planes = None                                # [A, B] filtered plane sums of denoise_planes(), until the next add()
 
     @property
     def samples(self):
@@ -1544,6 +1566,7 @@ class Progressive:
         for k in self._STATS:
             self.stats[k] += st[k]
         self._resolved = None
+        self._denoised_planes = None
         return st
 
     def _resolve(self, sums=False):
@@ -1556,7 +1579,6 @@ class Progressive:
     def _halves(self, weights=None):
         """The sums of halves A and B, [rows, width, 3] each: with planes (light groups, AOVs, components) the combination
         of the planes with weights [n_planes, 3] or [n_planes] (None: every weight 1, the beauty frame's sums)."""
-        import torch
         if self.lpes is not None:
             if weights is None:
                 return [self.rgb[0][-1], self.rgb[1][-1]]   # the beauty plane
@@ -1566,12 +1588,16 @@ class Progressive:
             if weights is not None:
                 raise McrtError("weights need a render with light groups, AOVs, photon-mapper components or light path expressions")
             return self.rgb
-        w = np.ones(self.n_planes) if weights is None else weights
+        return self._combine(self.rgb, self.n_planes, np.ones(self.n_planes) if weights is None else weights)
+
+    def _combine(self, planes, n, weights):
+        """The first n planes of halves [A, B] summed with weights [n, 3] or [n] (mcrt_light_groups_combine_dev)."""
+        import torch
         out = []
         for h in (0, 1):
-            o = torch.empty(self.rgb[h].shape[1:], dtype=torch.float64, device=self.rgb[h].device)
+            o = torch.empty(planes[h].shape[1:], dtype=torch.float64, device=planes[h].device)
             torch.cuda.synchronize(o.device)   # the library works on its own stream
-            self.integrator.light_groups_combine_dev(self.rgb[h].data_ptr(), self.n_planes, o.numel(), w, o.data_ptr())
+            self.integrator.light_groups_combine_dev(planes[h].data_ptr(), n, o.numel(), weights, o.data_ptr())
             out.append(o)
         return out
 
@@ -1756,15 +1782,7 @@ class Progressive:
         weights (light groups, AOVs or components only): denoise the frame relit or recomposited with these weights (relight) instead of
         the beauty frame."""
         import torch
-        if (self.y_first, self.y_step, self.n_rows) != (0, 1, self.camera.height):
-            raise McrtError("denoise needs the whole frame as the row set (y_first 0, y_step 1, n_rows = height)")
-        if not (self.tile_counts > 0).all():
-            raise McrtError("denoise needs samples in both halves of every tile")
-        given = {"iterations": iterations, "sigma_color": sigma_color, "sigma_normal": sigma_normal,
-                 "sigma_depth": sigma_depth, "sigma_albedo": sigma_albedo}
-        v = {k: DENOISE_DEFAULTS[k] if x is None else x for k, x in given.items()}
-        params = DenoiseParams(int(v["iterations"]), 0, float(v["sigma_color"]), float(v["sigma_normal"]),
-                               float(v["sigma_depth"]), float(v["sigma_albedo"]))
+        params = self._denoise_params(iterations, sigma_color, sigma_normal, sigma_depth, sigma_albedo)
         rgb = self._halves(weights)
         feats = self._feature_sums(feature_samples, specular_depth)
         out = torch.empty_like(rgb[0])
@@ -1772,6 +1790,62 @@ class Progressive:
         err = self.integrator.denoise_dev(rgb[0].data_ptr(), w[0], rgb[1].data_ptr(), w[1], self.tile_counts, self.tile,
                                           feats.data_ptr(), self.camera.width, self.camera.height, out.data_ptr(), params)
         return out.cpu().numpy(), err
+
+    def _denoise_params(self, iterations, sigma_color, sigma_normal, sigma_depth, sigma_albedo):
+        """The checks denoise and denoise_planes share -> DenoiseParams, arguments left None at DENOISE_DEFAULTS."""
+        if (self.y_first, self.y_step, self.n_rows) != (0, 1, self.camera.height):
+            raise McrtError("denoise needs the whole frame as the row set (y_first 0, y_step 1, n_rows = height)")
+        if not (self.tile_counts > 0).all():
+            raise McrtError("denoise needs samples in both halves of every tile")
+        given = {"iterations": iterations, "sigma_color": sigma_color, "sigma_normal": sigma_normal,
+                 "sigma_depth": sigma_depth, "sigma_albedo": sigma_albedo}
+        v = {k: DENOISE_DEFAULTS[k] if x is None else x for k, x in given.items()}
+        return DenoiseParams(int(v["iterations"]), 0, float(v["sigma_color"]), float(v["sigma_normal"]),
+                             float(v["sigma_depth"]), float(v["sigma_albedo"]))
+
+    def denoise_planes(self, iterations=None, sigma_color=None, sigma_normal=None, sigma_depth=None, sigma_albedo=None,
+                       feature_samples=8, specular_depth=0):
+        """Every plane denoised with the beauty frame's filter weights (mcrt_denoise_planes_dev) -> (planes float64
+        [n, H, W, 3], each plane's residual error float64 [n]). The planes are those of group_frames(), aov_frames(),
+        component_frames() or lpe_frames(); the weights are those denoise() computes for the beauty frame (with light
+        path expressions, the "C.*" plane, which is the guide and is not returned). Each plane is resolved from its
+        filtered sums like the noisy planes, so its error is estimated from the difference of its two filtered halves.
+        The filter is linear once its weights are fixed, so planes that sum to the beauty frame (light groups, AOVs,
+        components) stay a decomposition of the denoised frame: relight_denoised(weights) recomposites them without
+        filtering again. The filtered sums stay on the device until the next add() or load().
+
+        Arguments as denoise()'s. Raises McrtError on a render without planes and where denoise() does.
+
+        Known limit: a plane is smoothed with edges the beauty frame shows; an edge only that plane shows (one light
+        group's shadow filled by another group) is blurred by as much as the beauty's noise allows (DESIGN.md §6)."""
+        import torch
+        if not self._planar and self.lpes is None:
+            raise McrtError("denoise_planes needs a render with light groups, AOVs, photon-mapper components or light path expressions")
+        params = self._denoise_params(iterations, sigma_color, sigma_normal, sigma_depth, sigma_albedo)
+        n = len(self.lpes) if self.lpes is not None else self.n_planes
+        guide = self._halves()
+        feats = self._feature_sums(feature_samples, specular_depth)
+        out = [torch.empty((n,) + tuple(self.rgb[h].shape[1:]), dtype=torch.float64, device=self.rgb[h].device) for h in (0, 1)]
+        torch.cuda.synchronize(out[0].device)   # the library works on its own stream
+        self.integrator.denoise_planes_dev(guide[0].data_ptr(), guide[1].data_ptr(), self.rgb[0].data_ptr(), self.rgb[1].data_ptr(), n,
+                                           self.tile_counts, self.tile, feats.data_ptr(), self.camera.width, self.camera.height,
+                                           out[0].data_ptr(), out[1].data_ptr(), params)
+        self._denoised_planes = out
+        res = [self._resolve_halves([out[0][k], out[1][k]]) for k in range(n)]
+        return np.stack([r[0] for r in res]), np.array([r[1] for r in res])
+
+    def relight_denoised(self, weights):
+        """The frame recomposited from the planes of the last denoise_planes() call: their filtered sums combined with
+        weights (layout and meaning as relight's) and resolved -> (frame, frame relative error, per-tile relative errors).
+        With unit weights on light groups, AOVs or components it is denoise()'s frame, up to rounding. No filter runs:
+        the weights all come from the beauty frame. denoise(weights=w) instead filters the relit frame with weights
+        computed on that relit frame, so its results for different w do not add up. Raises McrtError unless
+        denoise_planes() ran since the last add() or load()."""
+        if self._denoised_planes is None:
+            raise McrtError("relight_denoised needs denoise_planes() since the last add() or load()")
+        planes = self._denoised_planes
+        frame, err, tiles, _ = self._resolve_halves(self._combine(planes, planes[0].shape[0], weights))
+        return frame, err, tiles
 
     # -- checkpoint / resume
     def _identity(self):

@@ -94,6 +94,8 @@ struct mcrt_ctx
     size_t resolve_scratch_values = 0;
     double* d_denoise_scratch = nullptr;   // state, guides, tile counts and sums of mcrt_denoise_dev (grow-only)
     size_t denoise_scratch_values = 0;
+    double* d_denoise_planes_scratch = nullptr;   // tap weights and plane states of mcrt_denoise_planes_dev (grow-only)
+    size_t denoise_planes_scratch_values = 0;
     uint32_t* d_pixel_list = nullptr;      // pixels of the active tiles of mcrt_render_accumulate_tiles_dev (grow-only)
     size_t pixel_list_values = 0;
     std::vector<uint32_t> h_pixel_list;
@@ -1183,6 +1185,7 @@ void mcrt_destroy(mcrt_ctx* ctx)
     if (ctx->d_host_out) cudaFree(ctx->d_host_out);
     if (ctx->d_resolve_scratch) cudaFree(ctx->d_resolve_scratch);
     if (ctx->d_denoise_scratch) cudaFree(ctx->d_denoise_scratch);
+    if (ctx->d_denoise_planes_scratch) cudaFree(ctx->d_denoise_planes_scratch);
     if (ctx->d_pixel_list) cudaFree(ctx->d_pixel_list);
     if (ctx->d_group_of_light) cudaFree(ctx->d_group_of_light);
     if (ctx->d_group_weights) cudaFree(ctx->d_group_weights);
@@ -2406,6 +2409,56 @@ int mcrt_render_features_chain_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uin
                           specular_depth, features_dev, stats);
 }
 
+namespace
+{
+    // The arguments mcrt_denoise_dev and mcrt_denoise_planes_dev both check: frame size, tile, each tile's halves,
+    // iterations and sigmas. -> MCRT_OK with the parameters in *pr and the tile count in *n_tiles.
+    int denoiseCheck(mcrt_ctx* ctx, const char* fn, uint32_t width, uint32_t height, uint32_t tile, const uint32_t* tile_samples,
+                     const mcrt_denoise_params* params, mcrt_denoise_params* pr, uint64_t* n_tiles)
+    {
+        const std::string name(fn);
+        const uint64_t n_pixels = (uint64_t)width * height;
+        if (n_pixels == 0 || n_pixels > 0xFFFFFFFFull) { ctx->error = name + ": empty frame or more than 2^32 pixels"; return MCRT_ERR_INVALID; }
+        if (tile == 0) { ctx->error = name + ": tile is 0"; return MCRT_ERR_INVALID; }
+        *pr = { MCRT_DENOISE_DEFAULT_ITERATIONS, 0u, MCRT_DENOISE_DEFAULT_SIGMA_COLOR, MCRT_DENOISE_DEFAULT_SIGMA_NORMAL,
+                MCRT_DENOISE_DEFAULT_SIGMA_DEPTH, MCRT_DENOISE_DEFAULT_SIGMA_ALBEDO };
+        if (params) *pr = *params;
+        if (pr->iterations > MCRT_DENOISE_MAX_ITERATIONS) { ctx->error = name + ": more than MCRT_DENOISE_MAX_ITERATIONS iterations"; return MCRT_ERR_INVALID; }
+        for (double sg : { pr->sigma_color, pr->sigma_normal, pr->sigma_depth, pr->sigma_albedo })
+            if (!std::isfinite(sg) || sg < 0.0) { ctx->error = name + ": a sigma is negative or not finite"; return MCRT_ERR_INVALID; }
+        const uint64_t tiles_x = (width + tile - 1) / tile, tiles_y = (height + tile - 1) / tile;
+        *n_tiles = tiles_x * tiles_y;
+        for (uint64_t t = 0; t < *n_tiles; t++)
+            if (tile_samples[2 * t] == 0 || tile_samples[2 * t + 1] == 0)
+            {
+                ctx->error = name + ": a tile has no samples in one half";
+                return MCRT_ERR_INVALID;
+            }
+        return MCRT_OK;
+    }
+
+    // Grows the context's denoiser scratch (the denoiser's, then the tiles' {nA, nB}, then {sum v', sum out^2}), uploads
+    // the tile counts and zeroes the sums. -> MCRT_OK with the device counts and sums.
+    int denoiseScratch(mcrt_ctx* ctx, uint64_t n_pixels, uint64_t n_tiles, const uint32_t* tile_samples, double** d_counts, double** d_sums)
+    {
+        const size_t dn_values = denoiseScratchValues((size_t)n_pixels);
+        const size_t scratch_values = dn_values + 2 * n_tiles + 2;
+        if (ctx->denoise_scratch_values < scratch_values)
+        {
+            if (ctx->d_denoise_scratch) cudaFree(ctx->d_denoise_scratch);
+            ctx->d_denoise_scratch = nullptr; ctx->denoise_scratch_values = 0;
+            CK(cudaMalloc((void**)&ctx->d_denoise_scratch, scratch_values * sizeof(double)));
+            ctx->denoise_scratch_values = scratch_values;
+        }
+        *d_counts = ctx->d_denoise_scratch + dn_values;
+        *d_sums = *d_counts + 2 * n_tiles;
+        const std::vector<double> counts(tile_samples, tile_samples + 2 * n_tiles);
+        CK(cudaMemcpyAsync(*d_counts, counts.data(), counts.size() * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+        CK(cudaMemsetAsync(*d_sums, 0, 2 * sizeof(double), ctx->stream));
+        return MCRT_OK;
+    }
+}
+
 int mcrt_denoise_dev(mcrt_ctx* ctx, const double* a_rgb_dev, const double* a_weight_dev,
                      const double* b_rgb_dev, const double* b_weight_dev, const uint32_t* tile_samples,
                      uint32_t tile, const double* features_dev, uint32_t width, uint32_t height,
@@ -2425,38 +2478,15 @@ int mcrt_denoise_dev(mcrt_ctx* ctx, const double* a_rgb_dev, const double* a_wei
         ctx->error = "mcrt_denoise_dev: weight sums must be given for both halves or for neither";
         return MCRT_ERR_INVALID;
     }
-    mcrt_denoise_params pr = { MCRT_DENOISE_DEFAULT_ITERATIONS, 0u, MCRT_DENOISE_DEFAULT_SIGMA_COLOR, MCRT_DENOISE_DEFAULT_SIGMA_NORMAL,
-                               MCRT_DENOISE_DEFAULT_SIGMA_DEPTH, MCRT_DENOISE_DEFAULT_SIGMA_ALBEDO };
-    if (params) pr = *params;
-    if (pr.iterations > MCRT_DENOISE_MAX_ITERATIONS) { ctx->error = "mcrt_denoise_dev: more than MCRT_DENOISE_MAX_ITERATIONS iterations"; return MCRT_ERR_INVALID; }
-    for (double sg : { pr.sigma_color, pr.sigma_normal, pr.sigma_depth, pr.sigma_albedo })
-        if (!std::isfinite(sg) || sg < 0.0) { ctx->error = "mcrt_denoise_dev: a sigma is negative or not finite"; return MCRT_ERR_INVALID; }
-    const uint64_t tiles_x = (width + tile - 1) / tile, tiles_y = (height + tile - 1) / tile;
-    const uint64_t n_tiles = tiles_x * tiles_y;
-    for (uint64_t t = 0; t < n_tiles; t++)
-        if (tile_samples[2 * t] == 0 || tile_samples[2 * t + 1] == 0)
-        {
-            ctx->error = "mcrt_denoise_dev: a tile has no samples in one half";
-            return MCRT_ERR_INVALID;
-        }
+    mcrt_denoise_params pr;
+    uint64_t n_tiles = 0;
+    if (int rc = denoiseCheck(ctx, "mcrt_denoise_dev", width, height, tile, tile_samples, params, &pr, &n_tiles)) return rc;
     CK(cudaSetDevice(ctx->device));
-    // scratch: the denoiser's, then the tiles' {nA, nB}, then {sum v', sum out^2}
-    const size_t dn_values = denoiseScratchValues((size_t)n_pixels);
-    const size_t scratch_values = dn_values + 2 * n_tiles + 2;
-    if (ctx->denoise_scratch_values < scratch_values)
-    {
-        if (ctx->d_denoise_scratch) cudaFree(ctx->d_denoise_scratch);
-        ctx->d_denoise_scratch = nullptr; ctx->denoise_scratch_values = 0;
-        CK(cudaMalloc((void**)&ctx->d_denoise_scratch, scratch_values * sizeof(double)));
-        ctx->denoise_scratch_values = scratch_values;
-    }
-    double* d_counts = ctx->d_denoise_scratch + dn_values;
-    double* d_sums = d_counts + 2 * n_tiles;
-    const std::vector<double> counts(tile_samples, tile_samples + 2 * n_tiles);
+    double *d_counts = nullptr, *d_sums = nullptr;
+    if (int rc = denoiseScratch(ctx, n_pixels, n_tiles, tile_samples, &d_counts, &d_sums)) return rc;
     cudaStream_t s = ctx->stream;
-    CK(cudaMemcpyAsync(d_counts, counts.data(), counts.size() * sizeof(double), cudaMemcpyHostToDevice, s));
-    CK(cudaMemsetAsync(d_sums, 0, 2 * sizeof(double), s));
-    const DenoiseInput in = { a_rgb_dev, a_weight_dev, b_rgb_dev, b_weight_dev, d_counts, features_dev, width, height, tile, (uint32_t)tiles_x };
+    const uint32_t tiles_x = (width + tile - 1) / tile;
+    const DenoiseInput in = { a_rgb_dev, a_weight_dev, b_rgb_dev, b_weight_dev, d_counts, features_dev, width, height, tile, tiles_x };
     const DenoiseSigmas sg = { pr.sigma_color, pr.sigma_normal, pr.sigma_depth, pr.sigma_albedo };
     launchDenoise(in, sg, pr.iterations, ctx->d_denoise_scratch, out_rgb_dev, d_sums, s);
     double sums[2] = { 0.0, 0.0 };
@@ -2464,6 +2494,77 @@ int mcrt_denoise_dev(mcrt_ctx* ctx, const double* a_rgb_dev, const double* a_wei
     CK(cudaStreamSynchronize(s));
     CK(cudaGetLastError());
     *frame_error = progressiveRelativeError(sums[0], sums[1], true);
+    return MCRT_OK;
+}
+
+int mcrt_denoise_planes_dev(mcrt_ctx* ctx, const double* a_rgb_dev, const double* b_rgb_dev,
+                            const double* a_planes_dev, const double* b_planes_dev, uint32_t n_planes,
+                            const uint32_t* tile_samples, uint32_t tile, const double* features_dev,
+                            uint32_t width, uint32_t height, const mcrt_denoise_params* params,
+                            double* a_out_planes_dev, double* b_out_planes_dev,
+                            double* out_rgb_dev, double* frame_error)
+{
+    if (!ctx) return MCRT_ERR_INVALID;
+    if (!a_rgb_dev || !b_rgb_dev || !a_planes_dev || !b_planes_dev || !tile_samples || !features_dev || !a_out_planes_dev ||
+        !b_out_planes_dev)
+    {
+        ctx->error = "mcrt_denoise_planes_dev: null buffer";
+        return MCRT_ERR_INVALID;
+    }
+    if (!out_rgb_dev != !frame_error)
+    {
+        ctx->error = "mcrt_denoise_planes_dev: out_rgb_dev and frame_error must be given together or not at all";
+        return MCRT_ERR_INVALID;
+    }
+    if (n_planes == 0) { ctx->error = "mcrt_denoise_planes_dev: n_planes is 0"; return MCRT_ERR_INVALID; }
+    mcrt_denoise_params pr;
+    uint64_t n_tiles = 0;
+    if (int rc = denoiseCheck(ctx, "mcrt_denoise_planes_dev", width, height, tile, tile_samples, params, &pr, &n_tiles)) return rc;
+    const uint64_t n_pixels = (uint64_t)width * height;
+    if (n_planes > (1ull << 40) / n_pixels)   // 48 TB of plane states: no device holds them, and the sizes below stay in range
+    {
+        ctx->error = "mcrt_denoise_planes_dev: more than 2^40 plane pixels";
+        return MCRT_ERR_INVALID;
+    }
+    // the outputs are written while the inputs are still read, and the plane outputs also hold plane states
+    const uintptr_t frame_bytes = 3 * sizeof(double) * n_pixels, planes_bytes = frame_bytes * n_planes;
+    struct Range { const void* p; uintptr_t bytes; };
+    const Range inputs[] = { { a_rgb_dev, frame_bytes }, { b_rgb_dev, frame_bytes }, { a_planes_dev, planes_bytes },
+                             { b_planes_dev, planes_bytes }, { features_dev, 8 * sizeof(double) * n_pixels } };
+    const Range outputs[] = { { a_out_planes_dev, planes_bytes }, { b_out_planes_dev, planes_bytes }, { out_rgb_dev, frame_bytes } };
+    auto overlap = [](const Range& u, const Range& v) {
+        const uintptr_t a = (uintptr_t)u.p, b = (uintptr_t)v.p;
+        return u.p && v.p && a < b + v.bytes && b < a + u.bytes;
+    };
+    for (int o = 0; o < 3; o++)
+    {
+        for (const Range& r : inputs)
+            if (overlap(outputs[o], r)) { ctx->error = "mcrt_denoise_planes_dev: an output buffer overlaps an input"; return MCRT_ERR_INVALID; }
+        for (int p = o + 1; p < 3; p++)
+            if (overlap(outputs[o], outputs[p])) { ctx->error = "mcrt_denoise_planes_dev: two output buffers overlap"; return MCRT_ERR_INVALID; }
+    }
+    CK(cudaSetDevice(ctx->device));
+    const size_t planes_values = denoisePlanesScratchValues((size_t)n_pixels, n_planes);
+    if (ctx->denoise_planes_scratch_values < planes_values)
+    {
+        if (ctx->d_denoise_planes_scratch) cudaFree(ctx->d_denoise_planes_scratch);
+        ctx->d_denoise_planes_scratch = nullptr; ctx->denoise_planes_scratch_values = 0;
+        CK(cudaMalloc((void**)&ctx->d_denoise_planes_scratch, planes_values * sizeof(double)));
+        ctx->denoise_planes_scratch_values = planes_values;
+    }
+    double *d_counts = nullptr, *d_sums = nullptr;
+    if (int rc = denoiseScratch(ctx, n_pixels, n_tiles, tile_samples, &d_counts, &d_sums)) return rc;
+    cudaStream_t s = ctx->stream;
+    const uint32_t tiles_x = (width + tile - 1) / tile;
+    const DenoiseInput in = { a_rgb_dev, nullptr, b_rgb_dev, nullptr, d_counts, features_dev, width, height, tile, tiles_x };
+    const DenoiseSigmas sg = { pr.sigma_color, pr.sigma_normal, pr.sigma_depth, pr.sigma_albedo };
+    const DenoisePlanes planes = { a_planes_dev, b_planes_dev, a_out_planes_dev, b_out_planes_dev, n_planes };
+    launchDenoisePlanes(in, planes, sg, pr.iterations, ctx->d_denoise_scratch, ctx->d_denoise_planes_scratch, out_rgb_dev, d_sums, s);
+    double sums[2] = { 0.0, 0.0 };
+    CK(cudaMemcpyAsync(sums, d_sums, sizeof(sums), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    CK(cudaGetLastError());
+    if (frame_error) *frame_error = progressiveRelativeError(sums[0], sums[1], true);
     return MCRT_OK;
 }
 
