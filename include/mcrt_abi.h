@@ -699,6 +699,14 @@ int mcrt_frame_free(mcrt_ctx* ctx, void* dev_ptr);
 int mcrt_bvh4_host(const mcrt_scene_desc* scene, uint32_t max_leaf, void** handle, const void** nodes128, uint32_t* n_nodes);
 void mcrt_bvh4_host_free(void* handle);
 
+/* Test hook (host only, no CUDA call): the 4-wide BVH with spatial splits that mcrt_scene_upload builds for small scenes
+ * (option bvh4_split). Nodes as mcrt_bvh4_host's, but a leaf's first / count index refs[], the ordered primitive of each
+ * reference; a primitive cut by a spatial split has several references. node_cost: cost of a node visit in primitive
+ * tests; ref_budget: references per primitive at most (>= 1). */
+int mcrt_bvh4_split_host(const mcrt_scene_desc* scene, double node_cost, double ref_budget, void** handle, const void** nodes128,
+                         uint32_t* n_nodes, const uint32_t** refs, uint32_t* n_refs);
+void mcrt_bvh4_split_host_free(void* handle);
+
 /* Measured FP64 issue rate of this GPU (independent DFMA chains on every SM), thread-instructions per second:
  * the denominator of bench.py's FP64 roofline for the float64 kernels. */
 int mcrt_fp64_peak(mcrt_ctx* ctx, double* dfma_per_second);

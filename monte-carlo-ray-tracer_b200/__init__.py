@@ -34,7 +34,7 @@ ABI_SYMBOLS = [
     "mcrt_bvh_build", "mcrt_bvh_free", "mcrt_image_tonemap", "mcrt_image_tonemap_dev",
     "mcrt_render_rows_strided_peers", "mcrt_frame_alloc", "mcrt_frame_open", "mcrt_frame_close", "mcrt_frame_free",
     "mcrt_render_film_sums_strided_dev", "mcrt_film_resolve_dev",
-    "mcrt_bvh4_host", "mcrt_bvh4_host_free",
+    "mcrt_bvh4_host", "mcrt_bvh4_host_free", "mcrt_bvh4_split_host", "mcrt_bvh4_split_host_free",
     "mcrt_fp64_peak", "mcrt_photon_emit_total", "mcrt_photon_emit_range", "mcrt_photon_build_dev",
     "mcrt_render_accumulate_dev", "mcrt_progressive_resolve_dev",
     "mcrt_render_accumulate_tiles_dev", "mcrt_progressive_resolve_tiles_dev",
@@ -263,6 +263,10 @@ def lib():
         L.mcrt_bvh4_host.argtypes = [C.POINTER(SceneDesc), C.c_uint32, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_uint32)]
         L.mcrt_bvh4_host_free.argtypes = [C.c_void_p]
         L.mcrt_bvh4_host_free.restype = None
+        L.mcrt_bvh4_split_host.argtypes = [C.POINTER(SceneDesc), C.c_double, C.c_double, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
+                                           C.POINTER(C.c_uint32), C.POINTER(C.c_void_p), C.POINTER(C.c_uint32)]
+        L.mcrt_bvh4_split_host_free.argtypes = [C.c_void_p]
+        L.mcrt_bvh4_split_host_free.restype = None
         L.mcrt_render_film_sums_strided_dev.argtypes = [C.c_void_p, C.POINTER(CameraRec), C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
                                                         C.c_uint32, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.POINTER(Stats)]
         L.mcrt_film_resolve_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]
@@ -1253,6 +1257,28 @@ def bvh4_host(scene, max_leaf=0xFFFFFFFF):
         return np.frombuffer(buf, dtype=BVH4_NODE_DTYPE).copy()
     finally:
         lib().mcrt_bvh4_host_free(h)
+
+
+BVH4_SPLIT_NODE_COST = 0.5      # abi.cu: the upload's defaults (MCRT_BVH4_SPLIT_COST overrides the cost there)
+BVH4_SPLIT_REF_BUDGET = 2.0
+
+
+def bvh4_split_host(scene, node_cost=BVH4_SPLIT_NODE_COST, ref_budget=BVH4_SPLIT_REF_BUDGET):
+    """The 4-wide BVH with spatial splits (option bvh4_split) -> (nodes as bvh4_host's, refs: the ordered primitive of each
+    reference a leaf's (first, count) indexes)."""
+    d = scene.desc()
+    h, p, n, r, nr = C.c_void_p(), C.c_void_p(), C.c_uint32(), C.c_void_p(), C.c_uint32()
+    rc = lib().mcrt_bvh4_split_host(C.byref(d), float(node_cost), float(ref_budget), C.byref(h), C.byref(p), C.byref(n), C.byref(r), C.byref(nr))
+    if rc:
+        raise McrtError(f"mcrt_bvh4_split_host failed with {rc}")
+    try:
+        if n.value == 0:
+            return np.zeros(0, BVH4_NODE_DTYPE), np.zeros(0, np.uint32)
+        nodes = np.frombuffer((C.c_uint8 * (128 * n.value)).from_address(p.value), dtype=BVH4_NODE_DTYPE).copy()
+        refs = np.frombuffer((C.c_uint8 * (4 * nr.value)).from_address(r.value), dtype=np.uint32).copy()
+        return nodes, refs
+    finally:
+        lib().mcrt_bvh4_split_host_free(h)
 
 
 def _lpe_strings(exprs):

@@ -7,6 +7,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <string>
 #include <vector>
 
@@ -69,7 +70,9 @@ struct mcrt_ctx
     float scene_scale = 1.0f;
     uint32_t n_bvh4_nodes = 0;
     uint32_t bvh4_max_leaf = 0xFFFFFFFFu;   // auto; 0: keep the reference's leaves; n: cut larger leaves into runs of n (option / MCRT_BVH4_MAX_LEAF)
-    int dynamic_fetch = -1;       // -1 auto (scenes with >= 2048 BVH4 nodes), 0 off, 1 on
+    int dynamic_fetch = -1;       // -1 auto (scenes with >= 2048 BVH4 nodes without spatial splits), 0 off, 1 on
+    int bvh4_split = -1;          // BVH4 with spatial splits (buildBvh4Split): -1 auto (below 4096 primitives, leaves cut by the auto rule), 0 off, 1 on
+    double bvh4_split_cost = 0.5; // buildBvh4Split's node cost in primitive tests (MCRT_BVH4_SPLIT_COST)
     PeerFrames peer_out{};   // n_frames != 0: the next resolve writes into these frames (mcrt_render_rows_strided_peers)
     int exact_traversal = 0;   // 1: every ray takes the reference-order replay (traverseReferenceOrder)
 
@@ -546,6 +549,290 @@ namespace
             too_big = emit(kids, self) != 0;
         }
         if (too_big) out.clear();   // a leaf with more than 255 primitives: the replay traversal handles the scene
+        return MCRT_OK;
+    }
+
+    // A BVH4 for traverseFast built anew with spatial splits (Stich, Friedrich and Dietrich, "Spatial Splits in Bounding Volume
+    // Hierarchies", HPG 2009): binned SAH over object and spatial splits, the binary tree collapsed to <= 4 children per node like
+    // buildBvh4's. A spatial split cuts a primitive into references with a box each, clipped to its part of the primitive: a large
+    // triangle lying diagonally to the axes (the hexagon room's walls) is then tested only by rays that come near it. Leaf
+    // references (first, count) index `refs`, which maps each reference to its ordered primitive. The search stays exact because
+    // the float boxes conservatively contain what they hold: every point of a primitive lies in the box of at least one of its
+    // references. Triangles are clipped in float64 and each clipped coordinate is widened by a bound on its rounding error
+    // (2^-40 of the magnitudes involved, and more where an edge crosses the plane at a grazing angle); spheres keep their box
+    // intersected with the cuts (interval operations, exact); quadrics are never split. `node_cost` is the cost of visiting a
+    // node (four box tests) in float64 primitive tests; references are capped at `ref_budget` times the primitive count.
+    int buildBvh4Split(const mcrt_scene_desc& s, double node_cost, double ref_budget, std::vector<Bvh4Node>& out, std::vector<uint32_t>& refs)
+    {
+        out.clear(); refs.clear();
+        if (s.n_nodes == 0 || s.n_prims == 0 || s.n_prims >= BVH4_MAX_PRIMS) return MCRT_OK;
+        auto lower = [](double v) { float r = (float)v; if ((double)r > v) r = std::nextafter(r, -INFINITY); return r; };
+        auto upper = [](double v) { float r = (float)v; if ((double)r < v) r = std::nextafter(r, INFINITY); return r; };
+        struct Ref { uint32_t prim; double b[6]; };
+        struct SNode { double b[6]; int32_t kid[2]; uint32_t first, count; };   // kid[0] < 0: leaf over refs[first, first + count)
+        constexpr int NB = 32;
+        constexpr uint32_t MAX_LEAF = 2;
+        const double eps = std::ldexp(1.0, -40);
+        auto empty = [](double* b) { for (int k = 0; k < 3; k++) { b[k] = 1e300; b[3 + k] = -1e300; } };
+        auto grow = [](double* b, const double* c) { for (int k = 0; k < 3; k++) { b[k] = std::min(b[k], c[k]); b[3 + k] = std::max(b[3 + k], c[3 + k]); } };
+        auto area = [](const double* b) { const double x = b[3] - b[0], y = b[4] - b[1], z = b[5] - b[2]; return (x < 0 || y < 0 || z < 0) ? 0.0 : x * y + y * z + z * x; };
+        auto isEmpty = [](const double* b) { return b[0] > b[3] || b[1] > b[4] || b[2] > b[5]; };
+        auto vert = [&](const double* base, uint32_t idx, double* p) { for (int k = 0; k < 3; k++) p[k] = base[3 * (size_t)idx + k]; };
+
+        // The part of primitive `prim` inside the box c (the reference's box with one face moved to a cut), boxed conservatively.
+        auto clip = [&](uint32_t prim, const double* c, double* out_b)
+        {
+            empty(out_b);
+            const uint32_t type = s.prim_type[prim], idx = s.prim_index[prim];
+            if (type == MCRT_PRIM_TRIANGLE)
+            {
+                // Sutherland-Hodgman against the six planes of c; every vertex carries its error bound
+                struct P { double x[3]; double e; };
+                P poly[16], next[16];
+                int n = 3;
+                vert(s.tri_v0, idx, poly[0].x); vert(s.tri_v1, idx, poly[1].x); vert(s.tri_v2, idx, poly[2].x);
+                for (int i = 0; i < 3; i++) poly[i].e = 0.0;
+                for (int plane = 0; plane < 6 && n > 0; plane++)
+                {
+                    const int k = plane % 3;
+                    const bool is_lo = plane < 3;
+                    const double pos = c[plane];
+                    auto inside = [&](const P& p) { return is_lo ? p.x[k] >= pos : p.x[k] <= pos; };
+                    int m = 0;
+                    for (int i = 0; i < n; i++)
+                    {
+                        const P& a = poly[i];
+                        const P& b = poly[(i + 1) % n];
+                        const bool ia = inside(a), ib = inside(b);
+                        if (ia) next[m++] = a;
+                        if (ia != ib)
+                        {
+                            const double den = b.x[k] - a.x[k];
+                            const double t = std::min(1.0, std::max(0.0, (pos - a.x[k]) / den));
+                            P q;
+                            double span = 0.0;
+                            for (int j = 0; j < 3; j++) { q.x[j] = a.x[j] + t * (b.x[j] - a.x[j]); span = std::max(span, std::fabs(b.x[j] - a.x[j])); }
+                            q.x[k] = pos;
+                            const double mag = std::fabs(pos) + std::fabs(a.x[k]) + std::fabs(b.x[k]);
+                            q.e = std::max(a.e, b.e) + span * std::min(1.0, eps * mag / std::fabs(den)) +
+                                  eps * (std::fabs(q.x[0]) + std::fabs(q.x[1]) + std::fabs(q.x[2]) + span);
+                            next[m++] = q;
+                        }
+                    }
+                    n = m;
+                    for (int i = 0; i < n; i++) poly[i] = next[i];
+                }
+                for (int i = 0; i < n; i++)
+                    for (int k = 0; k < 3; k++)
+                    {
+                        out_b[k] = std::min(out_b[k], poly[i].x[k] - poly[i].e - eps * std::fabs(poly[i].x[k]));
+                        out_b[3 + k] = std::max(out_b[3 + k], poly[i].x[k] + poly[i].e + eps * std::fabs(poly[i].x[k]));
+                    }
+            }
+            else
+            {
+                const double* sp = s.sphere_origin_radius + 4 * (size_t)idx;
+                for (int k = 0; k < 3; k++) { out_b[k] = sp[k] - sp[3]; out_b[3 + k] = sp[k] + sp[3]; }
+            }
+            // never outside c: every point of the primitive inside c is inside this
+            for (int k = 0; k < 3; k++) { out_b[k] = std::max(out_b[k], c[k]); out_b[3 + k] = std::min(out_b[3 + k], c[3 + k]); }
+        };
+        // ref cut at `pos` on axis k -> left / right parts (an empty box: nothing of the primitive on that side)
+        auto cut = [&](const Ref& r, int k, double pos, Ref& l, Ref& rr)
+        {
+            double c[6];
+            l.prim = rr.prim = r.prim;
+            std::memcpy(c, r.b, sizeof(c)); c[3 + k] = std::min(c[3 + k], pos); clip(r.prim, c, l.b);
+            std::memcpy(c, r.b, sizeof(c)); c[k] = std::max(c[k], pos); clip(r.prim, c, rr.b);
+        };
+
+        std::vector<Ref> all(s.n_prims);
+        bool quadrics = false;
+        for (uint32_t i = 0; i < s.n_prims; i++)
+        {
+            Ref& r = all[i];
+            r.prim = i;
+            const uint32_t type = s.prim_type[i], idx = s.prim_index[i];
+            if (type == MCRT_PRIM_TRIANGLE)
+            {
+                double v[3][3];
+                vert(s.tri_v0, idx, v[0]); vert(s.tri_v1, idx, v[1]); vert(s.tri_v2, idx, v[2]);
+                for (int k = 0; k < 3; k++) { r.b[k] = std::min(v[0][k], std::min(v[1][k], v[2][k])); r.b[3 + k] = std::max(v[0][k], std::max(v[1][k], v[2][k])); }
+            }
+            else if (type == MCRT_PRIM_SPHERE)
+            {
+                const double* sp = s.sphere_origin_radius + 4 * (size_t)idx;
+                for (int k = 0; k < 3; k++) { r.b[k] = sp[k] - sp[3]; r.b[3 + k] = sp[k] + sp[3]; }
+            }
+            else { quadrics = true; for (int k = 0; k < 6; k++) r.b[k] = s.quadric_bounds[6 * (size_t)idx + k]; }
+        }
+        const size_t budget = (size_t)(ref_budget * s.n_prims);
+        size_t n_refs = all.size();
+        std::vector<SNode> nodes;
+
+        // binary SBVH, depth first; returns the node index
+        std::function<int32_t(std::vector<Ref>&)> build = [&](std::vector<Ref>& rs) -> int32_t
+        {
+            SNode nd;
+            empty(nd.b);
+            for (const Ref& r : rs) grow(nd.b, r.b);
+            nd.kid[0] = nd.kid[1] = -1; nd.first = 0; nd.count = (uint32_t)rs.size();
+            const int32_t self = (int32_t)nodes.size();
+            nodes.push_back(nd);
+            const size_t n = rs.size();
+            auto makeLeaf = [&]() { nodes[self].first = (uint32_t)refs.size(); for (const Ref& r : rs) refs.push_back(r.prim); return self; };
+            if (n <= 1) return makeLeaf();
+            const double pa = std::max(area(nd.b), 1e-300);
+            double best = INFINITY; int best_axis = -1, best_bin = -1; bool best_spatial = false;
+            double cbox[6]; empty(cbox);
+            for (const Ref& r : rs) for (int k = 0; k < 3; k++) { const double cc = 0.5 * (r.b[k] + r.b[3 + k]); cbox[k] = std::min(cbox[k], cc); cbox[3 + k] = std::max(cbox[3 + k], cc); }
+            auto centroidBin = [&](const Ref& r, int k) { const double ext = cbox[3 + k] - cbox[k]; int b = (int)(NB * ((0.5 * (r.b[k] + r.b[3 + k]) - cbox[k]) / ext)); return std::min(NB - 1, std::max(0, b)); };
+            // object splits: centroid bins
+            for (int k = 0; k < 3; k++)
+            {
+                if (!(cbox[3 + k] > cbox[k])) continue;
+                double bb[NB][6]; uint32_t cnt[NB] = {};
+                for (int b = 0; b < NB; b++) empty(bb[b]);
+                for (const Ref& r : rs) { const int b = centroidBin(r, k); grow(bb[b], r.b); cnt[b]++; }
+                double right[NB][6]; uint32_t rc[NB];
+                double acc[6]; empty(acc); uint32_t ac = 0;
+                for (int b = NB - 1; b >= 1; b--) { grow(acc, bb[b]); ac += cnt[b]; std::memcpy(right[b], acc, sizeof(acc)); rc[b] = ac; }
+                empty(acc); ac = 0;
+                for (int b = 0; b < NB - 1; b++)
+                {
+                    grow(acc, bb[b]); ac += cnt[b];
+                    if (ac == 0 || rc[b + 1] == 0) continue;
+                    const double cost = node_cost + (area(acc) * ac + area(right[b + 1]) * rc[b + 1]) / pa;
+                    if (cost < best) { best = cost; best_axis = k; best_bin = b; best_spatial = false; }
+                }
+            }
+            // spatial splits: bins over the node's box, references chopped at every bin boundary they cross
+            bool has_quadric = false;
+            if (quadrics) for (const Ref& r : rs) has_quadric |= s.prim_type[r.prim] == MCRT_PRIM_QUADRIC;
+            if (!has_quadric && n_refs + n <= budget)
+            {
+                for (int k = 0; k < 3; k++)
+                {
+                    const double lo = nd.b[k], ext = nd.b[3 + k] - nd.b[k];
+                    if (!(ext > 0.0)) continue;
+                    auto plane = [&](int b) { return lo + ext * b / NB; };
+                    auto binOf = [&](double x) { return std::min(NB - 1, std::max(0, (int)(NB * ((x - lo) / ext)))); };
+                    double bb[NB][6]; uint32_t enter[NB] = {}, leave[NB] = {};
+                    for (int b = 0; b < NB; b++) empty(bb[b]);
+                    for (const Ref& r : rs)
+                    {
+                        const int b0 = binOf(r.b[k]), b1 = binOf(r.b[3 + k]);
+                        enter[b0]++; leave[b1]++;
+                        Ref cur = r, l, rr;
+                        for (int b = b0; b < b1; b++)
+                        {
+                            cut(cur, k, plane(b + 1), l, rr);
+                            if (!isEmpty(l.b)) grow(bb[b], l.b);
+                            cur = rr;
+                            if (isEmpty(cur.b)) break;
+                        }
+                        if (!isEmpty(cur.b)) grow(bb[b1], cur.b);
+                    }
+                    double right[NB][6]; uint32_t rc[NB];
+                    double acc[6]; empty(acc); uint32_t ac = 0;
+                    for (int b = NB - 1; b >= 1; b--) { grow(acc, bb[b]); ac += leave[b]; std::memcpy(right[b], acc, sizeof(acc)); rc[b] = ac; }
+                    empty(acc); ac = 0;
+                    for (int b = 0; b < NB - 1; b++)
+                    {
+                        grow(acc, bb[b]); ac += enter[b];
+                        if (ac == 0 || rc[b + 1] == 0 || (ac == n && rc[b + 1] == n)) continue;
+                        const double cost = node_cost + (area(acc) * ac + area(right[b + 1]) * rc[b + 1]) / pa;
+                        if (cost < best) { best = cost; best_axis = k; best_bin = b; best_spatial = true; }
+                    }
+                }
+            }
+            if (n <= MAX_LEAF && (double)n <= best) return makeLeaf();
+            std::vector<Ref> ls, rrs;
+            if (best_spatial)
+            {
+                const int k = best_axis;
+                const double lo = nd.b[k], ext = nd.b[3 + k] - nd.b[k];
+                const double pos = lo + ext * (best_bin + 1) / NB;
+                for (const Ref& r : rs)
+                {
+                    if (r.b[3 + k] <= pos) ls.push_back(r);
+                    else if (r.b[k] >= pos) rrs.push_back(r);
+                    else
+                    {
+                        Ref l, rr;
+                        cut(r, k, pos, l, rr);
+                        if (!isEmpty(l.b)) ls.push_back(l);
+                        if (!isEmpty(rr.b)) rrs.push_back(rr);
+                    }
+                }
+                if (ls.empty() || rrs.empty() || (ls.size() == n && rrs.size() == n)) { ls.clear(); rrs.clear(); }
+                else n_refs += ls.size() + rrs.size() - n;
+            }
+            else if (best_axis >= 0)
+            {
+                for (const Ref& r : rs) (centroidBin(r, best_axis) <= best_bin ? ls : rrs).push_back(r);
+            }
+            if (ls.empty() || rrs.empty())
+            {
+                // no usable split (coincident centroids): halves in centroid order along the widest axis
+                ls.clear(); rrs.clear();
+                int k = 0;
+                for (int j = 1; j < 3; j++) if (nd.b[3 + j] - nd.b[j] > nd.b[3 + k] - nd.b[k]) k = j;
+                std::vector<Ref> sorted = rs;
+                std::stable_sort(sorted.begin(), sorted.end(), [&](const Ref& a, const Ref& b) { return a.b[k] + a.b[3 + k] < b.b[k] + b.b[3 + k]; });
+                ls.assign(sorted.begin(), sorted.begin() + n / 2);
+                rrs.assign(sorted.begin() + n / 2, sorted.end());
+            }
+            rs.clear(); rs.shrink_to_fit();
+            const int32_t l = build(ls);
+            const int32_t r = build(rrs);
+            nodes[self].kid[0] = l; nodes[self].kid[1] = r;
+            return self;
+        };
+        build(all);
+        if (refs.size() >= BVH4_MAX_PRIMS) { out.clear(); refs.clear(); return MCRT_OK; }
+
+        // collapse to 4-wide nodes: pull up the grandchildren of the largest inner child while there is room, breadth first
+        auto isInner = [&](int32_t i) { return nodes[i].kid[0] >= 0; };
+        struct Pending { int32_t node; uint32_t parent, slot; };
+        std::vector<Pending> queue;
+        auto emit = [&](int32_t bnode, uint32_t self)
+        {
+            std::vector<int32_t> kids;
+            if (isInner(bnode)) kids = { nodes[bnode].kid[0], nodes[bnode].kid[1] };
+            else kids = { bnode };   // the root is a leaf
+            while (kids.size() < 4)
+            {
+                int pick = -1; double pick_area = -1.0;
+                for (size_t i = 0; i < kids.size(); i++)
+                    if (isInner(kids[i]) && area(nodes[kids[i]].b) > pick_area) { pick_area = area(nodes[kids[i]].b); pick = (int)i; }
+                if (pick < 0) break;
+                const int32_t c = kids[pick];
+                kids[pick] = nodes[c].kid[0];
+                kids.insert(kids.begin() + pick + 1, nodes[c].kid[1]);
+            }
+            Bvh4Node n;
+            std::memset(&n, 0, sizeof(n));
+            for (int c = 0; c < 4; c++) for (int k = 0; k < 3; k++) { n.lo[k][c] = 3.0e38f; n.hi[k][c] = -3.0e38f; }
+            for (size_t c = 0; c < kids.size(); c++)
+            {
+                const SNode& sn = nodes[kids[c]];
+                for (int k = 0; k < 3; k++) { n.lo[k][c] = lower(sn.b[k]); n.hi[k][c] = upper(sn.b[3 + k]); }
+                if (!isInner(kids[c])) n.child[c] = BVH4_LEAF | (sn.first << 8) | sn.count;
+                else queue.push_back({ kids[c], self, (uint32_t)c });
+            }
+            out[self] = n;
+        };
+        out.emplace_back();
+        emit(0, 0);
+        for (size_t q = 0; q < queue.size(); q++)
+        {
+            const Pending pn = queue[q];
+            const uint32_t self = (uint32_t)out.size();
+            out.emplace_back();
+            out[pn.parent].child[pn.slot] = self;
+            emit(pn.node, self);
+        }
         return MCRT_OK;
     }
 
@@ -1145,6 +1432,8 @@ int mcrt_init(int device, mcrt_ctx** out_ctx)
     if (cudaGetDeviceCount(&count) != cudaSuccess || device < 0 || device >= count) return MCRT_ERR_CUDA;
     mcrt_ctx* ctx = new mcrt_ctx();
     if (const char* e = std::getenv("MCRT_BVH4_MAX_LEAF")) ctx->bvh4_max_leaf = (uint32_t)std::atoi(e);   // tuning experiments
+    if (const char* e = std::getenv("MCRT_BVH4_SPLIT")) ctx->bvh4_split = std::atoi(e);
+    if (const char* e = std::getenv("MCRT_BVH4_SPLIT_COST")) ctx->bvh4_split_cost = std::atof(e);
     ctx->device = device;
     auto fail = [&](int rc) { mcrt_destroy(ctx); return rc; };
     if (cudaSetDevice(device) != cudaSuccess) return fail(MCRT_ERR_CUDA);
@@ -1226,6 +1515,7 @@ int mcrt_set_option(mcrt_ctx* ctx, const char* key, double value)
     else if (k == "sort_prim_key") { ctx->sort_prim_key = (int)value; }
     else if (k == "exact_traversal") { ctx->exact_traversal = value != 0.0; }
     else if (k == "dynamic_fetch") { ctx->dynamic_fetch = (int)value; }
+    else if (k == "bvh4_split") { if (value < -1 || value > 1) return MCRT_ERR_INVALID; ctx->bvh4_split = (int)value; }   // takes effect at the next mcrt_scene_upload
     else if (k == "bvh4_max_leaf") { if (value < 0 || value > 255) return MCRT_ERR_INVALID; ctx->bvh4_max_leaf = (uint32_t)value; }   // takes effect at the next mcrt_scene_upload
     else { ctx->error = "unknown option " + k; return MCRT_ERR_INVALID; }
     return MCRT_OK;
@@ -1309,9 +1599,36 @@ int mcrt_scene_upload(mcrt_ctx* ctx, const mcrt_scene_desc* scene, uint64_t* h2d
         if ((rc = uploadArrays(ctx, s, a, bytes))) return rc;
         std::vector<Bvh4Node> bvh4;
         if ((rc = buildBvh4(ctx->bvh4_max_leaf, s, bvh4))) return rc;
-        a.dev.bvh4 = nullptr;
-        if (!bvh4.empty() && (rc = devUpload(ctx, ctx->scene_allocs, &a.dev.bvh4, bvh4, bytes))) return rc;
-        ctx->n_bvh4_nodes = (uint32_t)bvh4.size();
+        ctx->n_bvh4_nodes = (uint32_t)bvh4.size();   // dynamic fetch's auto rule counts the tree without spatial splits
+        a.dev.bvh4 = nullptr; a.dev.bvh4_geom = nullptr; a.dev.bvh4_prim = nullptr;
+        std::vector<uint32_t> refs;
+        std::vector<V4<double>> ref_geom;
+        if (!bvh4.empty())
+        {
+            // spatial splits where buildBvh4 cuts the reference's leaves (small scenes); big scenes keep the reference's leaves
+            const bool split = ctx->bvh4_split < 0 ? ctx->bvh4_max_leaf == 0xFFFFFFFFu && s.n_prims < 4096u : ctx->bvh4_split != 0;
+            if (split)
+            {
+                std::vector<Bvh4Node> split_nodes;
+                if ((rc = buildBvh4Split(s, ctx->bvh4_split_cost, 2.0, split_nodes, refs))) return rc;
+                if (!split_nodes.empty()) bvh4.swap(split_nodes);
+                else refs.clear();
+            }
+            if (refs.empty())
+            {
+                refs.resize(s.n_prims);
+                for (uint32_t i = 0; i < s.n_prims; i++) refs[i] = i;
+                a.dev.bvh4_geom = a.dev.geom;
+            }
+            else
+            {
+                ref_geom.resize(3 * refs.size());
+                for (size_t r = 0; r < refs.size(); r++) for (int j = 0; j < 3; j++) ref_geom[3 * r + j] = a.geom[3 * (size_t)refs[r] + j];
+                if ((rc = devUpload(ctx, ctx->scene_allocs, &a.dev.bvh4_geom, ref_geom, bytes))) return rc;
+            }
+            if ((rc = devUpload(ctx, ctx->scene_allocs, &a.dev.bvh4_prim, refs, bytes))) return rc;
+            if ((rc = devUpload(ctx, ctx->scene_allocs, &a.dev.bvh4, bvh4, bytes))) return rc;
+        }
         CK(cudaStreamSynchronize(ctx->stream)); // host vectors die at scope exit
         ctx->scene64 = a.dev;
     }
@@ -2592,6 +2909,27 @@ int mcrt_bvh4_host(const mcrt_scene_desc* scene, uint32_t max_leaf, void** handl
 void mcrt_bvh4_host_free(void* handle)
 {
     delete static_cast<std::vector<Bvh4Node>*>(handle);
+}
+
+namespace
+{
+    struct Bvh4SplitHost { std::vector<Bvh4Node> nodes; std::vector<uint32_t> refs; };
+}
+
+int mcrt_bvh4_split_host(const mcrt_scene_desc* scene, double node_cost, double ref_budget, void** handle, const void** nodes128,
+                         uint32_t* n_nodes, const uint32_t** refs, uint32_t* n_refs)
+{
+    if (!scene || !handle || !nodes128 || !n_nodes || !refs || !n_refs || !(node_cost >= 0.0) || !(ref_budget >= 1.0)) return MCRT_ERR_INVALID;
+    auto* v = new Bvh4SplitHost();
+    const int rc = buildBvh4Split(*scene, node_cost, ref_budget, v->nodes, v->refs);
+    if (rc) { delete v; return rc; }
+    *handle = v; *nodes128 = v->nodes.data(); *n_nodes = (uint32_t)v->nodes.size(); *refs = v->refs.data(); *n_refs = (uint32_t)v->refs.size();
+    return MCRT_OK;
+}
+
+void mcrt_bvh4_split_host_free(void* handle)
+{
+    delete static_cast<Bvh4SplitHost*>(handle);
 }
 
 int mcrt_lpe_compile_host(const char* const* exprs, uint32_t n, uint32_t n_groups, uint8_t* next, uint32_t* accept,

@@ -90,23 +90,24 @@ namespace mcrt
         return r;
     }
 
-    // One ordered primitive against the ray with the reference's float64 arithmetic (no acceptance rule)
+    // One primitive record of `geom` (sc.geom: ordered primitives, sc.bvh4_geom: leaf references) against the ray with the
+    // reference's float64 arithmetic (no acceptance rule)
     template <int PRIMS, class R>
-    MCRT_D bool intersectPrim(const DeviceScene<R>& sc, uint32_t prim, const RayQ<R>& ray, R& t, R& u, R& v, bool& is_triangle)
+    MCRT_D bool intersectPrim(const DeviceScene<R>& sc, const V4<R>* __restrict__ geom, uint32_t prim, const RayQ<R>& ray, R& t, R& u, R& v, bool& is_triangle)
     {
-        const V4<R> g0 = sc.geom[3 * prim + 0];
+        const V4<R> g0 = geom[3 * prim + 0];
         const uint32_t type = PRIMS == PRIMS_TRI ? (uint32_t)PRIM_TRIANGLE : (uint32_t)g0.w;
         u = R(0); v = R(0);
         is_triangle = type == PRIM_TRIANGLE;
         if (type == PRIM_TRIANGLE)
         {
-            const V4<R> g1 = sc.geom[3 * prim + 1];
-            const V4<R> g2 = sc.geom[3 * prim + 2];
+            const V4<R> g1 = geom[3 * prim + 1];
+            const V4<R> g2 = geom[3 * prim + 2];
             return intersectTriangle(g0, g1, g2, ray, t, u, v);
         }
         else if (PRIMS == PRIMS_TRI_SPHERE || type == PRIM_SPHERE)
         {
-            const V4<R> g1 = sc.geom[3 * prim + 1];
+            const V4<R> g1 = geom[3 * prim + 1];
             return intersectSphere(g0, g1, ray, t);
         }
         else
@@ -168,7 +169,7 @@ namespace mcrt
             double t, u, v;
             bool is_tri;
             cnt.prim_tests++;
-            if (!intersectPrim<PRIMS>(sc, target_prim, ray, t, u, v, is_tri)) return false;
+            if (!intersectPrim<PRIMS>(sc, sc.geom, target_prim, ray, t, u, v, is_tri)) return false;
             best.t = t; best.u = u; best.v = v; best.prim = target_prim;
             degenerate = degenerateDirection(ray.d) || (is_tri && onTriangleBoundary(u, v, t, (double)sc.scene_scale));
             if (degenerate) { verdict = 2u; return true; }     // step() is not entered: see traceManyFast / traceVisible
@@ -258,7 +259,10 @@ namespace mcrt
             return true;
         }
 
-        // The primitives of one leaf. -> false: the search is over (OCC only: an occluder or a tie was found).
+        // The primitives of one leaf: references i into sc.bvh4_geom / sc.bvh4_prim. A primitive cut by a spatial split has a
+        // reference in several leaves, and each test of it gives a bit-identical t: such a repeat is not a competitor of the best
+        // hit, and the target of an occlusion query is skipped by its ordered id. -> false: the search is over (OCC only: an
+        // occluder or a tie was found).
         MCRT_D bool testLeaf(uint32_t leaf, const DeviceScene<double>& sc, const RayQ<double>& ray, TraceCounters& cnt)
         {
             const uint32_t first = (leaf >> 8) & (BVH4_MAX_PRIMS - 1u), count = leaf & 0xFFu;
@@ -268,8 +272,8 @@ namespace mcrt
                 bool is_tri;
                 if constexpr (OCC)
                 {
-                    if (i == target) continue;
-                    if (intersectPrim<PRIMS>(sc, i, ray, t, u, v, is_tri))
+                    if (__ldg(sc.bvh4_prim + i) == target) continue;
+                    if (intersectPrim<PRIMS>(sc, sc.bvh4_geom, i, ray, t, u, v, is_tri))
                     {
                         const double delta = ambiguityDelta(best.t, (double)sc.scene_scale);
                         // an occluder hit on its own boundary may be one the reference never reaches: replay
@@ -279,16 +283,16 @@ namespace mcrt
                     }
                     continue;
                 }
-                if (intersectPrim<PRIMS>(sc, i, ray, t, u, v, is_tri))
+                if (intersectPrim<PRIMS>(sc, sc.bvh4_geom, i, ray, t, u, v, is_tri))
                 {
                     if (t < best.t)
                     {
                         second_t = best.t;
-                        best.t = t; best.u = u; best.v = v; best.prim = i;
+                        best.t = t; best.u = u; best.v = v; best.prim = __ldg(sc.bvh4_prim + i);
                         best.interpolate = (is_tri && onTriangleBoundary(u, v, t, (double)sc.scene_scale)) ? 1u : 0u;   // scratch use: winner on its boundary
                         limit = __double2float_ru(t + 2.0 * ambiguityDelta(t, (double)sc.scene_scale));
                     }
-                    else if (t < second_t)
+                    else if (t < second_t && !(t == best.t && __ldg(sc.bvh4_prim + i) == best.prim))
                     {
                         second_t = t;
                     }

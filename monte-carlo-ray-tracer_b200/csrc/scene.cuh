@@ -11,6 +11,9 @@
 //   geom      3 × V4<R> per ordered primitive = the 48 B (float) / 96 B (double) intersection
 //             record: triangle {v0,type | E1 | E2}, sphere {origin,type | radius | -},
 //             quadric {index,type | - | -}. Indexed by ordered-primitive id: no indirection.
+//   bvh4_geom the same records in the order of the BVH4's leaf references, so that a leaf's primitives
+//             are contiguous also where spatial splits give a primitive several references (bvh4.cuh);
+//             bvh4_prim maps each reference back to its ordered primitive.
 //   shade     per ordered primitive: geometric normal (triangles), material id, vertex-normal id,
 //             area, light id.
 //   vnormals  3 × V4<R> per smooth triangle.
@@ -95,6 +98,8 @@ namespace mcrt
     template <class R> struct DeviceScene
     {
         const Bvh4Node* bvh4;    // 4-wide float-box BVH of the order-free search (parity mode); null: replay traversal only
+        const V4<R>* bvh4_geom;      // geom records in the order of bvh4's leaf references (geom itself when no primitive is split)
+        const uint32_t* bvh4_prim;   // ordered primitive of each leaf reference of bvh4
         const WideChild<R>* wide;
         const V4<R>* geom;
         const PrimShade<R>* shade;
