@@ -260,7 +260,7 @@ namespace
     };
 
     // optional cross-check of every Scene::intersect call of a render against the order-free search (oracle_render_rows_checked)
-    struct SearchCheck { const void* nodes; double scale; uint64_t calls, flagged, mismatches; };
+    struct SearchCheck { const void* nodes; const uint32_t* refs; double scale; uint64_t calls, flagged, mismatches; };
     SearchCheck* g_search_check = nullptr;
     Isect intersectReferenceOrder(const Scene& s, const Ray& r, uint64_t* counter, size_t* peak = nullptr);
     void (*g_cross_fn)(const Scene& s, const Ray& r, const Isect& ref) = nullptr;
@@ -838,8 +838,11 @@ namespace
         }
     }
 
-    Isect searchFast(const Scene& s, const Node4* nodes, const Ray& r, double scene_scale, bool& ambiguous, uint64_t& box_tests, uint64_t& prim_tests,
-                     size_t* peak = nullptr)
+    // refs: the ordered primitive of each leaf reference (a tree with spatial splits, mcrt_bvh4_split_host); null: leaves index ordered
+    // primitives. A primitive with several references gives the same t at each: a repeat of the best primitive is not its competitor
+    // (FastSearch::testLeaf).
+    Isect searchFast(const Scene& s, const Node4* nodes, const uint32_t* refs, const Ray& r, double scene_scale, bool& ambiguous, uint64_t& box_tests,
+                     uint64_t& prim_tests, size_t* peak = nullptr)
     {
         const FastRay4 f = fastRay(r);
         Isect best;
@@ -852,13 +855,14 @@ namespace
             const uint32_t first = (cur >> 8) & 0x7FFFFFu, count = cur & 0xFFu;
             for (uint32_t i = first; i < first + count; i++)
             {
+                const uint32_t prim = refs ? refs[i] : i;
                 Isect c;
                 prim_tests++;
                 double eu = 0.5, ev = 0.25;
-                if (hitPrimUV(s, i, r, c, eu, ev))
+                if (hitPrimUV(s, prim, r, c, eu, ev))
                 {
-                    if (c.t < best.t) { second_t = best.t; best = c; best.prim = i; best_edge = onBoundary(eu, ev, c.t, scene_scale); limit = roundUpToFloat(c.t + 2.0 * ambiguityDelta(c.t, scene_scale)); }
-                    else if (c.t < second_t) second_t = c.t;
+                    if (c.t < best.t) { second_t = best.t; best = c; best.prim = prim; best_edge = onBoundary(eu, ev, c.t, scene_scale); limit = roundUpToFloat(c.t + 2.0 * ambiguityDelta(c.t, scene_scale)); }
+                    else if (c.t < second_t && !(c.t == best.t && prim == best.prim)) second_t = c.t;
                 }
             }
             return true;
@@ -876,7 +880,7 @@ namespace
 // 1: something lies in front of it (or the ray misses the target itself), 2: a tie within delta -> the product replays the ray.
 namespace
 {
-    int searchVisible(const Scene& s, const Node4* nodes, const Ray& r, double scene_scale, uint32_t target, double& t_target)
+    int searchVisible(const Scene& s, const Node4* nodes, const uint32_t* refs, const Ray& r, double scene_scale, uint32_t target, double& t_target)
     {
         Isect tgt;
         double tu = 0.5, tv = 0.25;
@@ -899,10 +903,11 @@ namespace
                 const uint32_t first = (cur >> 8) & 0x7FFFFFu, count = cur & 0xFFu;
                 for (uint32_t i = first; i < first + count; i++)
                 {
-                    if (i == target) continue;
+                    const uint32_t prim = refs ? refs[i] : i;
+                    if (prim == target) continue;      // every reference of the target, by its ordered id
                     Isect c;
                     double cu = 0.5, cv = 0.25;
-                    if (hitPrimUV(s, i, r, c, cu, cv))
+                    if (hitPrimUV(s, prim, r, c, cu, cv))
                     {
                         if (c.t <= tgt.t + delta && onBoundary(cu, cv, c.t, scene_scale)) return 2;   // an occluder hit on its edge: the reference may have missed it
                         if (c.t < tgt.t - delta) return 1;
@@ -933,7 +938,8 @@ namespace
 // verdict equals searchVisible's unless a ray holds both an occluder and a tie (either is a correct verdict: both keep the reference's answer).
 namespace
 {
-    int searchVisibleOrdered(const Scene& s, const Node4* nodes, const Ray& r, double scene_scale, uint32_t target, double& t_target, size_t& peak)
+    int searchVisibleOrdered(const Scene& s, const Node4* nodes, const uint32_t* refs, const Ray& r, double scene_scale, uint32_t target, double& t_target,
+                             size_t& peak)
     {
         Isect tgt;
         double tu = 0.5, tv = 0.25;
@@ -950,10 +956,11 @@ namespace
             const uint32_t first = (cur >> 8) & 0x7FFFFFu, count = cur & 0xFFu;
             for (uint32_t i = first; i < first + count; i++)
             {
-                if (i == target) continue;
+                const uint32_t prim = refs ? refs[i] : i;
+                if (prim == target) continue;
                 Isect c;
                 double cu = 0.5, cv = 0.25;
-                if (hitPrimUV(s, i, r, c, cu, cv))
+                if (hitPrimUV(s, prim, r, c, cu, cv))
                 {
                     if (c.t <= tgt.t + delta && onBoundary(cu, cv, c.t, scene_scale)) { verdict = 2; return false; }
                     if (c.t < tgt.t - delta) { verdict = 1; return false; }
@@ -966,14 +973,14 @@ namespace
     }
 }
 
-void oracle_trace_visible(void* h, const void* nodes128, double scene_scale, const mcrt_ray* rays, const uint32_t* target, size_t n,
-                          uint8_t* verdict, double* t_target)
+void oracle_trace_visible(void* h, const void* nodes128, const uint32_t* refs, double scene_scale, const mcrt_ray* rays, const uint32_t* target,
+                          size_t n, uint8_t* verdict, double* t_target)
 {
     const Scene& s = *static_cast<Scene*>(h);
     for (size_t i = 0; i < n; i++)
     {
         double t = 0.0;
-        verdict[i] = (uint8_t)searchVisible(s, static_cast<const Node4*>(nodes128), makeRay(D3(rays[i].origin), D3(rays[i].direction), s.d.scene_ior), scene_scale, target[i], t);
+        verdict[i] = (uint8_t)searchVisible(s, static_cast<const Node4*>(nodes128), refs, makeRay(D3(rays[i].origin), D3(rays[i].direction), s.d.scene_ior), scene_scale, target[i], t);
         t_target[i] = t;
     }
 }
@@ -984,7 +991,7 @@ namespace
     {
         SearchCheck& c = *g_search_check;
         bool amb = false; uint64_t bt = 0, pt = 0;
-        Isect f = searchFast(s, static_cast<const Node4*>(c.nodes), r, c.scale, amb, bt, pt);
+        Isect f = searchFast(s, static_cast<const Node4*>(c.nodes), c.refs, r, c.scale, amb, bt, pt);
         c.calls++;
         if (amb) { c.flagged++; return; }
         if (f.prim != ref.prim || (ref.prim != 0xFFFFFFFFu && (f.t != ref.t || f.u != ref.u || f.v != ref.v))) c.mismatches++;
@@ -995,10 +1002,10 @@ namespace
 // answered by the order-free search over `nodes128`: counts[0] calls, counts[1] flagged (would be replayed), counts[2] unflagged answers
 // that differ from the reference-order answer (must be 0).
 void oracle_render_rows(void* h, const mcrt_camera* cam, uint32_t y0, uint32_t y1, uint32_t sqrtspp, uint32_t seed, double* out, uint64_t* rays);
-void oracle_render_rows_checked(void* h, const void* nodes128, double scene_scale, const mcrt_camera* cam, uint32_t y0, uint32_t y1,
-                                uint32_t sqrtspp, uint32_t seed, double* out, uint64_t* counts)
+void oracle_render_rows_checked(void* h, const void* nodes128, const uint32_t* refs, double scene_scale, const mcrt_camera* cam, uint32_t y0,
+                                uint32_t y1, uint32_t sqrtspp, uint32_t seed, double* out, uint64_t* counts)
 {
-    SearchCheck c{ nodes128, scene_scale, 0, 0, 0 };
+    SearchCheck c{ nodes128, refs, scene_scale, 0, 0, 0 };
     g_search_check = &c;
     g_cross_fn = crossCheckImpl;
     uint64_t rays = 0;
@@ -1007,8 +1014,8 @@ void oracle_render_rows_checked(void* h, const void* nodes128, double scene_scal
     counts[0] = c.calls; counts[1] = c.flagged; counts[2] = c.mismatches;
 }
 
-void oracle_trace_fast(void* h, const void* nodes128, uint32_t n_nodes, double scene_scale, const mcrt_ray* rays, size_t n, mcrt_hit* hits,
-                       uint8_t* flags, uint64_t* box_tests, uint64_t* prim_tests)
+void oracle_trace_fast(void* h, const void* nodes128, uint32_t n_nodes, const uint32_t* refs, double scene_scale, const mcrt_ray* rays, size_t n,
+                       mcrt_hit* hits, uint8_t* flags, uint64_t* box_tests, uint64_t* prim_tests)
 {
     const Scene& s = *static_cast<Scene*>(h);
     (void)n_nodes;
@@ -1016,7 +1023,7 @@ void oracle_trace_fast(void* h, const void* nodes128, uint32_t n_nodes, double s
     for (size_t i = 0; i < n; i++)
     {
         bool amb = false;
-        Isect is = searchFast(s, static_cast<const Node4*>(nodes128), makeRay(D3(rays[i].origin), D3(rays[i].direction), s.d.scene_ior), scene_scale, amb, bt, pt);
+        Isect is = searchFast(s, static_cast<const Node4*>(nodes128), refs, makeRay(D3(rays[i].origin), D3(rays[i].direction), s.d.scene_ior), scene_scale, amb, bt, pt);
         hits[i].t = is.t; hits[i].u = is.u; hits[i].v = is.v; hits[i].prim = is.prim; hits[i].interpolate = is.interpolate;
         flags[i] = amb ? 1 : 0;
     }
@@ -1039,8 +1046,8 @@ void oracle_trace_peaks(void* h, const mcrt_ray* rays, size_t n, mcrt_hit* hits,
     }
 }
 
-void oracle_trace_fast_peaks(void* h, const void* nodes128, double scene_scale, const mcrt_ray* rays, size_t n, mcrt_hit* hits, uint8_t* flags,
-                             uint32_t* stack_peak)
+void oracle_trace_fast_peaks(void* h, const void* nodes128, const uint32_t* refs, double scene_scale, const mcrt_ray* rays, size_t n, mcrt_hit* hits,
+                             uint8_t* flags, uint32_t* stack_peak)
 {
     const Scene& s = *static_cast<Scene*>(h);
     uint64_t bt = 0, pt = 0;
@@ -1048,7 +1055,8 @@ void oracle_trace_fast_peaks(void* h, const void* nodes128, double scene_scale, 
     {
         bool amb = false;
         size_t peak = 0;
-        Isect is = searchFast(s, static_cast<const Node4*>(nodes128), makeRay(D3(rays[i].origin), D3(rays[i].direction), s.d.scene_ior), scene_scale, amb, bt, pt, &peak);
+        Isect is = searchFast(s, static_cast<const Node4*>(nodes128), refs, makeRay(D3(rays[i].origin), D3(rays[i].direction), s.d.scene_ior), scene_scale, amb, bt, pt,
+                             &peak);
         hits[i].t = is.t; hits[i].u = is.u; hits[i].v = is.v; hits[i].prim = is.prim; hits[i].interpolate = is.interpolate;
         flags[i] = amb ? 1 : 0;
         stack_peak[i] = (uint32_t)peak;
@@ -1090,15 +1098,15 @@ void oracle_wide_stack_bound(void* h, const mcrt_ray* rays, size_t n, double mar
         bound[i] = s.node_first.empty() ? 0u : widePathBound(s, makeRay(D3(rays[i].origin), D3(rays[i].direction), s.d.scene_ior), margin, 0);
 }
 
-void oracle_trace_visible_peaks(void* h, const void* nodes128, double scene_scale, const mcrt_ray* rays, const uint32_t* target, size_t n,
-                                uint8_t* verdict, double* t_target, uint32_t* stack_peak)
+void oracle_trace_visible_peaks(void* h, const void* nodes128, const uint32_t* refs, double scene_scale, const mcrt_ray* rays, const uint32_t* target,
+                                size_t n, uint8_t* verdict, double* t_target, uint32_t* stack_peak)
 {
     const Scene& s = *static_cast<Scene*>(h);
     for (size_t i = 0; i < n; i++)
     {
         double t = 0.0;
         size_t peak = 0;
-        verdict[i] = (uint8_t)searchVisibleOrdered(s, static_cast<const Node4*>(nodes128), makeRay(D3(rays[i].origin), D3(rays[i].direction), s.d.scene_ior),
+        verdict[i] = (uint8_t)searchVisibleOrdered(s, static_cast<const Node4*>(nodes128), refs, makeRay(D3(rays[i].origin), D3(rays[i].direction), s.d.scene_ior),
                                                    scene_scale, target[i], t, peak);
         t_target[i] = t;
         stack_peak[i] = (uint32_t)peak;

@@ -28,16 +28,17 @@ def lib():
         L.oracle_sample_rays.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32, C.c_void_p]
         L.oracle_render_rows.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint64)]
         L.oracle_sample_pixels.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32, C.c_void_p, C.c_void_p]
-        L.oracle_trace_fast.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_double, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
+        L.oracle_trace_fast.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_double, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
                                         C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
-        L.oracle_trace_visible.argtypes = [C.c_void_p, C.c_void_p, C.c_double, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
+        L.oracle_trace_visible.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
         L.oracle_trace_peaks.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
-        L.oracle_trace_fast_peaks.argtypes = [C.c_void_p, C.c_void_p, C.c_double, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p]
-        L.oracle_trace_visible_peaks.argtypes = [C.c_void_p, C.c_void_p, C.c_double, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
-                                                 C.c_void_p]
-        L.oracle_wide_stack_bound.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_double, C.c_void_p]
-        L.oracle_render_rows_checked.argtypes = [C.c_void_p, C.c_void_p, C.c_double, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
+        L.oracle_trace_fast_peaks.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
+                                              C.c_void_p]
+        L.oracle_trace_visible_peaks.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p,
                                                  C.c_void_p, C.c_void_p]
+        L.oracle_wide_stack_bound.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_double, C.c_void_p]
+        L.oracle_render_rows_checked.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32,
+                                                 C.c_uint32, C.c_void_p, C.c_void_p]
         L.oracle_bvh_build.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_void_p), C.c_void_p]
         L.oracle_bvh_free.argtypes = [C.c_void_p]
         L.oracle_octree_build.argtypes = [C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p]
@@ -69,6 +70,15 @@ def lib():
 
 def _p(a):
     return a.ctypes.data_as(C.c_void_p)
+
+
+def _refs(refs):
+    """-> (array to keep alive, pointer): the leaf references' ordered primitives of a tree with spatial splits
+    (mcrt.bvh4_split_host), or a null pointer: leaves index ordered primitives"""
+    if refs is None:
+        return None, None
+    refs = np.ascontiguousarray(refs, dtype=np.uint32)
+    return refs, _p(refs)
 
 
 def sampler_stream(pixel, sample, n_shuffles, seed):
@@ -160,23 +170,29 @@ class PortScene:
         lib().oracle_render_film(self.h, C.addressof(camera.rec), C.addressof(rec), sqrtspp, seed, _p(out))
         return out
 
-    def trace_fast(self, nodes, scene_scale, rays):
-        """The product's order-free search restated on the CPU over `nodes` (mcrt.bvh4_host). -> (hits, ambiguous flags, box tests, primitive tests)"""
+    def trace_fast(self, nodes, scene_scale, rays, refs=None):
+        """The product's order-free search restated on the CPU over `nodes` (mcrt.bvh4_host, or mcrt.bvh4_split_host's nodes with its
+        `refs`: a leaf's (first, count) then index refs, and a repeat of the best primitive is not its competitor). Hits name ordered
+        primitives. -> (hits, ambiguous flags, box tests, primitive tests)"""
         rays = np.ascontiguousarray(rays, dtype=np.float64).reshape(-1, 6)
         nodes = np.ascontiguousarray(nodes)
+        refs, rp = _refs(refs)
         hits = np.zeros(len(rays), dtype=self.pkg.HIT_DTYPE)
         flags = np.zeros(len(rays), dtype=np.uint8)
         bt, pt = C.c_uint64(), C.c_uint64()
-        lib().oracle_trace_fast(self.h, _p(nodes), len(nodes), float(scene_scale), _p(rays), len(rays), _p(hits), _p(flags), C.byref(bt), C.byref(pt))
+        lib().oracle_trace_fast(self.h, _p(nodes), len(nodes), rp, float(scene_scale), _p(rays), len(rays), _p(hits), _p(flags), C.byref(bt),
+                                C.byref(pt))
         return hits, flags.astype(bool), bt.value, pt.value
 
-    def trace_visible(self, nodes, scene_scale, rays, target):
-        """The product's occlusion query restated on the CPU. -> (verdict 0 visible / 1 not / 2 tie-to-replay, t of the target)"""
+    def trace_visible(self, nodes, scene_scale, rays, target, refs=None):
+        """The product's occlusion query restated on the CPU (refs as trace_fast's; every reference of the target, an ordered primitive, is
+        skipped). -> (verdict 0 visible / 1 not / 2 tie-to-replay, t of the target)"""
         rays = np.ascontiguousarray(rays, dtype=np.float64).reshape(-1, 6)
         target = np.ascontiguousarray(target, dtype=np.uint32)
         nodes = np.ascontiguousarray(nodes)
+        refs, rp = _refs(refs)
         verdict = np.zeros(len(rays), dtype=np.uint8); t = np.zeros(len(rays))
-        lib().oracle_trace_visible(self.h, _p(nodes), float(scene_scale), _p(rays), _p(target), len(rays), _p(verdict), _p(t))
+        lib().oracle_trace_visible(self.h, _p(nodes), rp, float(scene_scale), _p(rays), _p(target), len(rays), _p(verdict), _p(t))
         return verdict, t
 
     def trace_peaks(self, rays):
@@ -187,24 +203,26 @@ class PortScene:
         lib().oracle_trace_peaks(self.h, _p(rays), len(rays), _p(hits), _p(peak))
         return hits, peak
 
-    def trace_fast_peaks(self, nodes, scene_scale, rays):
+    def trace_fast_peaks(self, nodes, scene_scale, rays, refs=None):
         """trace_fast() and, per ray, the largest number of entries the order-free search's stack held -> (hits, flags, stack peaks);
         a ray whose peak exceeds the device's stack is flagged"""
         rays = np.ascontiguousarray(rays, dtype=np.float64).reshape(-1, 6)
         nodes = np.ascontiguousarray(nodes)
+        refs, rp = _refs(refs)
         hits = np.zeros(len(rays), dtype=self.pkg.HIT_DTYPE)
         flags = np.zeros(len(rays), dtype=np.uint8)
         peak = np.zeros(len(rays), dtype=np.uint32)
-        lib().oracle_trace_fast_peaks(self.h, _p(nodes), float(scene_scale), _p(rays), len(rays), _p(hits), _p(flags), _p(peak))
+        lib().oracle_trace_fast_peaks(self.h, _p(nodes), rp, float(scene_scale), _p(rays), len(rays), _p(hits), _p(flags), _p(peak))
         return hits, flags.astype(bool), peak
 
-    def trace_visible_peaks(self, nodes, scene_scale, rays, target):
+    def trace_visible_peaks(self, nodes, scene_scale, rays, target, refs=None):
         """The occlusion query in the device's visiting order -> (verdict as trace_visible, t of the target, stack peaks)"""
         rays = np.ascontiguousarray(rays, dtype=np.float64).reshape(-1, 6)
         target = np.ascontiguousarray(target, dtype=np.uint32)
         nodes = np.ascontiguousarray(nodes)
+        refs, rp = _refs(refs)
         verdict = np.zeros(len(rays), dtype=np.uint8); t = np.zeros(len(rays)); peak = np.zeros(len(rays), dtype=np.uint32)
-        lib().oracle_trace_visible_peaks(self.h, _p(nodes), float(scene_scale), _p(rays), _p(target), len(rays), _p(verdict), _p(t), _p(peak))
+        lib().oracle_trace_visible_peaks(self.h, _p(nodes), rp, float(scene_scale), _p(rays), _p(target), len(rays), _p(verdict), _p(t), _p(peak))
         return verdict, t, peak
 
     def wide_stack_bound(self, rays, margin):
@@ -222,12 +240,15 @@ class PortScene:
         lib().oracle_sample_pixels(self.h, C.addressof(camera.rec), _p(pixel), _p(sample), len(pixel), seed, _p(rgb), _p(rays))
         return rgb, rays
 
-    def render_rows_checked(self, nodes, scene_scale, camera, y0, y1, sqrtspp, seed):
-        """render_rows with every Scene::intersect call cross-checked against the order-free search -> (image, calls, flagged, mismatches)"""
+    def render_rows_checked(self, nodes, scene_scale, camera, y0, y1, sqrtspp, seed, refs=None):
+        """render_rows with every Scene::intersect call cross-checked against the order-free search over `nodes` (refs as trace_fast's)
+        -> (image, calls, flagged, mismatches)"""
         nodes = np.ascontiguousarray(nodes)
+        refs, rp = _refs(refs)
         out = np.zeros((y1 - y0, camera.width, 3))
         counts = np.zeros(3, dtype=np.uint64)
-        lib().oracle_render_rows_checked(self.h, _p(nodes), float(scene_scale), C.addressof(camera.rec), y0, y1, sqrtspp, seed, _p(out), _p(counts))
+        lib().oracle_render_rows_checked(self.h, _p(nodes), rp, float(scene_scale), C.addressof(camera.rec), y0, y1, sqrtspp, seed, _p(out),
+                                         _p(counts))
         return out, int(counts[0]), int(counts[1]), int(counts[2])
 
     def render_rows(self, camera, y0, y1, sqrtspp, seed):
