@@ -1461,6 +1461,12 @@ class Progressive:
     expression (the beauty plane's weight is 0)."""
 
     _STATS = ("paths", "extension_rays", "shadow_rays")
+    # the kinds of planes A and B can hold (self._planes): the entry point that renders into them, the checkpoint
+    # identity key that records them and what messages call them
+    _PLANES = {"groups": ("mcrt_render_accumulate_groups_dev", "light_groups", "light groups"),
+               "aovs": ("mcrt_render_accumulate_aovs_dev", "aovs", "light-path AOVs"),
+               "components": ("mcrt_render_accumulate_photon_components_dev", "photon_components", "photon-mapper components"),
+               "lpes": ("mcrt_render_accumulate_lpe_dev", "lpes", "light path expressions")}
 
     def __init__(self, integrator, camera, y_first=0, y_step=1, n_rows=None, tile=16, light_groups=None, aovs=False,
                  components=False, lpes=None):
@@ -1490,9 +1496,13 @@ class Progressive:
         self.rows = camera.height if self.filtered else self.n_rows   # rows of the sums and of the resolved frame
         self.light_groups, self.n_planes = None, 1
         self.lpes, self.lpe_groups = None, None
-        if lpes is not None:
-            if self.filtered:
-                raise McrtError("light path expressions take the box film only")
+        self.aovs, self.components = bool(aovs), bool(components)
+        # with expressions, light_groups only supplies the groups their labels name
+        self._planes = ("lpes" if lpes is not None else "groups" if light_groups is not None else "aovs" if self.aovs
+                        else "components" if self.components else None)
+        if self._planes is not None and self.filtered:
+            raise McrtError(f"{self._PLANES[self._planes][2]} take the box film only")
+        if self._planes == "lpes":
             self.lpes = [str(e) for e in lpes]
             if not self.lpes:
                 raise McrtError("lpes: at least one expression")
@@ -1505,24 +1515,15 @@ class Progressive:
             self._set_lpe_tables()   # refuses a wrong expression or table before anything is allocated
             if integrator.kind == INTEGRATOR_PHOTON:
                 integrator.emit_again()   # the same photons, now carrying their states under this table
-            light_groups = None
-        if light_groups is not None:
-            if self.filtered:
-                raise McrtError("light groups take the box film only")
+        elif self._planes == "groups":
             self.light_groups = np.ascontiguousarray(light_groups, dtype=np.uint32).reshape(-1)
             self.n_planes = (int(self.light_groups.max()) + 1 if self.light_groups.size else 0) + 1
             integrator.set_light_groups(self.light_groups, self.n_planes - 1)   # refuses a wrong table before anything is allocated
-        self.aovs = bool(aovs)
-        if self.aovs:
-            if self.filtered:
-                raise McrtError("light-path AOVs take the box film only")
+        elif self._planes == "aovs":
             self.n_planes = len(AOV_NAMES)
-        self.components = bool(components)
-        if self.components:
-            if self.filtered:
-                raise McrtError("photon-mapper components take the box film only")
+        elif self._planes == "components":
             self.n_planes = len(PHOTON_COMPONENT_NAMES)
-        planes = (self.n_planes,) if self._planar or self.lpes is not None else ()
+        planes = (self.n_planes,) if self._planes is not None else ()
         dev = torch.device("cuda", integrator.device)
         self.rgb = [torch.zeros(planes + (self.rows, camera.width, 3), dtype=torch.float64, device=dev) for _ in range(2)]
         self.wsum = [torch.zeros((self.rows, camera.width), dtype=torch.float64, device=dev) for _ in range(2)] if self.filtered else None
@@ -1543,11 +1544,6 @@ class Progressive:
     def samples(self):
         return self.counts[0] + self.counts[1]
 
-    @property
-    def _planar(self):
-        """A and B hold planes (light groups, AOVs or photon-mapper components) whose sum is the beauty frame's sums."""
-        return self.light_groups is not None or self.aovs or self.components
-
     def _set_lpe_tables(self):
         # without light_groups the integrator's group table is cleared, so that labels L'g' are refused rather than
         # resolved against whatever table it holds, which the checkpoint's identity would not record
@@ -1562,24 +1558,16 @@ class Progressive:
         """Renders samples [self.samples, self.samples + samples) of the active tiles into A (even pass) or B (odd pass)."""
         half = self.passes % 2
         wsum = self.wsum[half].data_ptr() if self.filtered else None
-        if self.light_groups is not None:
-            self.integrator.set_light_groups(self.light_groups, self.n_planes - 1)   # the integrator may serve other renders
-            st = self.integrator.render_accumulate_groups_dev(self.camera, self.rgb[half].data_ptr(), self.n_planes, self.samples,
-                                                              int(samples), self.tile, None if self.active.all() else self.active,
-                                                              self.y_first, self.y_step, self.n_rows)
-        elif self.lpes is not None:
-            self._set_lpe_tables()   # the integrator may serve other renders
-            st = self.integrator.render_accumulate_lpe_dev(self.camera, self.rgb[half].data_ptr(), self.n_planes, self.samples,
-                                                           int(samples), self.tile, None if self.active.all() else self.active,
-                                                           self.y_first, self.y_step, self.n_rows)
-        elif self.aovs:
-            st = self.integrator.render_accumulate_aovs_dev(self.camera, self.rgb[half].data_ptr(), self.samples, int(samples), self.tile,
-                                                            None if self.active.all() else self.active, self.y_first, self.y_step,
-                                                            self.n_rows)
-        elif self.components:
-            st = self.integrator.render_accumulate_components_dev(self.camera, self.rgb[half].data_ptr(), self.samples, int(samples),
-                                                                  self.tile, None if self.active.all() else self.active, self.y_first,
-                                                                  self.y_step, self.n_rows)
+        if self._planes is not None:
+            # the integrator may serve other renders
+            if self._planes == "groups":
+                self.integrator.set_light_groups(self.light_groups, self.n_planes - 1)
+            elif self._planes == "lpes":
+                self._set_lpe_tables()
+            st = self.integrator._render_accumulate_planes(getattr(lib(), self._PLANES[self._planes][0]), self.camera,
+                                                           self.rgb[half].data_ptr(), self.n_planes, self.samples, int(samples),
+                                                           self.tile, None if self.active.all() else self.active, self.y_first,
+                                                           self.y_step, self.n_rows, None)
         elif self.active.all():
             st = self.integrator.render_accumulate_dev(self.camera, self.rgb[half].data_ptr(), wsum, self.samples,
                                                        int(samples), self.y_first, self.y_step, self.n_rows)
@@ -1605,12 +1593,12 @@ class Progressive:
     def _halves(self, weights=None):
         """The sums of halves A and B, [rows, width, 3] each: with planes (light groups, AOVs, components) the combination
         of the planes with weights [n_planes, 3] or [n_planes] (None: every weight 1, the beauty frame's sums)."""
-        if self.lpes is not None:
+        if self._planes == "lpes":
             if weights is None:
                 return [self.rgb[0][-1], self.rgb[1][-1]]   # the beauty plane
             w = light_group_weights(weights, len(self.lpes))
             weights = np.concatenate([w, np.zeros((1, 3))])   # the beauty plane's weight is 0
-        elif not self._planar:
+        elif self._planes is None:
             if weights is not None:
                 raise McrtError("weights need a render with light groups, AOVs, photon-mapper components or light path expressions")
             return self.rgb
@@ -1845,10 +1833,10 @@ class Progressive:
         Known limit: a plane is smoothed with edges the beauty frame shows; an edge only that plane shows (one light
         group's shadow filled by another group) is blurred by as much as the beauty's noise allows (DESIGN.md §6)."""
         import torch
-        if not self._planar and self.lpes is None:
+        if self._planes is None:
             raise McrtError("denoise_planes needs a render with light groups, AOVs, photon-mapper components or light path expressions")
         params = self._denoise_params(iterations, sigma_color, sigma_normal, sigma_depth, sigma_albedo)
-        n = len(self.lpes) if self.lpes is not None else self.n_planes
+        n = len(self.lpes) if self._planes == "lpes" else self.n_planes
         guide = self._halves()
         feats = self._feature_sums(feature_samples, specular_depth)
         out = [torch.empty((n,) + tuple(self.rgb[h].shape[1:]), dtype=torch.float64, device=self.rgb[h].device) for h in (0, 1)]
@@ -1891,13 +1879,13 @@ class Progressive:
                  "scene_digest": np.array(h.hexdigest())}
         if ig.kind == INTEGRATOR_PHOTON:
             ident.update(self._photon_identity())
-        if self.light_groups is not None:
+        if self._planes == "groups":
             ident["light_groups"] = self.light_groups.copy()
-        if self.aovs:
+        elif self._planes == "aovs":
             ident["aovs"] = np.int64(len(AOV_NAMES))
-        if self.components:
+        elif self._planes == "components":
             ident["photon_components"] = np.int64(len(PHOTON_COMPONENT_NAMES))
-        if self.lpes is not None:
+        elif self._planes == "lpes":
             ident["lpes"] = np.array(self.lpes)
             ident["lpe_groups"] = self.lpe_groups.copy() if self.lpe_groups is not None else np.zeros(0, np.int64)
         return ident
@@ -1910,7 +1898,7 @@ class Progressive:
         ph = hashlib.sha256(np.array([k, dv], np.int64).tobytes())
         for which, m in enumerate((caustic, glob)):
             rows = np.ascontiguousarray(np.asarray(m["photons"], np.float32).reshape(-1, 8))
-            if self.light_groups is not None:
+            if self._planes == "groups":
                 # which light emitted a photon decides its plane: each row is the photon and its light index
                 rows = np.concatenate([rows.view(np.uint32), ig.photon_lights(which)[:, None]], axis=1)
             rows = np.ascontiguousarray(rows).view(np.dtype((np.void, rows.shape[1] * 4))).ravel()
@@ -1945,14 +1933,9 @@ class Progressive:
         """Takes over the sums, counts and tile state of checkpoint `data` after checking its identity."""
         import torch
         ident = self._identity()
-        if ("light_groups" in data) != ("light_groups" in ident):
-            raise McrtError(f"checkpoint {path}: light groups differ from this render's; not resuming")
-        if ("aovs" in data) != ("aovs" in ident):
-            raise McrtError(f"checkpoint {path}: light-path AOVs differ from this render's; not resuming")
-        if ("photon_components" in data) != ("photon_components" in ident):
-            raise McrtError(f"checkpoint {path}: photon-mapper components differ from this render's; not resuming")
-        if ("lpes" in data) != ("lpes" in ident):
-            raise McrtError(f"checkpoint {path}: light path expressions differ from this render's; not resuming")
+        for _, key, what in self._PLANES.values():
+            if (key in data) != (key in ident):
+                raise McrtError(f"checkpoint {path}: {what} differ from this render's; not resuming")
         for k, want in ident.items():
             if k not in data or not np.array_equal(data[k], want):
                 raise McrtError(f"checkpoint {path}: {k} differs from this render's; not resuming")
@@ -2079,7 +2062,7 @@ class ProgressivePhotonMapping(Progressive):
 
     def add(self, samples):
         """Emits the map of pass self.passes, gathers with that pass's radii and renders the next samples (Progressive.add)."""
-        if self.lpes is not None:
+        if self._planes == "lpes":
             self._set_lpe_tables()   # the pass's photons carry their states under this render's table
         self._emit(self.passes)
         self.integrator.gather_radius(*self.pass_radii(self.passes))

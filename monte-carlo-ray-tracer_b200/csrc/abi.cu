@@ -997,11 +997,13 @@ namespace
     {
         double* rgb;    // box film [n_pixels][3] in film_index order; filtered film [height*width][3]
         double* wsum;   // filtered film [height*width]; null with the box film
-        uint32_t n_planes = 0;   // box film only: rgb holds this many light-group planes (mcrt_render_accumulate_groups_dev)
-        bool aovs = false;       // ... or planes each deposit site names: the MCRT_AOV_COUNT light-path planes of the
-                                 // path tracer (mcrt_render_accumulate_aovs_dev), the MCRT_PM_COMPONENT_COUNT estimator planes
-                                 // of the photon mapper (mcrt_render_accumulate_photon_components_dev)
-        bool lpe = false;        // ... or one plane per light path expression (mcrt_render_accumulate_lpe_dev)
+        uint32_t n_planes = 0;   // box film only: rgb holds this many planes of the mode below; 0: one plane
+        // FILM_MODE_GROUPS: light-group planes (mcrt_render_accumulate_groups_dev); FILM_MODE_AOV: planes each deposit site
+        // names, the MCRT_AOV_COUNT light-path planes of the path tracer (mcrt_render_accumulate_aovs_dev) or the
+        // MCRT_PM_COMPONENT_COUNT estimator planes of the photon mapper (mcrt_render_accumulate_photon_components_dev);
+        // FILM_MODE_LPE: one plane per light path expression (mcrt_render_accumulate_lpe_dev). Without planes
+        // runWavefront picks FILM_MODE_BOX or FILM_MODE_SPLAT.
+        FilmMode mode = FILM_MODE_BOX;
     };
 
     // The wavefront loop shared by mcrt_render_rows(_dev) and mcrt_sample_rays. Camera work item w is sample
@@ -1065,13 +1067,14 @@ namespace
         double* const film_rgb = accum ? accum->rgb : ctx->d_film;
         double* const film_wsum = accum ? accum->wsum : ctx->d_film_wsum;
         p.film = film_rgb;
+        p.film_mode = filtered ? FILM_MODE_SPLAT : FILM_MODE_BOX;
         if (accum && accum->n_planes)
         {
+            p.film_mode = accum->mode;
             p.group_of_light = ctx->d_group_of_light;
             p.plane_values = film_pixels * 3;
             p.n_planes = accum->n_planes;
-            p.aovs = accum->aovs ? 1u : 0u;
-            if (accum->lpe)
+            if (accum->mode == FILM_MODE_LPE)
             {
                 p.lpe_next = ctx->d_lpe_next;
                 p.lpe_accept = ctx->d_lpe_accept;
@@ -1079,7 +1082,6 @@ namespace
                 p.lpe_symbols = ctx->lpe_symbols;
             }
         }
-        p.filmp.is_default_box = filtered ? 0u : 1u;
         if (filtered)
         {
             p.filmp.rgb = film_rgb; p.filmp.wsum = film_wsum;
@@ -1151,7 +1153,7 @@ namespace
             p.pm.query_capacity = knn_capacity;
             p.pm.gather_r2[0] = ctx->gather_r2[0]; p.pm.gather_r2[1] = ctx->gather_r2[1];
             if (ctx->photon_lights) { p.pm.lights[0] = ctx->built_dev[0].lights; p.pm.lights[1] = ctx->built_dev[1].lights; }
-            if (accum && accum->lpe)
+            if (p.film_mode == FILM_MODE_LPE)
             {
                 p.pm.lpe_states[0] = ctx->built_dev[0].lpe_states; p.pm.lpe_states[1] = ctx->built_dev[1].lpe_states;
                 p.pm.lpe_join = ctx->d_lpe_join;
@@ -2446,10 +2448,8 @@ int mcrt_render_accumulate_lpe_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uin
         ctx->error = name + ": n_planes " + std::to_string(n_planes) + ", the table has " + std::to_string(ctx->lpe_n) + " expressions";
         return MCRT_ERR_INVALID;
     }
-    FilmSums sums{ planes_dev, nullptr, n_planes };
-    sums.lpe = true;
     return accumulatePlanes(ctx, name, camera, y_first, y_step, n_rows, tile, active_tiles, sample_first, sample_count, global_seed,
-                            integrator_kind, precision, sums, stats);
+                            integrator_kind, precision, FilmSums{ planes_dev, nullptr, n_planes, FILM_MODE_LPE }, stats);
 }
 
 int mcrt_render_accumulate_groups_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_t y_first, uint32_t y_step, uint32_t n_rows,
@@ -2473,7 +2473,7 @@ int mcrt_render_accumulate_groups_dev(mcrt_ctx* ctx, const mcrt_camera* camera, 
         return MCRT_ERR_INVALID;
     }
     return accumulatePlanes(ctx, name, camera, y_first, y_step, n_rows, tile, active_tiles, sample_first, sample_count, global_seed,
-                            integrator_kind, precision, FilmSums{ planes_dev, nullptr, n_planes }, stats);
+                            integrator_kind, precision, FilmSums{ planes_dev, nullptr, n_planes, FILM_MODE_GROUPS }, stats);
 }
 
 int mcrt_render_accumulate_aovs_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_t y_first, uint32_t y_step, uint32_t n_rows,
@@ -2495,7 +2495,7 @@ int mcrt_render_accumulate_aovs_dev(mcrt_ctx* ctx, const mcrt_camera* camera, ui
         return MCRT_ERR_INVALID;
     }
     return accumulatePlanes(ctx, name, camera, y_first, y_step, n_rows, tile, active_tiles, sample_first, sample_count, global_seed,
-                            integrator_kind, precision, FilmSums{ planes_dev, nullptr, n_planes, true }, stats);
+                            integrator_kind, precision, FilmSums{ planes_dev, nullptr, n_planes, FILM_MODE_AOV }, stats);
 }
 
 int mcrt_render_accumulate_photon_components_dev(mcrt_ctx* ctx, const mcrt_camera* camera, uint32_t y_first, uint32_t y_step,
@@ -2526,7 +2526,7 @@ int mcrt_render_accumulate_photon_components_dev(mcrt_ctx* ctx, const mcrt_camer
     }
     // the kernels' FILM_MODE_AOV instantiations: each deposit site names its plane, here the MCRT_PM_* estimator planes
     return accumulatePlanes(ctx, name, camera, y_first, y_step, n_rows, tile, active_tiles, sample_first, sample_count, global_seed,
-                            integrator_kind, precision, FilmSums{ planes_dev, nullptr, n_planes, true }, stats);
+                            integrator_kind, precision, FilmSums{ planes_dev, nullptr, n_planes, FILM_MODE_AOV }, stats);
 }
 
 int mcrt_light_groups_combine_dev(mcrt_ctx* ctx, const double* planes_dev, uint32_t n_planes, uint64_t n_values,

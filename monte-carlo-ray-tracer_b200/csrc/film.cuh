@@ -25,7 +25,7 @@ namespace mcrt
         const double* cache;    // Film::filter_cache or null
         double radius, two_inv_radius, inv_dx;
         uint32_t filter, cache_size, width, height;
-        uint32_t is_default_box, _pad;
+        uint32_t _pad[2];
     };
 
     // Filter::MitchellNetravali<B, C>, filter.hpp:15-38 (same constant expressions, evaluated at compile time)

@@ -260,16 +260,16 @@ namespace mcrt
         RaySort sort;           // coherence sort of the path / shadow queues (null order = disabled)
         const uint32_t* sobol_bytes; // byte-sliced Sobol matrices [6][4][256] (makeSobolByteTable)
         EmitParams<R> emit;         // photon emission pass (mcrt_photon_emit) only
-        FilmParams filmp;           // reconstruction filter (default box: only `film` is used)
+        FilmParams filmp;           // reconstruction filter (FILM_MODE_SPLAT only)
         // light-group render (mcrt_render_accumulate_groups_dev): `film` holds n_planes planes of plane_values values each;
         // a contribution of light l goes to plane group_of_light[l], the sky's to plane n_planes - 1. 0: one plane.
-        // AOV render (mcrt_render_accumulate_aovs_dev, aovs = 1): n_planes = MCRT_AOV_COUNT light-path planes instead;
-        // photon-mapper components (mcrt_render_accumulate_photon_components_dev, aovs = 1): MCRT_PM_COMPONENT_COUNT
+        // AOV render (mcrt_render_accumulate_aovs_dev, FILM_MODE_AOV): n_planes = MCRT_AOV_COUNT light-path planes instead;
+        // photon-mapper components (mcrt_render_accumulate_photon_components_dev, FILM_MODE_AOV): MCRT_PM_COMPONENT_COUNT
         const uint32_t* group_of_light;
         size_t plane_values;
         uint32_t n_planes;
-        uint32_t aovs;
-        // LPE render (mcrt_render_accumulate_lpe_dev, lpe_next non-null): n_planes = the expressions; the DFA's
+        uint32_t film_mode;     // FilmMode: which kernel instantiations the launchers pick (host only)
+        // LPE render (mcrt_render_accumulate_lpe_dev, FILM_MODE_LPE): n_planes = the expressions; the DFA's
         // transitions [states][lpe_symbols], accept masks [256] and the symbol of each light (lpe.h)
         const uint8_t* lpe_next;
         const uint32_t* lpe_accept;

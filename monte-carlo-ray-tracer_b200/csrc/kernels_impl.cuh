@@ -1,88 +1,98 @@
 // Shared body of kernels_f64.cu / kernels_f32.cu: defines Launch<MCRT_REAL>.
+#include <type_traits>
+
 #include "launch.h"
 
 namespace mcrt
 {
+    template <int V> using Int = std::integral_constant<int, V>;
+    template <uint32_t V> using Feats = std::integral_constant<uint32_t, V>;
+
+    // f(Int<V>{}) for the first V of Vs equal to v, or for the last V when none is: turns a run-time value into a
+    // template argument, instantiating f for every V listed
+    template <int V, int... Vs, class F> static void pick(int v, F&& f)
+    {
+        if constexpr (sizeof...(Vs) == 0) f(Int<V>{});
+        else if (v == V) f(Int<V>{});
+        else pick<Vs...>(v, f);
+    }
+
+    // f(film mode): the one runWavefront stored, for the launchers of every depositing kernel
+    template <class F> static void withFilmMode(const WaveParams<MCRT_REAL>& p, F&& f)
+    {
+        pick<FILM_MODE_BOX, FILM_MODE_SPLAT, FILM_MODE_GROUPS, FILM_MODE_AOV, FILM_MODE_LPE>((int)p.film_mode, f);
+    }
+
+    // f(film mode, shade features) of the kernels that shade. Scenes whose materials use no Oren-Nayar / GGX / conductor
+    // Fresnel run the instantiation without that code; the filtered film, the rare configuration, has one generic
+    // instantiation.
+    template <class F> static void withFilm(const WaveParams<MCRT_REAL>& p, F&& f)
+    {
+        const bool lite = (p.scene.material_flags_any & ~SHADE_FEATS_LITE) == 0;
+        withFilmMode(p, [&](auto film) {
+            if constexpr (film == FILM_MODE_SPLAT) f(film, Feats<SHADE_FEATS_ALL>{});
+            else if (lite) f(film, Feats<SHADE_FEATS_LITE>{});
+            else f(film, Feats<SHADE_FEATS_ALL>{});
+        });
+    }
+
+    // f(prims, traversal, dynamic shared bytes) of k_extend / k_shadow: triangle-only scenes (every OBJ scene) run the
+    // traversal without sphere / quadric code; parity mode takes the order-free BVH4 search whenever the scene has that
+    // BVH (2: with dynamic fetch), fast mode always the plain traversal (0)
+    template <class F> static void withTraversal(const WaveParams<MCRT_REAL>& p, F&& f)
+    {
+        const auto prims = [&](auto fast) {
+            const size_t smem = fast ? fastStackSharedBytes(256) : 0;
+            pick<PRIMS_TRI, PRIMS_TRI_SPHERE, PRIMS_ALL>((int)p.scene.prims_class, [&](auto pr) { f(pr, fast, smem); });
+        };
+        if constexpr (Mode<MCRT_REAL>::parity)
+        {
+            if (p.scene.bvh4 && p.scene.dynamic_fetch) return prims(Int<2>{});
+            if (p.scene.bvh4) return prims(Int<1>{});
+        }
+        prims(Int<0>{});
+    }
+
     template <> void Launch<MCRT_REAL>::generate(const WaveParams<MCRT_REAL>& p, int next, int grid, cudaStream_t s)
     {
+        const bool filtered = p.film_mode == FILM_MODE_SPLAT;
         if (p.pixel_list)
         {
-            if (p.filmp.is_default_box) k_generate<MCRT_REAL, false, true><<<grid, 256, 0, s>>>(p, next);
-            else k_generate<MCRT_REAL, true, true><<<grid, 256, 0, s>>>(p, next);
+            if (filtered) k_generate<MCRT_REAL, true, true><<<grid, 256, 0, s>>>(p, next);
+            else k_generate<MCRT_REAL, false, true><<<grid, 256, 0, s>>>(p, next);
             return;
         }
-        if (p.filmp.is_default_box) k_generate<MCRT_REAL, false, false><<<grid, 256, 0, s>>>(p, next);
-        else k_generate<MCRT_REAL, true, false><<<grid, 256, 0, s>>>(p, next);
+        if (filtered) k_generate<MCRT_REAL, true, false><<<grid, 256, 0, s>>>(p, next);
+        else k_generate<MCRT_REAL, false, false><<<grid, 256, 0, s>>>(p, next);
     }
     template <> void Launch<MCRT_REAL>::extend(const WaveParams<MCRT_REAL>& p, int cur, int grid, cudaStream_t s)
     {
-        // triangle-only scenes (every OBJ scene) run the traversal without sphere / quadric code
-        if constexpr (Mode<MCRT_REAL>::parity)
-        {
-            if (p.scene.bvh4 && p.scene.dynamic_fetch)
-            {
-                if (p.scene.prims_class == PRIMS_TRI) k_extend<MCRT_REAL, PRIMS_TRI, 2><<<grid, 256, fastStackSharedBytes(256), s>>>(p, cur);
-                else if (p.scene.prims_class == PRIMS_TRI_SPHERE) k_extend<MCRT_REAL, PRIMS_TRI_SPHERE, 2><<<grid, 256, fastStackSharedBytes(256), s>>>(p, cur);
-                else k_extend<MCRT_REAL, PRIMS_ALL, 2><<<grid, 256, fastStackSharedBytes(256), s>>>(p, cur);
-                return;
-            }
-            if (p.scene.bvh4)
-            {
-                if (p.scene.prims_class == PRIMS_TRI) k_extend<MCRT_REAL, PRIMS_TRI, 1><<<grid, 256, fastStackSharedBytes(256), s>>>(p, cur);
-                else if (p.scene.prims_class == PRIMS_TRI_SPHERE) k_extend<MCRT_REAL, PRIMS_TRI_SPHERE, 1><<<grid, 256, fastStackSharedBytes(256), s>>>(p, cur);
-                else k_extend<MCRT_REAL, PRIMS_ALL, 1><<<grid, 256, fastStackSharedBytes(256), s>>>(p, cur);
-                return;
-            }
-        }
-        if (p.scene.prims_class == PRIMS_TRI) k_extend<MCRT_REAL, PRIMS_TRI, 0><<<grid, 256, 0, s>>>(p, cur);
-        else if (p.scene.prims_class == PRIMS_TRI_SPHERE) k_extend<MCRT_REAL, PRIMS_TRI_SPHERE, 0><<<grid, 256, 0, s>>>(p, cur);
-        else k_extend<MCRT_REAL, PRIMS_ALL, 0><<<grid, 256, 0, s>>>(p, cur);
+        withTraversal(p, [&](auto prims, auto fast, size_t smem) { k_extend<MCRT_REAL, prims, fast><<<grid, 256, smem, s>>>(p, cur); });
+    }
+    // KIND 0: PathTracer loop body, 1: PhotonMapper loop body
+    template <int KIND> static void launchShade(const WaveParams<MCRT_REAL>& p, int cur, int grid, cudaStream_t s)
+    {
+        withFilm(p, [&](auto film, auto feats) { k_shade<MCRT_REAL, KIND, film, feats><<<grid * 2, 128, 0, s>>>(p, cur); });
     }
     template <> void Launch<MCRT_REAL>::shade(const WaveParams<MCRT_REAL>& p, int cur, int grid, cudaStream_t s)
     {
-        // scenes whose materials use no Oren-Nayar / GGX / conductor Fresnel run the instantiation without that code
-        const bool lite = (p.scene.material_flags_any & ~SHADE_FEATS_LITE) == 0;
-        if (!p.filmp.is_default_box) k_shade<MCRT_REAL, 0, FILM_MODE_SPLAT, SHADE_FEATS_ALL><<<grid * 2, 128, 0, s>>>(p, cur);
-        else if (p.n_planes && p.lpe_next)
-        {
-            if (lite) k_shade<MCRT_REAL, 0, FILM_MODE_LPE, SHADE_FEATS_LITE><<<grid * 2, 128, 0, s>>>(p, cur);
-            else k_shade<MCRT_REAL, 0, FILM_MODE_LPE, SHADE_FEATS_ALL><<<grid * 2, 128, 0, s>>>(p, cur);
-        }
-        else if (p.n_planes && p.aovs)
-        {
-            if (lite) k_shade<MCRT_REAL, 0, FILM_MODE_AOV, SHADE_FEATS_LITE><<<grid * 2, 128, 0, s>>>(p, cur);
-            else k_shade<MCRT_REAL, 0, FILM_MODE_AOV, SHADE_FEATS_ALL><<<grid * 2, 128, 0, s>>>(p, cur);
-        }
-        else if (p.n_planes)
-        {
-            if (lite) k_shade<MCRT_REAL, 0, FILM_MODE_GROUPS, SHADE_FEATS_LITE><<<grid * 2, 128, 0, s>>>(p, cur);
-            else k_shade<MCRT_REAL, 0, FILM_MODE_GROUPS, SHADE_FEATS_ALL><<<grid * 2, 128, 0, s>>>(p, cur);
-        }
-        else if (lite) k_shade<MCRT_REAL, 0, FILM_MODE_BOX, SHADE_FEATS_LITE><<<grid * 2, 128, 0, s>>>(p, cur);
-        else k_shade<MCRT_REAL, 0, FILM_MODE_BOX, SHADE_FEATS_ALL><<<grid * 2, 128, 0, s>>>(p, cur);
+        launchShade<0>(p, cur, grid, s);
     }
     template <> void Launch<MCRT_REAL>::shadePhoton(const WaveParams<MCRT_REAL>& p, int cur, int grid, cudaStream_t s)
     {
-        const bool lite = (p.scene.material_flags_any & ~SHADE_FEATS_LITE) == 0;
-        if (!p.filmp.is_default_box) k_shade<MCRT_REAL, 1, FILM_MODE_SPLAT, SHADE_FEATS_ALL><<<grid * 2, 128, 0, s>>>(p, cur);
-        else if (p.n_planes && p.lpe_next)
+        launchShade<1>(p, cur, grid, s);
+    }
+    template <int SLOTS, int FILM, uint32_t FEATS>
+    static void launchKnn(const WaveParams<MCRT_REAL>& p, dim3 g, dim3 b, size_t smem, cudaStream_t s)
+    {
+        // k > 672 needs more than the default 48 KB of dynamic shared memory (knnSharedBytes)
+        static bool attr_set = false;
+        if (!attr_set)
         {
-            if (lite) k_shade<MCRT_REAL, 1, FILM_MODE_LPE, SHADE_FEATS_LITE><<<grid * 2, 128, 0, s>>>(p, cur);
-            else k_shade<MCRT_REAL, 1, FILM_MODE_LPE, SHADE_FEATS_ALL><<<grid * 2, 128, 0, s>>>(p, cur);
+            cudaFuncSetAttribute(k_knn<MCRT_REAL, SLOTS, FILM, FEATS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)knnSharedBytes(1024));
+            attr_set = true;
         }
-        else if (p.n_planes && p.aovs)
-        {
-            // photon-mapper components: FILM_MODE_AOV deposits into the plane each site names (MCRT_PM_*)
-            if (lite) k_shade<MCRT_REAL, 1, FILM_MODE_AOV, SHADE_FEATS_LITE><<<grid * 2, 128, 0, s>>>(p, cur);
-            else k_shade<MCRT_REAL, 1, FILM_MODE_AOV, SHADE_FEATS_ALL><<<grid * 2, 128, 0, s>>>(p, cur);
-        }
-        else if (p.n_planes)
-        {
-            if (lite) k_shade<MCRT_REAL, 1, FILM_MODE_GROUPS, SHADE_FEATS_LITE><<<grid * 2, 128, 0, s>>>(p, cur);
-            else k_shade<MCRT_REAL, 1, FILM_MODE_GROUPS, SHADE_FEATS_ALL><<<grid * 2, 128, 0, s>>>(p, cur);
-        }
-        else if (lite) k_shade<MCRT_REAL, 1, FILM_MODE_BOX, SHADE_FEATS_LITE><<<grid * 2, 128, 0, s>>>(p, cur);
-        else k_shade<MCRT_REAL, 1, FILM_MODE_BOX, SHADE_FEATS_ALL><<<grid * 2, 128, 0, s>>>(p, cur);
+        k_knn<MCRT_REAL, SLOTS, FILM, FEATS><<<g, b, smem, s>>>(p);
     }
     template <> void Launch<MCRT_REAL>::knn(const WaveParams<MCRT_REAL>& p, int grid, cudaStream_t s)
     {
@@ -90,107 +100,31 @@ namespace mcrt
         if (p.pm.gather_r2[0] > 0.0)
         {
             // fixed-radius gather (mcrt_photon_gather_radius) in place of the k-NN estimate
-            const bool lite = (p.scene.material_flags_any & ~SHADE_FEATS_LITE) == 0;
-            if (!p.filmp.is_default_box) k_gather<MCRT_REAL, FILM_MODE_SPLAT, SHADE_FEATS_ALL><<<g, b, 0, s>>>(p);
-            else if (p.n_planes && p.lpe_next)
-            {
-                if (lite) k_gather<MCRT_REAL, FILM_MODE_LPE, SHADE_FEATS_LITE><<<g, b, 0, s>>>(p);
-                else k_gather<MCRT_REAL, FILM_MODE_LPE, SHADE_FEATS_ALL><<<g, b, 0, s>>>(p);
-            }
-            else if (p.n_planes && p.aovs)
-            {
-                if (lite) k_gather<MCRT_REAL, FILM_MODE_AOV, SHADE_FEATS_LITE><<<g, b, 0, s>>>(p);
-                else k_gather<MCRT_REAL, FILM_MODE_AOV, SHADE_FEATS_ALL><<<g, b, 0, s>>>(p);
-            }
-            else if (p.n_planes)
-            {
-                if (lite) k_gather<MCRT_REAL, FILM_MODE_GROUPS, SHADE_FEATS_LITE><<<g, b, 0, s>>>(p);
-                else k_gather<MCRT_REAL, FILM_MODE_GROUPS, SHADE_FEATS_ALL><<<g, b, 0, s>>>(p);
-            }
-            else if (lite) k_gather<MCRT_REAL, FILM_MODE_BOX, SHADE_FEATS_LITE><<<g, b, 0, s>>>(p);
-            else k_gather<MCRT_REAL, FILM_MODE_BOX, SHADE_FEATS_ALL><<<g, b, 0, s>>>(p);
+            withFilm(p, [&](auto film, auto feats) { k_gather<MCRT_REAL, film, feats><<<g, b, 0, s>>>(p); });
             return;
         }
         const size_t smem = knnSharedBytes(p.pm.k_nearest);
         // the photon maps hold at least k photons in every render that matters; if a map is smaller the
         // search clamps k itself and the register slots are simply not all used
-        if (!p.filmp.is_default_box)
-        {
-            // filtered film: the rare configuration, one generic instantiation
-            static bool attr_set = false;
-            if (!attr_set) { cudaFuncSetAttribute(k_knn<MCRT_REAL, 0, FILM_MODE_SPLAT, SHADE_FEATS_ALL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)knnSharedBytes(1024)); attr_set = true; }
-            k_knn<MCRT_REAL, 0, FILM_MODE_SPLAT, SHADE_FEATS_ALL><<<g, b, smem, s>>>(p);
-            return;
-        }
-        const bool lite = (p.scene.material_flags_any & ~SHADE_FEATS_LITE) == 0;
-        // film mode of the box film: one plane, light-group planes, the photon mapper's component planes (FILM_MODE_AOV)
-        // or LPE planes
-        const int film_mode = !p.n_planes ? FILM_MODE_BOX : (p.lpe_next ? FILM_MODE_LPE : (p.aovs ? FILM_MODE_AOV : FILM_MODE_GROUPS));
-        const int slots = knnSlotsFor(p.pm.k_nearest);
-        // k > 672 needs more than the default 48 KB of dynamic shared memory (knnSharedBytes)
-        #define MCRT_KNN_LAUNCH2(SL, FM, FE) \
-            do { static bool attr_set = false; \
-                 if (!attr_set) { cudaFuncSetAttribute(k_knn<MCRT_REAL, SL, FM, FE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)knnSharedBytes(1024)); attr_set = true; } \
-                 k_knn<MCRT_REAL, SL, FM, FE><<<g, b, smem, s>>>(p); } while (0)
-        #define MCRT_KNN_LAUNCH1(SL, FE) \
-            do { if (film_mode == FILM_MODE_GROUPS) MCRT_KNN_LAUNCH2(SL, FILM_MODE_GROUPS, FE); \
-                 else if (film_mode == FILM_MODE_AOV) MCRT_KNN_LAUNCH2(SL, FILM_MODE_AOV, FE); \
-                 else if (film_mode == FILM_MODE_LPE) MCRT_KNN_LAUNCH2(SL, FILM_MODE_LPE, FE); \
-                 else MCRT_KNN_LAUNCH2(SL, FILM_MODE_BOX, FE); } while (0)
-        #define MCRT_KNN_LAUNCH(SL) \
-            do { if (lite) MCRT_KNN_LAUNCH1(SL, SHADE_FEATS_LITE); else MCRT_KNN_LAUNCH1(SL, SHADE_FEATS_ALL); } while (0)
-        switch (slots)
-        {
-            case 1: MCRT_KNN_LAUNCH(1); break;
-            case 2: MCRT_KNN_LAUNCH(2); break;
-            case 4: MCRT_KNN_LAUNCH(4); break;
-            case 8: MCRT_KNN_LAUNCH(8); break;
-            default: MCRT_KNN_LAUNCH(0); break;
-        }
-        #undef MCRT_KNN_LAUNCH
-        #undef MCRT_KNN_LAUNCH1
-        #undef MCRT_KNN_LAUNCH2
-    }
-    // k_shadow of the box film (one plane, light-group planes, AOV / photon-mapper component planes, or LPE planes) with the
-    // scene-specialised traversal
-    template <int FILM> static void launchShadowBox(const WaveParams<MCRT_REAL>& p, int grid, cudaStream_t s)
-    {
-        if constexpr (Mode<MCRT_REAL>::parity)
-        {
-            if (p.scene.bvh4 && p.scene.dynamic_fetch)
-            {
-                if (p.scene.prims_class == PRIMS_TRI) k_shadow<MCRT_REAL, FILM, PRIMS_TRI, 2><<<grid, 256, fastStackSharedBytes(256), s>>>(p);
-                else if (p.scene.prims_class == PRIMS_TRI_SPHERE) k_shadow<MCRT_REAL, FILM, PRIMS_TRI_SPHERE, 2><<<grid, 256, fastStackSharedBytes(256), s>>>(p);
-                else k_shadow<MCRT_REAL, FILM, PRIMS_ALL, 2><<<grid, 256, fastStackSharedBytes(256), s>>>(p);
-                return;
-            }
-            if (p.scene.bvh4)
-            {
-                if (p.scene.prims_class == PRIMS_TRI) k_shadow<MCRT_REAL, FILM, PRIMS_TRI, 1><<<grid, 256, fastStackSharedBytes(256), s>>>(p);
-                else if (p.scene.prims_class == PRIMS_TRI_SPHERE) k_shadow<MCRT_REAL, FILM, PRIMS_TRI_SPHERE, 1><<<grid, 256, fastStackSharedBytes(256), s>>>(p);
-                else k_shadow<MCRT_REAL, FILM, PRIMS_ALL, 1><<<grid, 256, fastStackSharedBytes(256), s>>>(p);
-                return;
-            }
-        }
-        if (p.scene.prims_class == PRIMS_TRI) k_shadow<MCRT_REAL, FILM, PRIMS_TRI, 0><<<grid, 256, 0, s>>>(p);
-        else if (p.scene.prims_class == PRIMS_TRI_SPHERE) k_shadow<MCRT_REAL, FILM, PRIMS_TRI_SPHERE, 0><<<grid, 256, 0, s>>>(p);
-        else k_shadow<MCRT_REAL, FILM, PRIMS_ALL, 0><<<grid, 256, 0, s>>>(p);
+        withFilm(p, [&](auto film, auto feats) {
+            if constexpr (film == FILM_MODE_SPLAT) launchKnn<0, film, feats>(p, g, b, smem, s);   // the generic instantiation only
+            else pick<1, 2, 4, 8, 0>(knnSlotsFor(p.pm.k_nearest), [&](auto slots) { launchKnn<slots, film, feats>(p, g, b, smem, s); });
+        });
     }
     template <> void Launch<MCRT_REAL>::shadow(const WaveParams<MCRT_REAL>& p, int grid, cudaStream_t s)
     {
-        if (!p.filmp.is_default_box)
-        {
-            // filtered film: the rare configuration, the generic traversal only
-            if constexpr (Mode<MCRT_REAL>::parity)
+        withFilmMode(p, [&](auto film) {
+            if constexpr (film == FILM_MODE_SPLAT)
             {
-                if (p.scene.bvh4) { k_shadow<MCRT_REAL, FILM_MODE_SPLAT, PRIMS_ALL, 1><<<grid, 256, fastStackSharedBytes(256), s>>>(p); return; }
+                // filtered film: the rare configuration, the generic traversal only
+                if constexpr (Mode<MCRT_REAL>::parity)
+                {
+                    if (p.scene.bvh4) { k_shadow<MCRT_REAL, film, PRIMS_ALL, 1><<<grid, 256, fastStackSharedBytes(256), s>>>(p); return; }
+                }
+                k_shadow<MCRT_REAL, film, PRIMS_ALL, 0><<<grid, 256, 0, s>>>(p);
             }
-            k_shadow<MCRT_REAL, FILM_MODE_SPLAT, PRIMS_ALL, 0><<<grid, 256, 0, s>>>(p);
-        }
-        else if (p.n_planes && p.lpe_next) launchShadowBox<FILM_MODE_LPE>(p, grid, s);
-        else if (p.n_planes && p.aovs) launchShadowBox<FILM_MODE_AOV>(p, grid, s);
-        else if (p.n_planes) launchShadowBox<FILM_MODE_GROUPS>(p, grid, s);
-        else launchShadowBox<FILM_MODE_BOX>(p, grid, s);
+            else withTraversal(p, [&](auto prims, auto fast, size_t smem) { k_shadow<MCRT_REAL, film, prims, fast><<<grid, 256, smem, s>>>(p); });
+        });
     }
     template <> void Launch<MCRT_REAL>::shadeKey(const WaveParams<MCRT_REAL>& p, int grid, cudaStream_t s)
     {
